@@ -14,7 +14,7 @@ A "step" is one pass of ViDAR's two hot paths over one synthetic sample
        dvxlr autograd layer (`DifferentiableVoxelRendering`) forward + backward on them.
 metric = rays/sec = 30000 rays / step time (whole job); ms_per_step is the same thing as time.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 For N>1 launch under torchrun (one rank per GPU); the (camera, query) rows and the rays are
 sharded over ranks (strong scaling: total work fixed); per step one all-reduce of the BEV grid
 (the local scatter-add of SpatialCrossAttention's rows, 41 MB) and one of each grad_sigma.
@@ -77,7 +77,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def msda_algorithmic_bytes(rows, cams_touched):
@@ -277,10 +277,12 @@ def run_ours(args, light=False):
             # row-sharded in / out (the module's consumers in the encoder -- LayerNorm, FFN -- are row-wise): only the
             # 2.56 MB occupancy / feature / prob maps cross NVLink, never the 41 MB grid
             emb = embed.view(-1, EMBED)[lr0:lr1].detach().requires_grad_(True)
-            latent.forward_rows(emb, 1, GRID[1], GRID[2]).backward(grad_embed.view(-1, EMBED)[lr0:lr1])
+            lat_out = latent.forward_rows(emb, 1, GRID[1], GRID[2])
+            lat_out.backward(grad_embed.view(-1, EMBED)[lr0:lr1])
         else:
             emb = embed.detach().requires_grad_(True)
-            latent(emb).backward(grad_embed)
+            lat_out = latent(emb)
+            lat_out.backward(grad_embed)
         if record:
             e[3].record()
         sg = sigma[0].detach().requires_grad_(True)
@@ -304,7 +306,10 @@ def run_ours(args, light=False):
         if record:
             e[5].record()
             marks.append(e)
-        return bev.detach(), leaves, pred, grad_sigma, emb.grad, ce_grad, dv_grad
+        # the forward outputs a caller receives besides the gradients (for --dump-outputs)
+        fwd = {"latent_out": lat_out.detach(), "ray_ce": ce.detach(), "ray_ce_valid": valid, "render_gt": gt,
+               "dvxlr_layer_pred": dpred.detach()}
+        return bev.detach(), leaves, pred, grad_sigma, emb.grad, ce_grad, dv_grad, fwd
 
     def sync():
         torch.cuda.synchronize()
@@ -356,6 +361,8 @@ def run_ours(args, light=False):
     sync()
     sampler.mark_end()
     launches = _lib.launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     clocks = sampler.stop() if rank == 0 else None
     total_ms = t0.elapsed_time(t1)
     if world > 1:
@@ -515,14 +522,9 @@ def run_ours(args, light=False):
     dom_bytes = bwd_b if dom == "msda_bwd" else fwd_b
     n_launch = len(groups)
     achieved = dom_bytes / (parts[dom] * 1e-3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp) and world == 1:
-        with open(tp) as fh:
-            traffic = json.load(fh).get(dom)
     roofline = {"bound": "hbm", "kernel": "msda_backward_kernel<8>" if dom == "msda_bwd" else "msda_forward_kernel<8>",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": dom_bytes / n_launch,
                 "avg_launch_ms": parts[dom] / n_launch,
                 "note": "duration = CUDA events around the op in the timed region (incl. grad_value "
@@ -542,16 +544,37 @@ def run_ours(args, light=False):
     _finish(world)
 
 
+def dump_outputs(out_dir, last, sample=1 << 20):
+    """--dump-outputs: what the last timed step returned -- every stage's forward outputs and the gradients of
+    its inputs -- one DIR/<name>.npy (float32) per array.  An array of more than `sample` elements is stored as a
+    fixed seeded sample of about `sample` of its elements (the same positions in every run), which keeps the
+    directory under 64 MB; the inputs are seeded, so two builds of the project can be compared output for output."""
+    bev, leaves, pred, grad_sigma, gemb, ce_grad, dv_grad, fwd = last
+    arrays = {"bev_grid": bev, "render_pred": pred, "render_grad_sigma": grad_sigma, "latent_grad_embed": gemb,
+              "ray_ce_grad_sigma": ce_grad, "dvxlr_layer_grad_sigma": dv_grad, **fwd}
+    for i, (v, loc, aw) in enumerate(leaves):
+        sfx = "" if len(leaves) == 1 else f"_{i}"
+        arrays.update({f"msda_grad_value{sfx}": v.grad, f"msda_grad_sampling_loc{sfx}": loc.grad,
+                       f"msda_grad_attn_weight{sfx}": aw.grad})
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() > sample:
+            pos = np.unique(np.random.default_rng(0).integers(0, flat.numel(), sample))
+            flat = flat[torch.from_numpy(pos).to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.cpu().numpy())
+
+
 def check_sharded(dev, rank, world, grp, last, groups, msda_stage, grad_bev, latent, embed, grad_embed, sigma, origin,
                   rays_np, shapes, lsi, cam_groups):
-    """Sharded == single GPU, checked on the lease the scaling run gets (SCALE_rNN.json carries the result).
+    """Sharded == single GPU, checked inside every multi-GPU run (the line's `sharded_check`).
     The last timed step's results -- BEV grid, grad_value / grad_loc / grad_attn (summed over ranks into full
     tensors), both ray stages' grad_sigma, LatentRendering's input gradient -- against an UNSHARDED recompute of
     the same step on every rank (plan for world 1, all rays, no process group).  -> {name: max|a-b| / max|b|}"""
     import torch.distributed as dist
 
     from vidar_b200 import ray_head, render, sca
-    bev, leaves, pred, grad_sigma, gemb, ce_grad, dv_grad = last
+    bev, leaves, pred, grad_sigma, gemb, ce_grad, dv_grad, _ = last
     full = sca_like_inputs(dev)
     ref_groups = [dict(plan=sca.unit_plan(1, 0, NUM_CAMS)[0], value=full["value"], loc=full["loc"], attn=full["attn"])]
     rbev, rleaves = msda_stage(ref_groups, None, 1)
@@ -867,7 +890,7 @@ def run_pretrain(args):
 def _finish(world):
     """End of a multi-rank run.  With a captured CUDA graph that contains NCCL kernels, tearing the process group
     down (or the interpreter's exit handlers) was seen to hang for minutes AFTER the JSON line was out (8 and 4
-    ranks, gpurun r2h): every result is already written, so the ranks leave without running destructors."""
+    ranks): every result is already written, so the ranks leave without running destructors."""
     if world > 1:
         import torch.distributed as dist
         # nobody leaves before rank 0 has written the line (a rank that disappears early could be noticed by the
@@ -901,6 +924,9 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float32; arrays "
+                         "larger than 2^20 elements as a fixed seeded sample)")
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="launch the timed steps eagerly instead of replaying a CUDA graph")
     ap.add_argument("--row-sharded", dest="row_sharded", action="store_true",
                     help="--workload pretrain, N > 1: TSA / norms / FFN of the encoder on the rank's BEV rows (EncoderLayer.forward_rows)")
@@ -909,6 +935,8 @@ def main():
                          "(--impl reference there = the same graph with the reference's eager torch formulas for MSDA / LatentRendering, on the GPU)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
+    if args.dump_outputs and (args.workload != "hotpath" or args.impl != "ours"):
+        ap.error("--dump-outputs applies to the hotpath workload with --impl ours")
     if args.workload == "pretrain":
         run_pretrain(args)
     elif args.impl == "reference":

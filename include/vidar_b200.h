@@ -1,5 +1,5 @@
 /*
- * vidar_b200.h -- C ABI of libvidar_b200.so: the B200 (sm_100a) kernels that sit
+ * vidar_b200.h -- C ABI of libvidar_b200.so: the H100 (sm_90a) kernels that sit
  * under ViDAR's two hot-path operator boundaries.
  *
  *   (i)  multi-scale deformable attention   (mmcv `_ext.ms_deform_attn_{forward,backward}`,
@@ -41,7 +41,7 @@ enum {
 
 /* Message of the last error raised on this thread ("" if none). */
 const char* vidar_last_error(void);
-/* Library / build identification, e.g. "vidar_b200 0.1 sm_100a". */
+/* Library / build identification, e.g. "vidar_b200 0.1 sm_90a". */
 const char* vidar_version(void);
 /* Number of kernels this library has launched since load (all threads).  bench.py
  * reports the delta across the timed region as `gpu_launches`. */
@@ -147,9 +147,9 @@ int vidar_msda_sca_rows_backward(const float* value, const int64_t* spatial_shap
 
 /* (i-c) The Linear layer in front of the sampling (SURVEY.md 8f-4): value_proj of MSDeformableAttention3D
  * (spatial_cross_attention.py:333) over the flattened camera features (modules/transformer.py:159-179),
- * y [M, N] = x [M, K] w[N, K]^T + bias[N], fp32 in / out.  tcgen05 tensor cores with a 3xTF32 split (fp32
- * accuracy, ~1e-6 relative: a plain TF32 GEMM would miss the 1e-4 parity bar), operands by TMA, accumulator in
- * TMEM.  K % 32 == 0, N % 128 == 0; bias may be NULL.  w_split: 2*N*K floats of caller-owned scratch. */
+ * y [M, N] = x [M, K] w[N, K]^T + bias[N], fp32 in / out.  wgmma tensor cores with a 3xTF32 split (fp32
+ * accuracy, ~1e-6 relative: a plain TF32 GEMM would miss the 1e-4 parity bar), operands by TMA, accumulators in
+ * registers.  K % 32 == 0, N % 128 == 0; bias may be NULL.  w_split: 2*N*K floats of caller-owned scratch. */
 int vidar_linear_tf32x3(const float* x, const float* w, const float* bias, float* y, float* w_split,
                         int M, int N, int K, void* stream);
 

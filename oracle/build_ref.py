@@ -1,4 +1,4 @@
-"""Compile the reference's OWN ray-caster kernels for sm_100a into oracle/_ref/ (git-ignored).
+"""Compile the reference's OWN ray-caster kernels for sm_90a into oracle/_ref/ (git-ignored).
 
 TEST INFRASTRUCTURE.  third_lib/dvr and third_lib/dvxlr are torch C++/CUDA extensions made
 of two files each; they are compiled from where they lie under /root/reference by this
@@ -27,10 +27,10 @@ TARGETS = {
     "ref_dvxlr": ("dvxlr", ["dvxlr.cpp", "dvxlr.cu"]),
     "ref_dvxlr_v2": ("dvxlr", ["dvxlr_v2.cpp", "dvxlr_v2.cu"]),
 }
-# dvr.cu launches 1024-thread blocks (dvr.cu:345,651); built for sm_100a its render kernels
-# need > 64 registers/thread, and 1024 x 65+ exceeds the 64K-register file: every launch
-# fails with cudaErrorLaunchOutOfResources on a B200 (observed).  A register cap is the
-# build flag that makes the unmodified kernel launchable; it changes no arithmetic.
+# dvr.cu launches 1024-thread blocks (dvr.cu:345,651); uncapped, its render kernels need
+# > 64 registers/thread, and 1024 x 65+ exceeds the 64K-register file: every launch fails
+# with cudaErrorLaunchOutOfResources.  A register cap is the build flag that makes the
+# unmodified kernel launchable; it changes no arithmetic.
 EXTRA_FLAGS = {"ref_dvr": ["-maxrregcount=64"]}
 
 
@@ -68,11 +68,33 @@ def so_path(name):
     return os.path.join(OUT, name + ".so")
 
 
+def _cuda_flags(name):
+    return ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo"] + EXTRA_FLAGS.get(name, [])
+
+
+def _stamp_path(name):
+    return so_path(name) + ".flags"
+
+
+def is_current(name):
+    """The .so exists and, for the CUDA targets, was built with today's flags (architecture included): a
+    library left from a build for another GPU is rebuilt rather than loaded."""
+    if not os.path.exists(so_path(name)):
+        return False
+    if name not in TARGETS:
+        return True
+    try:
+        with open(_stamp_path(name)) as fh:
+            return fh.read().strip() == " ".join(_cuda_flags(name))
+    except OSError:
+        return False
+
+
 def _build_one(name, force=False):
     sub, files = TARGETS[name]
-    if os.path.exists(so_path(name)) and not force:
+    if is_current(name) and not force:
         return so_path(name)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     os.environ.setdefault("MAX_JOBS", "2")
     from torch.utils import cpp_extension
     os.makedirs(OUT, exist_ok=True)
@@ -89,10 +111,11 @@ def _build_one(name, force=False):
             srcs.append(dst)
         cpp_extension.load(
             name=name, sources=srcs, build_directory=bdir, verbose=False,
-            extra_cuda_cflags=["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo"]
-            + EXTRA_FLAGS.get(name, []),
+            extra_cuda_cflags=_cuda_flags(name),
             is_python_module=False)
         shutil.copy(os.path.join(bdir, name + ".so"), so_path(name))
+        with open(_stamp_path(name), "w") as fh:
+            fh.write(" ".join(_cuda_flags(name)))
         return so_path(name)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
@@ -107,7 +130,7 @@ def build(names=None, force=False, parallel=True):
     import subprocess
     os.makedirs(OUT, exist_ok=True)
     want = [n for n in list(TARGETS) + ["ref_knn_cpu"] if not names or n in names]
-    todo = [n for n in want if force or not os.path.exists(so_path(n))]
+    todo = [n for n in want if force or not is_current(n)]
     if parallel and len(todo) > 1:
         procs = [(n, subprocess.Popen([sys.executable, os.path.abspath(__file__), "--one", n] + (["--force"] if force else []),
                                       stdout=subprocess.DEVNULL, stderr=subprocess.PIPE, text=True)) for n in todo]

@@ -1,6 +1,6 @@
 """Pin the CPU oracle (oracle/dvr_ref.c) against outputs of the REFERENCE's own CUDA kernels
 (third_lib/dvr, third_lib/dvxlr, dvxlr_v2 compiled unmodified-in-arithmetic by
-oracle/build_ref.py and run on a B200; vectors made by tools/make_golden_dvr.py)."""
+oracle/build_ref.py and run on the GPU; vectors made by tools/make_golden_dvr.py)."""
 import glob
 import os
 

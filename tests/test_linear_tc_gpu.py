@@ -1,4 +1,4 @@
-"""The tcgen05 3xTF32 Linear (csrc/linear_tc.cu, SURVEY.md 8f-4) against fp64: value_proj's shape
+"""The wgmma 3xTF32 Linear (csrc/linear_tc.cu, SURVEY.md 8f-4) against fp64: value_proj's shape
 (rows = 30825 per camera, 256 -> 256), ragged row counts (TMA clipping / guarded stores), gradients; and
 through SpatialCrossAttention's value_proj.  Tolerance 2e-6 relative to max|y| (fp32 cuBLAS sits at ~1e-6,
 a plain TF32 GEMM at ~5e-4)."""

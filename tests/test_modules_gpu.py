@@ -63,13 +63,22 @@ def test_sca_fused_epilogue_equals_materialised_path(cuda):
 
 
 @pytest.mark.parametrize("bs", [1, 2])
-def test_sca_fused_rebatch_equals_reference_data_flow(cuda, bs):
+def test_sca_fused_rebatch_equals_reference_data_flow(cuda, bs, monkeypatch):
     """SpatialCrossAttention's default path (device-side visible lists, offsets / logits once per pillar,
     rows reduced straight into the BEV slots: vidar_b200/sca.py) against the reference's rebatch /
-    index_add_ data flow on the same CUDA op -- output, input gradients and every parameter gradient."""
+    index_add_ data flow on the same CUDA op -- output, input gradients and every parameter gradient.
+    value_proj / output_proj run on the tensor-core Linear in both flows, as by default.  sampling_offsets /
+    attention_weights run as plain nn.Linear (fp32 cuBLAS) in both: the rebatch flow calls them that way, and a
+    last-bit difference in an offset can move a sample across a pixel-centre line, where grad_sampling_loc is
+    discontinuous."""
+    from vidar_b200.modules import deform_attn
     m = build_attention(mc.SCA_CFG)
     m.load_state_dict(mc.seeded_state(m, 10))
     m.eval().to(cuda)
+    da = m.deformable_attention
+    tc_linear = deform_attn._linear
+    monkeypatch.setattr(deform_attn, "_linear", lambda layer, x: layer(x) if layer in (da.sampling_offsets, da.attention_weights)
+                        else tc_linear(layer, x))
     assert m.fuse_rebatch
     res = []
     for fused in (True, False):

@@ -1,4 +1,4 @@
-"""value_proj's GEMM (6 x 30825 rows, 256 -> 256, SURVEY.md 8f-4): the tcgen05 3xTF32 kernel against cuBLAS fp32
+"""value_proj's GEMM (6 x 30825 rows, 256 -> 256, SURVEY.md 8f-4): the wgmma 3xTF32 kernel against cuBLAS fp32
 (what the reference runs) and cuBLAS TF32 (faster, but 5e-4 off) on the same GPU.  JSON on stdout."""
 import json
 import os
@@ -39,8 +39,8 @@ torch.backends.cuda.matmul.allow_tf32 = True
 out["cublas_tf32_ms"] = timeit(lambda: torch.nn.functional.linear(x, w, b))
 out["cublas_tf32_err"] = float((torch.nn.functional.linear(x[:4096], w, b).double() - ref).abs().max() / ref.abs().max())
 torch.backends.cuda.matmul.allow_tf32 = False
-out["tcgen05_3xtf32_ms"] = timeit(lambda: linear.linear_tf32x3(x, w, b))
-out["tcgen05_3xtf32_err"] = float((linear.linear_tf32x3(x[:4096], w, b).double() - ref).abs().max() / ref.abs().max())
-out["tcgen05_tflops_effective"] = out["flop"] / (out["tcgen05_3xtf32_ms"] * 1e-3) / 1e12
-out["speedup_vs_cublas_fp32"] = out["cublas_fp32_ms"] / out["tcgen05_3xtf32_ms"]
+out["wgmma_3xtf32_ms"] = timeit(lambda: linear.linear_tf32x3(x, w, b))
+out["wgmma_3xtf32_err"] = float((linear.linear_tf32x3(x[:4096], w, b).double() - ref).abs().max() / ref.abs().max())
+out["wgmma_tflops_effective"] = out["flop"] / (out["wgmma_3xtf32_ms"] * 1e-3) / 1e12
+out["speedup_vs_cublas_fp32"] = out["cublas_fp32_ms"] / out["wgmma_3xtf32_ms"]
 print(json.dumps(out))

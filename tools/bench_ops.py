@@ -1,4 +1,4 @@
-"""Per-op timings on one B200: this repo's kernels next to the reference's own PyTorch code
+"""Per-op timings on one H100: this repo's kernels next to the reference's own PyTorch code
 run eagerly on the same GPU (test infrastructure; not the graded bench line).
     python tools/bench_ops.py > gpurun_out/ops.json
 MSDA eager = the grid_sample formula of mmcv's multi_scale_deformable_attn_pytorch (oracle

@@ -1,5 +1,5 @@
 """Same-box GPU baseline: the REFERENCE's own CUDA ray-casters (oracle/_ref, compiled for
-sm_100a by oracle/build_ref.py) next to this repo's kernels on BASELINE configs[2]
+sm_90a by oracle/build_ref.py) next to this repo's kernels on BASELINE configs[2]
 (sigma [1,3,16,200,200], 30000 rays), plus a direct output comparison.  Run on a GPU box:
     python tools/bench_ref_cuda.py > gpurun_out/ref_cuda.json
 The reference synchronises the device inside every call; timings are wall-clock around

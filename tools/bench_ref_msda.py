@@ -16,7 +16,7 @@ LIB = os.path.join(HERE, "libref_lineage_msda.so")
 
 
 def build():
-    cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-shared", "-Xcompiler", "-fPIC",
+    cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-shared", "-Xcompiler", "-fPIC",
            "-cudart", "static", os.path.join(HERE, "ref_lineage_msda.cu"), "-o", LIB]
     subprocess.check_call(cmd)
     return LIB

@@ -106,8 +106,8 @@ def main():
 
 
 def sass_evidence(lib="vidar_b200/libvidar_b200.so", out="profiles/r02_sass_evidence.txt"):
-    """`cuobjdump -sass` mnemonic counts per kernel -> profiles/ (what proves Blackwell-native code:
-    FFMA2, REDG...F32x4, UTMALDG / UTMAREDG, SYNCS).  python tools/summarize_profiles.py --sass"""
+    """`cuobjdump -sass` mnemonic counts per kernel -> profiles/ (what proves Hopper-native code:
+    HGMMA, REDG...F32x4, UTMALDG / UTMAREDG, SYNCS).  python tools/summarize_profiles.py --sass"""
     import collections
     import re
     import subprocess
@@ -123,10 +123,10 @@ def sass_evidence(lib="vidar_b200/libvidar_b200.so", out="profiles/r02_sass_evid
         m = pat.match(line)
         if m and cur:
             stats[cur][m.group(1)] += 1
-    keys = ["FFMA2", "RED", "LDG.E.NA", "LDG.E.128", "UTMALDG", "UTMAREDG", "SYNCS", "DFMA", "ATOMS", "SHFL", "BAR"]
+    keys = ["HGMMA", "RED", "LDG.E.NA", "LDG.E.128", "UTMALDG", "UTMAREDG", "SYNCS", "DFMA", "ATOMS", "SHFL", "BAR"]
     names = subprocess.run(["c++filt"], input="\n".join(stats), capture_output=True, text=True).stdout.splitlines()
-    lines = ["SASS evidence for " + lib + " (sm_100a): `cuobjdump -sass` mnemonic counts per kernel (tools/summarize_profiles.py --sass).",
-             "FFMA2 = packed fp32 FMA (fma.rn.f32x2); RED = red.global.add (the .F32x4 form is the 16-byte vector reduction); LDG.E.NA = "
+    lines = ["SASS evidence for " + lib + " (sm_90a): `cuobjdump -sass` mnemonic counts per kernel (tools/summarize_profiles.py --sass).",
+             "HGMMA = wgmma (Hopper tensor cores); RED = red.global.add (the .F32x4 form is the 16-byte vector reduction); LDG.E.NA = "
              "ld.global.nc.L1::no_allocate; UTMALDG / UTMAREDG = cp.async.bulk.tensor / cp.reduce.async.bulk.tensor (TMA); SYNCS = mbarrier.", ""]
     for (mangled, c), d in zip(stats.items(), names):
         short = re.sub(r"\(.*", "", d.replace("vidar::(anonymous namespace)::", ""))

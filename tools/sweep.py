@@ -1,4 +1,4 @@
-"""BASELINE.json configs[1], [2] and the configs[4] sweep on ONE B200: per-op time, units/s and
+"""BASELINE.json configs[1], [2] and the configs[4] sweep on ONE H100: per-op time, units/s and
 algorithmic GB/s (SURVEY.md 8d byte counts) -> JSON on stdout.  Test infrastructure."""
 import json
 import os

@@ -1,8 +1,8 @@
-"""Build libvidar_b200.so in-tree with nvcc for sm_100a.
+"""Build libvidar_b200.so in-tree with nvcc for sm_90a (H100).
 
 The library has no torch dependency (C ABI, include/vidar_b200.h): it is compiled
 directly with nvcc and linked against the static CUDA runtime, so the built .so travels
-with the repo snapshot to the GPU box.  `python -m vidar_b200.build` rebuilds it.
+with the source tree to the GPU machine.  `python -m vidar_b200.build` rebuilds it.
 """
 import hashlib
 import os
@@ -18,7 +18,7 @@ STAMP = os.path.join(HERE, ".libvidar_b200.stamp")
 
 SOURCES = ["core.cu", "msda.cu", "linear_tc.cu", "dvr.cu", "latent_render.cu", "latent_proj.cu", "ray_head.cu", "sca_glue.cu", "knn.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -84,7 +84,7 @@ def build(force=False, verbose=False):
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
     tmp = LIB + ".tmp"       # link next to the target, then rename: the library on disk is never half-written
     cmd = [nvcc, "-shared", "-o", tmp, *objs, "-cudart", "static",
-           "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC"]
+           "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

@@ -1,4 +1,4 @@
-"""Chamfer distance / nearest-neighbour op, B200-native (SURVEY.md 8(f) item 2).
+"""Chamfer distance / nearest-neighbour op, H100-native (SURVEY.md 8(f) item 2).
 
 Drop-in for the `chamferdist` package the reference builds from
 third_lib/chamfer_dist/chamferdist: `knn_points` (K = 1 only -- the only K ViDAR uses) and

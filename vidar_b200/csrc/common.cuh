@@ -1,4 +1,4 @@
-// Shared helpers for libvidar_b200.so (sm_100a only).
+// Shared helpers for libvidar_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,7 +27,17 @@ inline int check_launch(const char* what) {
     if (!(cond)) return ::vidar::set_error(VIDAR_E_INVALID, __VA_ARGS__); \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+// SMs of the current device (132 on an H100 SXM): sizes the persistent grids.  Grid sizes only
+// set how work is spread, never what is computed.
+inline int num_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      n <= 0) {
+    cudaGetLastError();
+    return 132;
+  }
+  return n;
+}
 
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));

@@ -24,7 +24,7 @@ int set_error(int code, const char* fmt, ...) {
 }  // namespace vidar
 
 extern "C" const char* vidar_last_error(void) { return vidar::err_buf(); }
-extern "C" const char* vidar_version(void) { return "vidar_b200 0.1 sm_100a"; }
+extern "C" const char* vidar_version(void) { return "vidar_b200 0.1 sm_90a"; }
 extern "C" int64_t vidar_launch_count(void) {
   return vidar::g_launches.load(std::memory_order_relaxed);
 }

@@ -1,4 +1,4 @@
-// Voxel ray-casters (dvr / dvxlr / dvxlr_v2) for B200 (sm_100a).
+// Voxel ray-casters (dvr / dvxlr / dvxlr_v2) for H100 (sm_90a).
 //
 // Reference: third_lib/dvr/dvr.cu (init :14-63, render_forward :65-317, render :385-627),
 // third_lib/dvxlr/dvxlr.cu (render :160-457, get_grad_sigma :63-112),
@@ -29,7 +29,7 @@
 // S_0 before the first emission, so gradient kernels walk the ray twice (pass 1: pred,
 // S_0; pass 2: emit) instead of storing the path.  Gradients are accumulated with
 // red.global.add.f32 (the reference's `+=` at dvr.cu:622 is a data race).
-// Launch: 64-thread blocks (30k rays -> 469 blocks over 148 SMs; the reference's
+// Launch: 64-thread blocks (30k rays -> 469 blocks over 132 SMs; the reference's
 // 1024-thread blocks give 30 blocks), one ray per thread, neighbouring rays in a warp.
 #include <float.h>
 #include <stdlib.h>

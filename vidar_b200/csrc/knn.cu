@@ -1,4 +1,4 @@
-// Nearest-neighbour (K = 1) search and its backward for the Chamfer distance, B200 (sm_100a).
+// Nearest-neighbour (K = 1) search and its backward for the Chamfer distance, H100 (sm_90a).
 //
 // Reference: third_lib/chamfer_dist/chamferdist/chamferdist/knn.cu:21-260 (brute-force KNN,
 // 256 blocks x 256 threads, every thread scans all of P2 from global memory), knn_cpu.cpp:7-106,
@@ -9,7 +9,7 @@
 //
 // Mapping: a thread owns one p1 point; p2 streams through shared memory in 1024-point tiles
 // (12 KB, read once per block instead of once per thread), and P2 is additionally split over
-// blockIdx.y so 30k x 30k points fill all 148 SMs; partial results merge with one 64-bit
+// blockIdx.y so 30k x 30k points fill all 132 SMs; partial results merge with one 64-bit
 // atomicMin on (distance bits << 32 | index) -- non-negative floats order like unsigned ints.
 #include "common.cuh"
 
@@ -113,8 +113,8 @@ extern "C" int vidar_nn_forward(const float* p1, const float* p2, const int64_t*
   cudaError_t e = cudaMemsetAsync(scratch, 0xff, sizeof(unsigned long long) * (size_t)N * P1, st);
   if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "knn_points: memset: %s", cudaGetErrorString(e));
   const int bx = (P1 + kNnThreads - 1) / kNnThreads;
-  // enough (block x split) pairs for ~4 waves of 148 SMs, at least one tile per split
-  int splits = (4 * kNumSMs + bx * N - 1) / (bx * N);
+  // enough (block x split) pairs for ~4 waves of the device's SMs, at least one tile per split
+  int splits = (4 * num_sms() + bx * N - 1) / (bx * N);
   const int max_splits = (P2 + kNnTile - 1) / kNnTile;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;

@@ -1,4 +1,4 @@
-// LatentRendering's projections, fused (sm_100a).
+// LatentRendering's projections, fused (sm_90a).
 //
 // Reference: projects/mmdet3d_plugin/bevformer/modules/ray_operations/latent_rendering.py
 //   :94   occ  = unsup_raymarching_head(embed)      (a single Linear E->D when num_pred_fcs == 0,
@@ -8,9 +8,8 @@
 //   :155  out  = out.view(.., D, E/D) * prob.view(.., D, 1)
 // In PyTorch these are 3 skinny cuBLAS GEMMs forward, 6 backward (three of them reductions over
 // all 40 000 rows into a [16..32, 256] weight gradient), 5 bias/elementwise kernels and ~0.6 GB of
-// traffic for 82 MB (fwd) / 123 MB (bwd) of algorithmic bytes (SURVEY.md 8d, B7) -- 0.76 ms of
-// the 2.06 ms module.  Here: one kernel per direction on each side of the ray-marching core,
-// fp32 FMA (the GEMMs have N or K = 16..32: HBM-bound, tensor cores are irrelevant),
+// traffic for 82 MB (fwd) / 123 MB (bwd) of algorithmic bytes (SURVEY.md 8d, B7).  Here: one kernel
+// per direction on each side of the ray-marching core, fp32 FMA (the GEMMs have N or K = 16..32: HBM-bound, tensor cores are irrelevant),
 // `embed` / `grad_out` are read once, `out` / `grad_embed` written once.
 //
 //   proj_in_fwd   [occ | feat] = embed W^T + b            W = [w_occ ; w_feat]  (N1 = D + A <= 32 rows)
@@ -458,7 +457,7 @@ int set_smem(K kernel, size_t bytes, const char* what) {
 }
 
 int grid_for(long long tiles, int per_sm) {
-  const long long cap = (long long)kNumSMs * per_sm;
+  const long long cap = (long long)num_sms() * per_sm;
   return (int)(tiles < cap ? (tiles > 0 ? tiles : 1) : cap);
 }
 

@@ -1,4 +1,4 @@
-// LatentRendering core (the paper's "latent rendering" operator) for B200 (sm_100a).
+// LatentRendering core (the paper's "latent rendering" operator) for H100 (sm_90a).
 //
 // Reference: projects/mmdet3d_plugin/bevformer/modules/ray_operations/latent_rendering.py:98-161
 // -- pure PyTorch: 3 grid_sample launches + cumprod + masks that materialise

@@ -1,4 +1,4 @@
-// Y = X W^T + b on the 5th-generation tensor cores, fp32-accurate (3xTF32), for B200 (sm_100a).
+// Y = X W^T + b on the Hopper tensor cores, fp32-accurate (3xTF32), for H100 (sm_90a).
 //
 // The one dense contraction on the hot path (SURVEY.md 8f-4): MSDeformableAttention3D.value_proj over the
 // flattened camera features, 6 x 30825 rows x 256 -> 256 (spatial_cross_attention.py:333; the operand is
@@ -6,17 +6,17 @@
 // default for matmuls), so a plain TF32 tensor-core GEMM (10-bit mantissas, ~1e-3) would break the 1e-4
 // parity bar.  3xTF32: x = x_hi + x_lo, w = w_hi + w_lo with tf32 parts,
 //     x w  ~=  x_hi w_hi + x_hi w_lo + x_lo w_hi          (dropped term ~2^-22 relative)
-// three tcgen05.mma (kind::tf32) per K step accumulating in fp32 in TMEM.
+// three wgmma.mma_async (tf32, m64n128k8) per K step accumulating in fp32 registers.
 //
-// Kernel (one persistent CTA per SM, 12 warps, warp-specialised, mbarrier pipelines):
-//   warp 0      TMA producer: per K block (32 floats = one 128-byte swizzle row) the raw X tile [128 x 32] and
-//               the pre-split W tiles W_hi / W_lo [128 x 32] -> shared memory (cp.async.bulk.tensor.2d, SWIZZLE_128B)
-//   warps 4-7   splitter: read the raw X tile, write x_hi / x_lo tiles at the same (swizzled) positions
-//               (the split is element-wise, so the TMA's swizzle pattern is preserved), fence.proxy.async
-//   warp 1      MMA issuer (one elected lane): 4 K steps x 3 products of tcgen05.mma.cta_group::1.kind::tf32,
-//               M = 128, N = 128, K = 8, operands by shared-memory descriptors (K-major, SWIZZLE_128B),
-//               accumulator = 128 TMEM columns, double buffered; tcgen05.commit frees the stage / publishes the tile
-//   warps 8-11  epilogue: tcgen05.ld (32 lanes x 32 columns per warp), + bias, 16-byte stores
+// Kernel (one persistent CTA per SM, 3 warpgroups, mbarrier pipeline of kStages stages):
+//   warp 0        TMA producer: per K block (32 floats = one 128-byte swizzle row) the raw X tile [128 x 32] and
+//                 the pre-split W tiles W_hi / W_lo [128 x 32] -> shared memory (cp.async.bulk.tensor.2d, SWIZZLE_128B)
+//   warpgroups 1-2  consumers, one per 64-row half of the tile: split their half of the raw X tile in place
+//                 (x_hi to its own tile, x_lo over the raw values: the split is element-wise, so the TMA's swizzle
+//                 pattern is preserved), fence.proxy.async, then 4 K steps x 3 products of wgmma m64n128k8
+//                 with shared-memory descriptors (K-major, SWIZZLE_128B); after the last K block, + bias and
+//                 8-byte stores straight from the accumulator registers.  The producer runs ahead into the
+//                 next tile while the consumers store, so loads overlap the epilogue.
 // Tiles: (row block of 128) x (column block of 128); K = in_features is looped in blocks of 32.
 // Requires in_features % 32 == 0, out_features % 128 == 0; rows are arbitrary (TMA clips, stores are guarded).
 #include <cuda.h>
@@ -29,11 +29,12 @@ namespace vidar {
 namespace {
 
 constexpr int kTM = 128, kTN = 128, kTK = 32;        // tile: 128 rows x 128 cols, K block of 32 floats (128 bytes)
-constexpr int kStages = 2;
+constexpr int kStages = 3;
 constexpr int kTileBytes = kTM * kTK * 4;            // 16 KB: one [128 x 32] fp32 operand tile
-// per stage: X raw, X hi, X lo, W hi, W lo
-constexpr int kStageBytes = 5 * kTileBytes;
-constexpr int kGemmThreads = 12 * 32;
+// per stage: X raw (then x_lo), X hi, W hi, W lo
+constexpr int kStageBytes = 4 * kTileBytes;
+constexpr int kGemmThreads = 3 * 128;
+constexpr int kConsumerWarps = 8;
 constexpr size_t kGemmSmem = (size_t)kStages * kStageBytes + 1024 /* alignment slack */ + 256 /* barriers */;
 
 __device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -61,28 +62,45 @@ __device__ __forceinline__ void tma_2d(void* dst, const CUtensorMap* m, int c0, 
       ::"r"(s32(dst)), "l"(m), "r"(c0), "r"(c1), "r"(s32(bar)) : "memory");
 }
 // K-major operand tile [rows x 32 floats], 128-byte rows, SWIZZLE_128B, 8-row groups 1024 bytes apart
-// (cute::UMMA::SmemDescriptor: start >> 4 | LBO(1) << 16 | SBO(1024 >> 4) << 32 | version 1 << 46 | layout 2 << 61)
-__device__ __forceinline__ unsigned long long umma_desc(const void* tile, int k_byte_offset) {
+// (wgmma matrix descriptor: start >> 4 | LBO(1, unused when swizzled) << 16 | SBO(1024 >> 4) << 32 | 128B swizzle << 62).
+// The tile is 1024-byte aligned, so the base-offset field stays 0; a K step of 8 tf32 moves the start by 32 bytes.
+__device__ __forceinline__ unsigned long long gmma_desc(const void* tile, int k_byte_offset) {
   const unsigned addr = s32(tile) + (unsigned)k_byte_offset;
   unsigned long long d = (unsigned long long)((addr >> 4) & 0x3fffu);
   d |= 1ull << 16;
   d |= (unsigned long long)(1024 >> 4) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
+  d |= 1ull << 62;
   return d;
 }
-// kind::tf32, fp32 accumulate, A and B K-major, N = 128, M = 128   (cute::UMMA::InstrDescriptor)
-constexpr unsigned kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(kTN >> 3) << 17) | ((unsigned)(kTM >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(unsigned d_tmem, unsigned long long a, unsigned long long b, bool accumulate) {
+// d[64x128] += a[64x8] b[8x128]^T, tf32 operands from shared memory, fp32 accumulators in registers
+// (thread layout: d[4j + 2h + e] is row 16 warp + lane / 4 + 8h, column 8j + 2 (lane % 4) + e).
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], unsigned long long a, unsigned long long b) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a), "l"(b), "r"(kIdesc), "r"((unsigned)accumulate) : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// The accumulators are written asynchronously: pin them so no register access moves across issue / wait.
+__device__ __forceinline__ void fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ float to_tf32(float x) {
   unsigned r;
@@ -103,12 +121,8 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   // SWIZZLE_128B tiles need 1024-byte alignment
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gemm_smem_raw) + 1023) & ~(uintptr_t)1023);
   unsigned long long* bars = reinterpret_cast<unsigned long long*>(smem + kStages * kStageBytes);
-  unsigned long long* tma_full = bars;                 // [kStages]  TMA -> splitter / MMA
-  unsigned long long* split_done = bars + kStages;     // [kStages]  splitter -> MMA
-  unsigned long long* stage_free = bars + 2 * kStages; // [kStages]  MMA (commit) -> TMA
-  unsigned long long* acc_full = bars + 3 * kStages;   // [2]        MMA (commit) -> epilogue
-  unsigned long long* acc_empty = bars + 3 * kStages + 2;   // [2]   epilogue -> MMA
-  __shared__ unsigned tmem_base_s;
+  unsigned long long* full = bars;                     // [kStages]  TMA -> consumers
+  unsigned long long* empty = bars + kStages;          // [kStages]  consumers (wgmma done) -> TMA
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k_blocks = g.K / kTK;
@@ -116,24 +130,12 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
-      mb_init(&tma_full[s], 1);
-      mb_init(&split_done[s], 4);          // one arrive per splitter warp
-      mb_init(&stage_free[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mb_init(&acc_full[b], 1);
-      mb_init(&acc_empty[b], 4);           // one arrive per epilogue warp
+      mb_init(&full[s], 1);
+      mb_init(&empty[s], kConsumerWarps);  // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {                         // TMEM: 2 accumulators x 128 columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(s32(&tmem_base_s)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tmem_base = tmem_base_s;
 
   if (warp == 0) {
     // ===== TMA producer =====
@@ -144,64 +146,37 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
         for (int kb = 0; kb < k_blocks; ++kb, ++it) {
           const int s = it % kStages;
           const unsigned ph = (it / kStages) & 1u;
-          mb_wait(&stage_free[s], ph ^ 1u);                      // first pass: passes immediately
+          mb_wait(&empty[s], ph ^ 1u);                           // first pass: passes immediately
           unsigned char* st = smem + s * kStageBytes;
-          mb_expect_tx(&tma_full[s], 3 * kTileBytes);
-          tma_2d(st, &map_x, kb * kTK, tm * kTM, &tma_full[s]);                      // X raw
-          tma_2d(st + 3 * kTileBytes, &map_whi, kb * kTK, tn * kTN, &tma_full[s]);   // W hi
-          tma_2d(st + 4 * kTileBytes, &map_wlo, kb * kTK, tn * kTN, &tma_full[s]);   // W lo
+          mb_expect_tx(&full[s], 3 * kTileBytes);
+          tma_2d(st, &map_x, kb * kTK, tm * kTM, &full[s]);                          // X raw
+          tma_2d(st + 2 * kTileBytes, &map_whi, kb * kTK, tn * kTN, &full[s]);       // W hi
+          tma_2d(st + 3 * kTileBytes, &map_wlo, kb * kTK, tn * kTN, &full[s]);       // W lo
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    unsigned it = 0, tile_i = 0;
-    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++tile_i) {
-      const int ab = tile_i & 1;
-      const unsigned aph = (tile_i >> 1) & 1u;
-      mb_wait(&acc_empty[ab], aph ^ 1u);                         // epilogue drained this accumulator
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const unsigned d_tmem = tmem_base + (unsigned)(ab * kTN);
-      for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-        const int s = it % kStages;
-        const unsigned ph = (it / kStages) & 1u;
-        mb_wait(&tma_full[s], ph);
-        mb_wait(&split_done[s], ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (lane == 0) {
-          unsigned char* st = smem + s * kStageBytes;
-          const void* xhi = st + 1 * kTileBytes;
-          const void* xlo = st + 2 * kTileBytes;
-          const void* whi = st + 3 * kTileBytes;
-          const void* wlo = st + 4 * kTileBytes;
-#pragma unroll
-          for (int k = 0; k < kTK / 8; ++k) {                    // tf32: K = 8 per instruction = 32 bytes
-            const int ko = k * 32;
-            umma_tf32(d_tmem, umma_desc(xhi, ko), umma_desc(whi, ko), (kb | k) != 0);
-            umma_tf32(d_tmem, umma_desc(xhi, ko), umma_desc(wlo, ko), true);
-            umma_tf32(d_tmem, umma_desc(xlo, ko), umma_desc(whi, ko), true);
-          }
-          umma_commit(&stage_free[s]);                           // the stage may be refilled when these MMAs finish
-          if (kb == k_blocks - 1) umma_commit(&acc_full[ab]);    // ... and the tile is complete
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===== splitter: x -> (tf32(x), tf32(x - tf32(x))) at the same swizzled positions =====
-    const int tid = threadIdx.x - 4 * 32;                        // 0..127
+  } else if (warp >= 4) {
+    // ===== consumers: warpgroup c owns rows [64 c, 64 c + 64) of the tile =====
+    const int c = (warp >> 2) - 1;
+    const int tid = threadIdx.x & 127;
+    const int half = c * (kTileBytes / 2);                       // byte offset of this half in an operand tile
     unsigned it = 0;
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+      const int tm = t / g.tiles_n, tn = t % g.tiles_n;
+      float d[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
       for (int kb = 0; kb < k_blocks; ++kb, ++it) {
         const int s = it % kStages;
         const unsigned ph = (it / kStages) & 1u;
-        mb_wait(&tma_full[s], ph);
-        const float4* raw = reinterpret_cast<const float4*>(smem + s * kStageBytes);
-        float4* hi = reinterpret_cast<float4*>(smem + s * kStageBytes + kTileBytes);
-        float4* lo = reinterpret_cast<float4*>(smem + s * kStageBytes + 2 * kTileBytes);
+        mb_wait(&full[s], ph);
+        unsigned char* st = smem + s * kStageBytes;
+        // x -> (tf32(x), tf32(x - tf32(x))) at the same swizzled positions; x_lo overwrites x
+        float4* lo = reinterpret_cast<float4*>(st + half);
+        float4* hi = reinterpret_cast<float4*>(st + kTileBytes + half);
 #pragma unroll
-        for (int i = 0; i < kTileBytes / 16 / 128; ++i) {        // 1024 float4 per tile, 128 threads
-          const float4 v = raw[i * 128 + tid];
+        for (int i = 0; i < kTileBytes / 2 / 16 / 128; ++i) {    // 512 float4 per half tile, 128 threads
+          const float4 v = lo[i * 128 + tid];
           float4 h, l;
           h.x = to_tf32(v.x); h.y = to_tf32(v.y); h.z = to_tf32(v.z); h.w = to_tf32(v.w);
           l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
@@ -209,58 +184,41 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
           lo[i * 128 + tid] = l;
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> tensor-core reads
-        __syncwarp();
-        if (lane == 0) mb_arrive(&split_done[s]);
-      }
-    }
-  } else if (warp >= 8) {
-    // ===== epilogue: TMEM -> registers -> + bias -> global =====
-    const int ew = warp - 8;                                     // TMEM lanes [32 ew, 32 ew + 32)
-    unsigned tile_i = 0;
-    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++tile_i) {
-      const int tm = t / g.tiles_n, tn = t % g.tiles_n;
-      const int ab = tile_i & 1;
-      const unsigned aph = (tile_i >> 1) & 1u;
-      mb_wait(&acc_full[ab], aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int row = tm * kTM + ew * 32 + lane;
-      float* yrow = y + (size_t)row * g.N + tn * kTN;
-      const float* brow = bias ? bias + tn * kTN : nullptr;
-#pragma unroll 1
-      for (int c0 = 0; c0 < kTN; c0 += 32) {
-        unsigned v[32];
-        const unsigned taddr = tmem_base + ((unsigned)(ew * 32) << 16) + (unsigned)(ab * kTN + c0);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (row < g.M) {
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + c) : "memory");      // the whole half is split
+        const unsigned char* xlo = st + half;
+        const unsigned char* xhi = st + kTileBytes + half;
+        const unsigned char* whi = st + 2 * kTileBytes;
+        const unsigned char* wlo = st + 3 * kTileBytes;
+        fence_acc(d);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 o;
-            o.x = __uint_as_float(v[j + 0]) + (brow ? __ldg(brow + c0 + j + 0) : 0.f);
-            o.y = __uint_as_float(v[j + 1]) + (brow ? __ldg(brow + c0 + j + 1) : 0.f);
-            o.z = __uint_as_float(v[j + 2]) + (brow ? __ldg(brow + c0 + j + 2) : 0.f);
-            o.w = __uint_as_float(v[j + 3]) + (brow ? __ldg(brow + c0 + j + 3) : 0.f);
-            *reinterpret_cast<float4*>(yrow + c0 + j) = o;
-          }
+        for (int k = 0; k < kTK / 8; ++k) {                      // tf32: K = 8 per instruction = 32 bytes
+          const int ko = k * 32;
+          wgmma_tf32(d, gmma_desc(xhi, ko), gmma_desc(whi, ko));
+          wgmma_tf32(d, gmma_desc(xhi, ko), gmma_desc(wlo, ko));
+          wgmma_tf32(d, gmma_desc(xlo, ko), gmma_desc(whi, ko));
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_acc(d);
+        __syncwarp();
+        if (lane == 0) mb_arrive(&empty[s]);                     // this warp's reads of the stage are done
+      }
+      // ===== epilogue: registers + bias -> global =====
+      const int row0 = tm * kTM + c * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int col0 = tn * kTN + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < kTN / 8; ++j) {
+        const int col = col0 + 8 * j;
+        const float b0 = bias ? __ldg(bias + col) : 0.f, b1 = bias ? __ldg(bias + col + 1) : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row < g.M)
+            *reinterpret_cast<float2*>(y + (size_t)row * g.N + col) = make_float2(d[4 * j + 2 * h] + b0, d[4 * j + 2 * h + 1] + b1);
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mb_arrive(&acc_empty[ab]);
     }
-  }
-
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base) : "memory");
   }
 }
 
@@ -291,7 +249,7 @@ EncodeFn encode_fn() {
   return fn;
 }
 
-// [rows, K] fp32 row-major, box [128 rows x 32 floats], 128-byte swizzle (what the UMMA descriptors expect)
+// [rows, K] fp32 row-major, box [128 rows x 32 floats], 128-byte swizzle (what the wgmma descriptors expect)
 bool make_operand_map(CUtensorMap* m, const float* base, long long rows, int K) {
   EncodeFn enc = encode_fn();
   if (!enc) return false;
@@ -308,7 +266,7 @@ bool make_operand_map(CUtensorMap* m, const float* base, long long rows, int K) 
 
 using namespace vidar;
 
-// y [M, N] = x [M, K] w[N, K]^T + bias [N]   (nn.Linear), fp32 in / out, 3xTF32 on tcgen05.
+// y [M, N] = x [M, K] w[N, K]^T + bias [N]   (nn.Linear), fp32 in / out, 3xTF32 on wgmma.
 // w_split: caller-provided scratch of 2 * N * K floats (the library never allocates).
 extern "C" int vidar_linear_tf32x3(const float* x, const float* w, const float* bias, float* y, float* w_split, int M,
                                    int N, int K, void* stream) {
@@ -334,7 +292,8 @@ extern "C" int vidar_linear_tf32x3(const float* x, const float* w, const float* 
   g.tiles_m = (M + kTM - 1) / kTM;
   g.tiles_n = N / kTN;
   const int tiles = g.tiles_m * g.tiles_n;
-  const int grid = tiles < kNumSMs ? tiles : kNumSMs;
+  const int sms = num_sms();
+  const int grid = tiles < sms ? tiles : sms;
   if (cudaFuncSetAttribute(linear_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmem) != cudaSuccess)
     return set_error(VIDAR_E_CUDA, "%s: cannot opt in to %zu bytes of shared memory", who, kGemmSmem);
   linear_tf32x3_kernel<<<grid, kGemmThreads, kGemmSmem, st>>>(mx, mhi, mlo, bias, y, g);

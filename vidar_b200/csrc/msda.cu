@@ -1,4 +1,4 @@
-// Multi-scale deformable attention, forward + backward, for B200 (sm_100a).
+// Multi-scale deformable attention, forward + backward, for H100 (sm_90a).
 //
 // Replaces mmcv-full 1.4.0 `_ext.ms_deform_attn_{forward,backward}` as called from
 // projects/mmdet3d_plugin/bevformer/modules/multi_scale_deformable_attn_function.py:118-124,150-160.
@@ -85,28 +85,6 @@ __device__ __forceinline__ void decode_sample(float lx, float ly, int Hl, int Wl
   }
 }
 
-// Blackwell packed fp32: one FFMA2 does two fused multiply-adds (fma.rn.f32x2, sm_100+), so
-// a float4 of channels costs two issue slots instead of four.  Same IEEE rounding as FFMA.
-typedef unsigned long long u64;
-__device__ __forceinline__ u64 pk(float lo, float hi) {
-  u64 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpk(u64 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ u64 fmul2(u64 a, u64 b) {
-  u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-
 // Cache policy of the gather.  The fine pyramid levels have (almost) no reuse inside an SM -- a
 // 24x24-pixel window per anchor and two samples in it -- while one head's coarse levels (15x25: 48 KB,
 // 29x50: 186 KB) are re-read by every query: fine-level lines are loaded with L1::no_allocate so they
@@ -121,22 +99,21 @@ __device__ __forceinline__ float4 ldg4_na(const float* p) {
 __device__ __forceinline__ float4 ldg4_h(const float* p, bool na) { return na ? ldg4_na(p) : ldg4(p); }
 
 __device__ __forceinline__ float4 f4_zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+// Explicitly rounded fp32 (fmaf / __fmul_rn): the order of operations is fixed, so results do not
+// depend on the compiler's contraction choices.
 __device__ __forceinline__ void f4_fma(float4& a, float s, const float4& v) {
-  const u64 ss = pk(s, s);
-  unpk(ffma2(ss, pk(v.x, v.y), pk(a.x, a.y)), a.x, a.y);
-  unpk(ffma2(ss, pk(v.z, v.w), pk(a.z, a.w)), a.z, a.w);
+  a.x = fmaf(s, v.x, a.x);
+  a.y = fmaf(s, v.y, a.y);
+  a.z = fmaf(s, v.z, a.z);
+  a.w = fmaf(s, v.w, a.w);
 }
 __device__ __forceinline__ float f4_dot(const float4& a, const float4& b) {
-  float lo, hi;
-  unpk(ffma2(pk(a.x, a.y), pk(b.x, b.y), fmul2(pk(a.z, a.w), pk(b.z, b.w))), lo, hi);
-  return lo + hi;
+  const float lo = fmaf(a.x, b.x, __fmul_rn(a.z, b.z));
+  const float hi = fmaf(a.y, b.y, __fmul_rn(a.w, b.w));
+  return __fadd_rn(lo, hi);
 }
 __device__ __forceinline__ float4 f4_scale(float s, const float4& v) {
-  float4 r;
-  const u64 ss = pk(s, s);
-  unpk(fmul2(ss, pk(v.x, v.y)), r.x, r.y);
-  unpk(fmul2(ss, pk(v.z, v.w)), r.z, r.w);
-  return r;
+  return make_float4(__fmul_rn(s, v.x), __fmul_rn(s, v.y), __fmul_rn(s, v.z), __fmul_rn(s, v.w));
 }
 
 
@@ -753,12 +730,10 @@ __global__ void msda_backward_generic_kernel(const MsdaParams p, const float* __
   }
 }
 
-// FORWARD only: per-head level slabs larger than this are read with L1::no_allocate (see ldg4_na).
-// Measured on B200, 6 cameras x 40000 queries (tools/exp_msda.py, profiles/r02_msda_cache_hints.json):
-//   off 2.44 ms | > 1 MB (level 0) 2.42 | > 256 KB (levels 0-1) 2.32 | > 100 KB (levels 0-2) 2.26
-// so everything but the 48 KB 15x25 level streams.  The backward gets slower with any of these
-// (4.60 -> 4.68 / 4.74 ms: its loads share the LSU -> XBAR request path with the reductions, and a
-// no-allocate miss cannot merge with a neighbouring warp's pending miss), so it keeps plain loads.
+// FORWARD only: per-head level slabs larger than this are read with L1::no_allocate (see ldg4_na), so at
+// the SpatialCrossAttention shape everything but the 48 KB 15x25 level streams (tools/exp_msda.py sweeps the
+// threshold).  The backward keeps plain loads: they share the LSU -> XBAR request path with the reductions,
+// and a no-allocate miss cannot merge with a neighbouring warp's pending miss.
 // VIDAR_MSDA_STREAM_BYTES overrides the forward threshold (experiments; 0xffffffff = off).
 inline unsigned stream_threshold() {
   static const unsigned v = [] {
@@ -830,11 +805,11 @@ inline long long num_blocks(const MsdaParams& p) {
 
 
 // ---- slab (persistent, shared-memory) variants: host side --------------------------------------
-// VIDAR_MSDA_SLAB: 0 = off (default), 1 = slab kernels with plain staging / flush, 2 = with TMA.  Measured on
-// B200 (profiles/r02_msda_slab_experiment.json): backward 4.48 -> 5.25 ms, forward 2.06 -> 2.19 ms per 6
-// cameras -- the shared-memory hand-over costs more than the 25 % of reduction lines it removes (a barrier
-// per 16-query tile, ~10 issue slots per record, half the L1), with or without TMA.  The variants stay
-// selectable (and parity-tested, tests/test_msda_gpu.py::test_slab_variants) but off.
+// VIDAR_MSDA_SLAB: 0 = off (default), 1 = slab kernels with plain staging / flush, 2 = with TMA.  Both
+// variants were measured slower than the default kernels at the SpatialCrossAttention shape: the
+// shared-memory hand-over costs more than the 25 % of reduction lines it removes (a barrier per 16-query tile,
+// ~10 issue slots per record, half the L1), with or without TMA.  They stay selectable (and parity-tested,
+// tests/test_msda_gpu.py::test_slab_variants) but off.
 inline int slab_mode() {
   static const int v = [] {
     const char* e = getenv("VIDAR_MSDA_SLAB");
@@ -880,7 +855,7 @@ inline bool slab_ok(const MsdaParams& p) {
 }
 
 inline void slab_geo(const MsdaParams& p, SlabGeo& sg, int& grid) {
-  const int slots = 2 * kNumSMs;
+  const int slots = 2 * num_sms();
   const int nh = p.B * p.H;
   sg.first_it = (p.LP - p.P) / 4;
   sg.pix_shift = 0;
@@ -1128,8 +1103,8 @@ extern "C" int vidar_msda_rows_forward(const float* value, const int64_t* spatia
   rc = fill_rows(p, idx, count, inv_count, bs, ncl, cam0, Qd, S, s_lo, s_hi, who);
   if (rc) return rc;
   VIDAR_REQUIRE(slots, "%s: null output", who);
-  // the streaming hint helps the plain forward (2.24 -> 2.06 ms) but not this one, whose epilogue also sends 245 MB
-  // of slot reductions through L2 (2.25 -> 2.35 ms, gpurun r2g): plain loads here
+  // the streaming hint helps the plain forward but not this one, whose epilogue also sends 245 MB
+  // of slot reductions through L2: plain loads here
   p.na_bytes = 0xffffffffu;
   if (slab_ok(p) && slab_forward_on()) return launch_slab_forward<false, true>(p, slots, (cudaStream_t)stream, who);
   VIDAR_ROWS_LAUNCH(msda_forward_kernel, false, p, slots);

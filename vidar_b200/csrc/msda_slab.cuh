@@ -1,8 +1,7 @@
 // Persistent "slab" variants of the SpatialCrossAttention-shaped MSDA kernels (textually included by
 // msda.cu inside namespace vidar { namespace { ... } }: they share its helpers).
 //
-// Why.  ncu (profiles/r01_ncu_summary.txt) puts msda_backward_kernel at 90 % of the SM's L1 -> XBAR
-// request path: every corner of every sample leaves the SM as one 128-byte `red.global.add.v4.f32` line
+// Why.  msda_backward_kernel is bound by the SM's L1 -> XBAR request path: every corner of every sample leaves the SM as one 128-byte `red.global.add.v4.f32` line
 // (~5 request cycles), 277 k lines per SM and launch, while the 15x25 level receives ~3400 of them per
 // pixel and head.  One head's slab of the coarsest level is 48 KB, so a block can keep it in SHARED
 // MEMORY and send it out once:
@@ -11,7 +10,7 @@
 //             in shared memory; after every tile (one query per warp, 16 warps) a barrier hands the 512
 //             records over: warp w owns the pixels with (pixel & 15) == w, finds its records with a
 //             ballot and adds weight * grad_out_row into the slab (lane = channel: conflict-free, no
-//             atomics -- fp32 shared-memory atomics are CAS loops on sm_100a).  The slab is flushed once
+//             atomics -- fp32 shared-memory atomics are CAS loops on sm_90a).  The slab is flushed once
 //             per unit: 375 lines instead of ~110 k.  The flush is a TMA bulk reduction
 //             (cp.reduce.async.bulk.tensor, SASS UTMAREDG) when a tensor map is available.
 //   forward   the same decomposition with the coarsest level's value slab STAGED in shared memory by TMA

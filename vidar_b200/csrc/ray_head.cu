@@ -1,4 +1,4 @@
-// ViDAR head ray sampler, fused cross-entropy and arg-max decode for B200 (sm_100a).
+// ViDAR head ray sampler, fused cross-entropy and arg-max decode for H100 (sm_90a).
 //
 // Reference (pure PyTorch, many launches and [R,513] intermediates):
 //   projects/mmdet3d_plugin/bevformer/dense_heads/vidar_head_base.py

@@ -1,4 +1,4 @@
-// BEV pillar -> camera projection of the BEV encoder (`point_sampling`) for B200 (sm_100a).
+// BEV pillar -> camera projection of the BEV encoder (`point_sampling`) for H100 (sm_90a).
 //
 // Reference: projects/mmdet3d_plugin/bevformer/modules/encoder.py:94-156 -- PyTorch: the
 // [D,B,cams,Q,4,4] lidar2img repeat (61 MB at 6 cams x 40000 pillars x 4 anchors), a batched

@@ -1,8 +1,8 @@
-"""nn.Linear on the B200 tensor cores with fp32 accuracy (3xTF32, csrc/linear_tc.cu).
+"""nn.Linear on the H100 tensor cores with fp32 accuracy (3xTF32, csrc/linear_tc.cu).
 
 The reference runs `value_proj` -- the one dense contraction on the hot path, 6 x 30825 x 256 -> 256 per
 SpatialCrossAttention layer (spatial_cross_attention.py:333) -- as an fp32 cuBLAS GEMM.  `linear_tf32x3`
-computes the same product on tcgen05 (TMA-fed, TMEM accumulators) with every operand split into two TF32
+computes the same product with wgmma (TMA-fed, register accumulators) with every operand split into two TF32
 parts, three MMAs per K step: ~1e-6 relative, i.e. inside the 1e-4 parity bar that a plain TF32 GEMM misses.
 Backward: grad_input through the same kernel (weight transposed); grad_weight / grad_bias are [N, K]-sized
 reductions over all rows and stay on cuBLAS (fp32).

@@ -34,7 +34,7 @@ TC_LINEAR = True      # Linear layers of these modules on the tensor cores (3xTF
 
 
 def _linear(layer, x):
-    """`layer(x)` for an nn.Linear: the tcgen05 3xTF32 kernel (fp32-accurate) for fp32 CUDA inputs whose in / out
+    """`layer(x)` for an nn.Linear: the wgmma 3xTF32 kernel (fp32-accurate) for fp32 CUDA inputs whose in / out
     features are multiples of 128 -- value_proj over 6 x 30825 rows is the one large GEMM on the path
     (spatial_cross_attention.py:333) -- otherwise the module itself (cuBLAS)."""
     if TC_LINEAR and layer.bias is not None and _tc.supported(layer.in_features, layer.out_features, x) and x.numel() > 0:

@@ -1,4 +1,4 @@
-"""Multi-scale deformable attention op boundary, B200-native.
+"""Multi-scale deformable attention op boundary, H100-native.
 
 Drop-in for projects/mmdet3d_plugin/bevformer/modules/multi_scale_deformable_attn_function.py
 of the reference:

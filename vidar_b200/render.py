@@ -1,4 +1,4 @@
-"""Voxel ray-caster op boundary (dvr / dvxlr / dvxlr_v2), B200-native.
+"""Voxel ray-caster op boundary (dvr / dvxlr / dvxlr_v2), H100-native.
 
 Drop-in for the reference's JIT-compiled pybind modules and their autograd wrappers:
 
