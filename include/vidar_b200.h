@@ -119,7 +119,9 @@ int vidar_msda_sca_backward(const float* value, const int64_t* spatial_shapes,
  *   camera that sees the pillar, so they are computed once per pillar and read through idx.
  * Backward: grad_slots [bs, Qd, H*C] is read through the same map; grad_value accumulated (caller zeroes);
  *   rows:     grad_sampling_loc / grad_attn_weight written for the rows of this launch (caller zeroes the rest);
- *   sca_rows: grad_offsets / grad_logits ACCUMULATED over cameras with red.global.add (caller zeroes). */
+ *   sca_rows: grad_offsets / grad_logits ACCUMULATED over cameras with red.global.add (caller zeroes).
+ *   At C = 32 with 4 levels x 8 points both backwards first put the rows in image order, with stream-ordered
+ *   scratch (8 B per row) from a memory pool of the library; `rows` then needs sampling_loc 16-byte aligned. */
 int vidar_sca_compact(const unsigned char* bev_mask, int32_t* idx, int32_t* count, float* inv_count,
                       int cams, int bs, int Q, int D, void* stream);
 int vidar_msda_rows_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,

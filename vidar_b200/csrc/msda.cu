@@ -24,6 +24,11 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <mutex>
+
+#include <cub/block/block_radix_sort.cuh>
+#include <cub/block/block_scan.cuh>
+
 #include "common.cuh"
 
 namespace vidar {
@@ -657,6 +662,377 @@ msda_backward_small_kernel(const MsdaParams p, const float* __restrict__ grad_ou
   }
 }
 
+// ---- row-indirect backward at SpatialCrossAttention's shape (C = 32, L*P = 32, P = 8): tile aggregation --------
+// The per-corner grad_value reductions of msda_backward_kernel (4 x 128-byte lines per sample) saturate the
+// SM -> L2 request path.  Rows close together in the *image* hit the same pixels, so the rows of each batch element
+// are first put in image order (a stable counting sort by a 16 x 16 cell of the row's mean sampling location), and
+// one CTA then owns a tile of kTileRows ordered rows of one head.  Per pyramid level it gathers and computes the
+// sampling-location / attention gradients as msda_backward_kernel does (same arithmetic), writes one record per
+// corner (level pixel, weight, row) to shared memory, sorts the records by pixel and sums each pixel's run with
+// lane = channel, so a (pixel, head) line is reduced once per tile instead of once per corner.
+constexpr int kTileRows = 256;                               // rows per tile
+constexpr int kTilePoints = 8;                               // points per level (P)
+constexpr int kTileRecs = kTileRows * kTilePoints * 4;       // corner records per level
+constexpr int kRecBits = 13;                                 // record index bits: log2(kTileRecs)
+constexpr int kTileThreads = 512;                            // 16 warps, 16 rows each
+constexpr int kTileItems = kTileRecs / kTileThreads;         // records per thread in the sort
+constexpr int kTileSeg = kTileRecs / (kTileThreads / 8);     // sorted records summed by one 8-lane group
+constexpr int kCells = 256;                                  // 16 x 16 image cells of the row order
+constexpr int kOrderChunk = 1024;                            // rows per block of the row-order kernels
+static_assert(kTileRecs == 1 << kRecBits, "record index width");
+
+// Is list entry j of batch element n one of this launch's rows?  (the rows resolve_row<true> accepts)
+__device__ __forceinline__ bool row_live(const MsdaParams& p, int n, int j) {
+  if (p.count && j >= __ldg(p.count + p.cam0 + n % p.ncl)) return false;
+  if (p.S > 1) {
+    const int sl = (j >> 6) % p.S;
+    if (sl < p.s_lo || sl >= p.s_hi) return false;
+  }
+  return true;
+}
+
+// Row order, pass 1: each live row's image cell (-1 = not a row of this launch) and the cell histogram of every
+// chunk of kOrderChunk rows.  The cell is taken from the mean of head 0's sampling locations, or with the fused
+// epilogue (EPI) from the mean of the pillar's reference_points_cam Z-anchors.
+template <bool EPI>
+__global__ void __launch_bounds__(kOrderChunk)
+rows_key_kernel(const MsdaParams p, int* __restrict__ key, int* __restrict__ hist) {
+  __shared__ int cnt[kCells];
+  const int n = blockIdx.y, j = blockIdx.x * kOrderChunk + threadIdx.x;
+  if (threadIdx.x < kCells) cnt[threadIdx.x] = 0;
+  __syncthreads();
+  if (j < p.Q) {
+    int k = -1;
+    if (row_live(p, n, j)) {
+      float sx = 0.f, sy = 0.f, s;
+      if (EPI) {
+        const int c = p.cam0 + n % p.ncl, b = n / p.ncl;
+        const size_t q = p.idx ? (size_t)__ldg(p.idx + (size_t)c * p.Qd + j) : (size_t)j;
+        const float2* r = reinterpret_cast<const float2*>(p.ref) + (((size_t)c * p.bs + b) * p.Qd + q) * p.D;
+        for (int i = 0; i < p.D; ++i) {
+          const float2 v = __ldg(r + i);
+          sx += v.x;
+          sy += v.y;
+        }
+        s = 16.f / (float)p.D;
+      } else {
+        const float4* l = reinterpret_cast<const float4*>(p.loc + ((size_t)n * p.Q + j) * p.H * p.LP * 2);
+        for (int i = 0; i < p.LP / 2; ++i) {
+          const float4 v = __ldg(l + i);
+          sx += v.x + v.z;
+          sy += v.y + v.w;
+        }
+        s = 16.f / (float)p.LP;
+      }
+      k = min(max((int)(sy * s), 0), 15) * 16 + min(max((int)(sx * s), 0), 15);
+      atomicAdd(&cnt[k], 1);
+    }
+    key[(size_t)n * p.Q + j] = k;
+  }
+  __syncthreads();
+  if (threadIdx.x < kCells) hist[((size_t)n * gridDim.x + blockIdx.x) * kCells + threadIdx.x] = cnt[threadIdx.x];
+}
+
+// pass 2, one block per batch element: hist becomes the first ordered position of each (chunk, cell), cell-major
+__global__ void __launch_bounds__(kCells)
+rows_scan_kernel(int* __restrict__ hist, int* __restrict__ nlive, int nch) {
+  using Scan = cub::BlockScan<int, kCells>;
+  __shared__ typename Scan::TempStorage tmp;
+  int* h = hist + (size_t)blockIdx.x * nch * kCells + threadIdx.x;
+  int run = 0;
+  for (int ch = 0; ch < nch; ++ch) {
+    const int v = h[(size_t)ch * kCells];
+    h[(size_t)ch * kCells] = run;
+    run += v;
+  }
+  int base, total;
+  Scan(tmp).ExclusiveSum(run, base, total);
+  for (int ch = 0; ch < nch; ++ch) h[(size_t)ch * kCells] += base;
+  if (threadIdx.x == 0) nlive[blockIdx.x] = total;
+}
+
+// pass 3: perm[n][position] = j, stable (rows of a cell keep their list order)
+__global__ void __launch_bounds__(kOrderChunk)
+rows_scatter_kernel(const int* __restrict__ key, const int* __restrict__ hist, int* __restrict__ perm, int Q) {
+  constexpr int W = kOrderChunk / 32;
+  __shared__ int wc[W][kCells];   // rows of each cell in each warp, then their exclusive prefix over warps
+  const int n = blockIdx.y, j = blockIdx.x * kOrderChunk + threadIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < W * kCells; i += kOrderChunk) (&wc[0][0])[i] = 0;
+  __syncthreads();
+  const int k = j < Q ? key[(size_t)n * Q + j] : -1;
+  const unsigned peers = __match_any_sync(0xffffffffu, k);
+  const int rank = __popc(peers & ((1u << lane) - 1u));
+  if (k >= 0 && rank == 0) wc[warp][k] = __popc(peers);
+  __syncthreads();
+  if (threadIdx.x < kCells) {
+    int run = 0;
+    for (int w = 0; w < W; ++w) {
+      const int v = wc[w][threadIdx.x];
+      wc[w][threadIdx.x] = run;
+      run += v;
+    }
+  }
+  __syncthreads();
+  if (k >= 0) perm[(size_t)n * Q + hist[((size_t)n * gridDim.x + blockIdx.x) * kCells + k] + wc[warp][k] + rank] = j;
+}
+
+using TileSort = cub::BlockRadixSort<unsigned, kTileThreads, kTileItems, cub::NullType, 5, false>;
+// The records and the sort's temp storage are static shared memory: their addresses are then constants rather than
+// registers (the kernel runs at the 64-register limit of 2 x 512 threads per SM).
+union __align__(16) TileKeys {
+  unsigned key[kTileRecs + kTileRecs / kTileSeg];   // records; once sorted, one pad word per group segment
+  typename TileSort::TempStorage sort;
+};
+struct TileSmem {                        // dynamic shared memory
+  float w[kTileRecs];                    // record weight attn * bilinear corner weight
+  float4 go[kTileRows * 8];              // row's grad_out head vector, scaled by 1 / #cameras
+  int item[kTileRows];                   // row's item index (EPI: its pillar's (b, q, h) index), -1 past the last row
+  size_t slab;                           // float offset of the (n, h) slab in value / grad_value
+};
+// EPI only, after TileSmem: the row's softmax statistics and its 32 attention gradients, which the logit gradient
+// needs together after the last level.  137 KB in all: one CTA per SM.
+struct TileSmemEpi {
+  float ga[kTileRows * 32];
+  float2 stat[kTileRows];                // max and sum of exp(logit - max) over the row's 32 logits
+  int refrow[kTileRows];                 // float2 index of the row's Z-anchor 0 in reference_points_cam
+};
+template <bool EPI>
+constexpr size_t tile_smem_bytes() { return sizeof(TileSmem) + (EPI ? sizeof(TileSmemEpi) : 0); }
+
+// grid: (batch element n, head h, tile) with the tile fastest; perm / nlive from the row-order kernels.
+// EPI: MSDeformableAttention3D's softmax and sampling-location prologue as in epi_decode, offset / logit gradients
+// accumulated into the per-pillar rows as in msda_backward_kernel<.., EPI, IDX>.
+template <bool EPI>
+__global__ void __launch_bounds__(kTileThreads, EPI ? 1 : 2)
+msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, const int* __restrict__ nlive,
+                          const float* __restrict__ grad_out, float* __restrict__ grad_value,
+                          float* __restrict__ grad_loc, float* __restrict__ grad_attn) {
+  constexpr int CV = 8, NG = 4, P = kTilePoints, NT = kTileThreads, RW = kTileRows / (NT / 32);   // RW rows per warp
+  extern __shared__ __align__(16) unsigned char tile_smem[];
+  TileSmem& sm = *reinterpret_cast<TileSmem*>(tile_smem);
+  TileSmemEpi& se = *reinterpret_cast<TileSmemEpi*>(tile_smem + sizeof(TileSmem));
+  __shared__ TileKeys tk;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int g = lane / CV, cl = lane % CV;
+  const int ntiles = (p.Q + kTileRows - 1) / kTileRows;
+  const int t = blockIdx.x % ntiles, nh = blockIdx.x / ntiles;
+  const int h = nh % p.H, n = nh / p.H;
+  const int nrows = min(kTileRows, __ldg(nlive + n) - t * kTileRows);
+  if (nrows <= 0) return;
+  const int b = n / p.ncl, c = p.cam0 + n % p.ncl;
+
+  // this warp's RW rows of the tile (4 per step, 8 lanes x float4 per head vector)
+  for (int i = 0; i < RW; i += 4) {
+    const int r = warp * RW + i + g;
+    float4 go = f4_zero();
+    int j = 0;
+    size_t q = 0, bq = 0;
+    if (r < nrows) {
+      j = __ldg(perm + (size_t)n * p.Q + t * kTileRows + r);
+      q = p.idx ? (size_t)__ldg(p.idx + (size_t)c * p.Qd + j) : (size_t)j;
+      bq = (size_t)b * p.Qd + q;
+      go = f4_scale(p.inv ? __ldg(p.inv + bq) : 1.f, ldg4(grad_out + (bq * p.H + h) * p.C + cl * 4));
+    }
+    if (cl == 0) {
+      sm.item[r] = r < nrows ? (int)(EPI ? bq * p.H + h : ((size_t)n * p.Q + j) * p.H + h) : -1;
+      if (EPI) se.refrow[r] = (int)((((size_t)c * p.bs + b) * p.Qd + q) * p.D);
+    }
+    sm.go[r * 8 + cl] = go;
+  }
+  if (threadIdx.x == 0) sm.slab = (size_t)n * p.K * p.pix_stride + (size_t)h * p.C;
+  __syncwarp();
+  if (EPI) {
+    // softmax statistics of each row, lane = sample (the warp_max / warp_sum of epi_decode, so the weights are
+    // bit-identical); rows past the last are at the warp's end
+    for (int i = 0; i < RW; ++i) {
+      const int item = sm.item[warp * RW + i];
+      if (item < 0) break;
+      const float logit = __ldg(p.attn + (size_t)item * p.LP + lane);
+      const float m = warp_max(logit);
+      const float sum = warp_sum(expf(logit - m));
+      if (lane == 0) se.stat[warp * RW + i] = make_float2(m, sum);
+    }
+  }
+  // the level loop reads the row items and the slab offset from shared memory: n, h and nrows need no registers there
+  __syncthreads();
+
+  const unsigned pix = (unsigned)p.pix_stride;
+  for (int l = 0; l < p.L; ++l) {
+    const size_t slab = sm.slab + cl * 4;
+    const float* vs = p.value + slab;
+    const int Hl = (int)__ldg(p.shapes + 2 * l), Wl = (int)__ldg(p.shapes + 2 * l + 1);
+    const int start = (int)__ldg(p.lsi + l);
+    const float fH = (float)Hl, fW = (float)Wl;
+    const int pb = 32 - __clz(Hl * Wl);             // pixel bits of the level's sort key
+    const unsigned none = (1u << pb) - 1;           // pixel field of an unused record: sorts last
+    // ---- row phase: a chunk is 4 rows x this level's 8 points, lane j decodes point j % 8 of row j / 8
+#pragma unroll 1
+    for (int ck = 0; ck < RW / 4; ++ck) {
+      const int r = warp * RW + ck * 4 + (lane >> 3);
+      const int item = sm.item[r];
+      const bool live = item >= 0;
+      size_t si = 0;   // sample index (row's item * L*P + l*P + point)
+      int base = 0, meta = 0;
+      float lh = 0.f, lw = 0.f, aw = 0.f;
+      float w1 = 0.f, w2 = 0.f, w3 = 0.f, w4 = 0.f;
+      if (live) {
+        si = (size_t)item * p.LP + l * P + (lane & 7);
+        float2 xy = __ldg(reinterpret_cast<const float2*>(p.loc) + si);
+        if (EPI) {
+          // epi_decode: w = softmax(logits), loc = offsets / (W, H) + reference_points_cam[p % D]
+          const float2 st = se.stat[r];
+          aw = __fdiv_rn(expf(__ldg(p.attn + si) - st.x), st.y);
+          const float2 rf = __ldg(reinterpret_cast<const float2*>(p.ref) + se.refrow[r] + (lane & 7) % p.D);
+          xy.x = __fadd_rn(__fdiv_rn(xy.x, fW), rf.x);
+          xy.y = __fadd_rn(__fdiv_rn(xy.y, fH), rf.y);
+        } else {
+          aw = __ldg(p.attn + si);
+        }
+        decode_sample(xy.x, xy.y, Hl, Wl, start, base, meta, lh, lw);   // base, dy in pixels
+        const float hh = 1.f - lh, hw = 1.f - lw;
+        w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
+        w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
+        w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
+        w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+      }
+      float r1 = 0.f, r2 = 0.f, r3 = 0.f, r4 = 0.f;
+#pragma unroll
+      for (int it = 0; it < CV; ++it) {
+        const int src = it * NG + g;
+        const int sbase = __shfl_sync(0xffffffffu, base, src);
+        const int smeta = __shfl_sync(0xffffffffu, meta, src);
+        const float4 go = sm.go[(warp * RW + ck * 4 + (it >> 1)) * 8 + cl];   // row of sample src
+        float d1 = 0.f, d2 = 0.f, d3 = 0.f, d4 = 0.f;
+        if (smeta & 15) {
+          const unsigned o1 = (unsigned)sbase * pix;
+          const unsigned o2 = o1 + ((smeta & 16) ? pix : 0u);
+          const unsigned o3 = o1 + (unsigned)(smeta >> 5) * pix;
+          const unsigned o4 = o3 + (o2 - o1);
+          d1 = f4_dot(go, ldg4(vs + o1));
+          d2 = f4_dot(go, ldg4(vs + o2));
+          d3 = f4_dot(go, ldg4(vs + o3));
+          d4 = f4_dot(go, ldg4(vs + o4));
+        }
+        // transposed reduction and hand-back, as in msda_backward_kernel
+        const bool up1 = (cl & (CV / 2)) != 0;
+        const float e0 = __shfl_xor_sync(0xffffffffu, up1 ? d1 : d3, CV / 2);
+        const float e1 = __shfl_xor_sync(0xffffffffu, up1 ? d2 : d4, CV / 2);
+        const float k0 = (up1 ? d3 : d1) + e0;
+        const float k1 = (up1 ? d4 : d2) + e1;
+        const bool up2 = (cl & (CV / 4)) != 0;
+        const float eb = __shfl_xor_sync(0xffffffffu, up2 ? k0 : k1, CV / 4);
+        float k = (up2 ? k1 : k0) + eb;
+#pragma unroll
+        for (int off = CV / 8; off >= 1; off >>= 1) k += __shfl_xor_sync(0xffffffffu, k, off);
+        const int back = (lane & (NG - 1)) * CV;
+        const float t1 = __shfl_sync(0xffffffffu, k, back);
+        const float t2 = __shfl_sync(0xffffffffu, k, back + CV / 4);
+        const float t3 = __shfl_sync(0xffffffffu, k, back + CV / 2);
+        const float t4 = __shfl_sync(0xffffffffu, k, back + CV / 2 + CV / 4);
+        if ((lane / NG) == it) { r1 = t1; r2 = t2; r3 = t3; r4 = t4; }
+      }
+      // this sample's 4 corner records: record = (row in tile, point, corner), key = level pixel << kRecBits | record
+      const unsigned rec = ((unsigned)(warp * RW + ck * 4) << 5) + lane * 4;
+      const unsigned px = (unsigned)(base - start), dx = (meta >> 4) & 1, dy = (unsigned)meta >> 5;
+      uint4 kk;
+      kk.x = (((meta & 1) ? px : none) << kRecBits) | rec;
+      kk.y = (((meta & 2) ? px + dx : none) << kRecBits) | (rec + 1);
+      kk.z = (((meta & 4) ? px + dy : none) << kRecBits) | (rec + 2);
+      kk.w = (((meta & 8) ? px + dy + dx : none) << kRecBits) | (rec + 3);
+      *reinterpret_cast<uint4*>(&tk.key[rec]) = kk;
+      *reinterpret_cast<float4*>(&sm.w[rec]) = make_float4(w1, w2, w3, w4);
+      if (live) {
+        const float hh = 1.f - lh, hw = 1.f - lw;
+        if (!(meta & 1)) r1 = 0.f;
+        if (!(meta & 2)) r2 = 0.f;
+        if (!(meta & 4)) r3 = 0.f;
+        if (!(meta & 8)) r4 = 0.f;
+        const bool ok = (meta & 15) != 0;
+        const float ga = ok ? (hh * hw) * r1 + (hh * lw) * r2 + (lh * hw) * r3 + (lh * lw) * r4 : 0.f;
+        const float gx = ok ? fW * aw * (hh * (r2 - r1) + lh * (r4 - r3)) : 0.f;
+        const float gy = ok ? fH * aw * (hw * (r3 - r1) + lw * (r4 - r2)) : 0.f;
+        if (EPI) {
+          // offsets are shared by every camera that sees the pillar: accumulate (caller zeroes); the logit
+          // gradient waits for the row's other levels
+          se.ga[r * 32 + l * P + (lane & 7)] = ga;
+          red_add_v2(grad_loc + 2 * si, __fdiv_rn(gx, fW), __fdiv_rn(gy, fH));
+        } else {
+          grad_attn[si] = ga;
+          reinterpret_cast<float2*>(grad_loc)[si] = make_float2(gx, gy);
+        }
+      }
+    }
+    __syncthreads();
+
+    // ---- tile phase: sort the level's records by pixel (stable, so the summation order is fixed)
+    unsigned keys[kTileItems];
+#pragma unroll
+    for (int i = 0; i < kTileItems; ++i) keys[i] = tk.key[i * NT + threadIdx.x];
+    __syncthreads();   // the sort's temp storage aliases key[]
+    TileSort(tk.sort).SortBlockedToStriped(keys, kRecBits, kRecBits + pb);
+    __syncthreads();
+    // sorted position R = i*NT + tid is stored at R + R / kTileSeg (the pad keeps the 4 groups of a warp on
+    // different banks)
+#pragma unroll
+    for (int i = 0; i < kTileItems; ++i) {
+      const int R = i * NT + threadIdx.x;
+      tk.key[R + R / kTileSeg] = keys[i];
+    }
+    __syncthreads();
+
+    // group G (8 lanes x float4 = one head vector) sums the runs of sorted positions [G*kTileSeg, (G+1)*kTileSeg):
+    // one 128-byte reduction per pixel run (a run split between two groups is reduced twice)
+    float* gl = grad_value + slab + (size_t)start * pix;
+    asm volatile("" : "+l"(gl));   // computed here, not kept live through the sort (64-register budget)
+    const unsigned* ks = tk.key + (warp * NG + g) * (kTileSeg + 1);
+    // records are read 4 at a time so that their shared-memory loads overlap; unused records (pixel `none`, weight 0)
+    // sort last and accumulate into a run that is never reduced
+    unsigned cur = none;
+    float4 acc = f4_zero();
+    for (int i0 = 0; i0 < kTileSeg; i0 += 4) {
+      unsigned kq[4];
+      float wq[4];
+      float4 gq[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) kq[u] = ks[i0 + u];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const unsigned rec = kq[u] & (kTileRecs - 1);
+        wq[u] = sm.w[rec];
+        gq[u] = sm.go[(rec >> 5) * 8 + cl];
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const unsigned kp = kq[u] >> kRecBits;
+        if (kp != cur) {
+          if (cur != none) red_add_v4(gl + cur * pix, acc);
+          cur = kp;
+          acc = f4_zero();
+        }
+        f4_fma(acc, wq[u], gq[u]);
+      }
+      if (cur == none) break;
+    }
+    if (cur != none) red_add_v4(gl + cur * pix, acc);
+    __syncthreads();   // key[] / w[] are rewritten by the next level
+  }
+  if (EPI) {
+    // grad_logit = w * (grad_w - sum_j w_j grad_w_j), lane = sample as in msda_backward_kernel
+    for (int i = 0; i < RW; ++i) {
+      const int r = warp * RW + i;
+      const int item = sm.item[r];
+      if (item < 0) break;
+      const size_t si = (size_t)item * p.LP + lane;
+      const float2 st = se.stat[r];
+      const float aw = __fdiv_rn(expf(__ldg(p.attn + si) - st.x), st.y);
+      const float ga = se.ga[r * 32 + lane];
+      const float dot = warp_sum(aw * ga);
+      red_add_f32(grad_attn + si, aw * (ga - dot));
+    }
+  }
+}
+
 #include "msda_slab.cuh"
 
 // ---- generic fallback (any C): one thread per (item, channel); scalar atomics.
@@ -911,6 +1287,84 @@ inline bool slab_forward_on() {
   return v;
 }
 
+// The tile-aggregating rows backward: C = 32, 8 points on each of 4 levels (SpatialCrossAttention).
+// A level's pixel index and the record index share a 32-bit sort key.
+inline bool tile_backward_ok(const MsdaParams& p) {
+  return p.C == 32 && p.P == kTilePoints && p.LP == 32 && p.K < (1 << (32 - kRecBits));
+}
+
+// The row order's scratch comes from a memory pool of this library that keeps what it has allocated (release
+// threshold = max): eager training does not pay a fresh physical allocation per backward, and the device's
+// default pool, which the rest of the process may use, keeps its settings.
+inline cudaError_t scratch_pool(cudaMemPool_t* pool) {
+  static std::mutex mu;
+  static cudaMemPool_t pools[128] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 128) return cudaErrorInvalidDevice;
+  std::lock_guard<std::mutex> lock(mu);
+  if (!pools[dev]) {
+    cudaMemPoolProps props = {};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = dev;
+    cudaMemPool_t p = nullptr;
+    e = cudaMemPoolCreate(&p, &props);
+    if (e != cudaSuccess) return e;
+    uint64_t keep = UINT64_MAX;
+    e = cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &keep);
+    if (e != cudaSuccess) {
+      cudaMemPoolDestroy(p);
+      return e;
+    }
+    pools[dev] = p;
+  }
+  *pool = pools[dev];
+  return cudaSuccess;
+}
+
+// Row order + tile kernel.  The order's scratch (two ints per row and a cell histogram per 1024 rows) is
+// stream-ordered (cudaMallocFromPoolAsync / cudaFreeAsync): no host sync, and a CUDA graph captures it as
+// allocation nodes, so the C signature needs no workspace argument.
+template <bool EPI>
+int launch_rows_backward_tiled(const MsdaParams& p, const float* grad_out, float* grad_value, float* grad_loc,
+                               float* grad_attn, cudaStream_t st, const char* who) {
+  const int nch = (p.Q + kOrderChunk - 1) / kOrderChunk;
+  const long long ntiles = (p.Q + kTileRows - 1) / kTileRows;
+  const long long nb = (long long)p.B * p.H * ntiles;
+  VIDAR_REQUIRE(nb < 2147483647LL && p.B < 65536, "%s: problem too large", who);
+  // row items and Z-anchor rows are 32-bit in the tile kernel
+  VIDAR_REQUIRE(!EPI || ((long long)p.bs * p.Qd * p.H < (1LL << 31) &&
+                         (long long)(p.cam0 + p.ncl) * p.bs * p.Qd * p.D < (1LL << 31)),
+                "%s: problem too large", who);
+  // the row order reads head 0's sampling locations as float4
+  VIDAR_REQUIRE(EPI || ((uintptr_t)p.loc & 15u) == 0, "%s: sampling_loc must be 16-byte aligned", who);
+  const size_t smem = tile_smem_bytes<EPI>();
+  if (cudaFuncSetAttribute(msda_backward_tile_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+      cudaSuccess)
+    return set_error(VIDAR_E_CUDA, "%s: cannot opt in to %zu bytes of shared memory", who, smem);
+  cudaMemPool_t pool;
+  cudaError_t e = scratch_pool(&pool);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: scratch memory pool: %s", who, cudaGetErrorString(e));
+  const size_t nkey = (size_t)p.B * p.Q, nhist = (size_t)p.B * nch * kCells;
+  int* scratch = nullptr;
+  e = cudaMallocFromPoolAsync((void**)&scratch, sizeof(int) * (2 * nkey + nhist + p.B), pool, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cudaMallocFromPoolAsync: %s", who, cudaGetErrorString(e));
+  int* key = scratch;
+  int* perm = key + nkey;
+  int* hist = perm + nkey;
+  int* nlive = hist + nhist;
+  rows_key_kernel<EPI><<<dim3(nch, p.B), kOrderChunk, 0, st>>>(p, key, hist);
+  rows_scan_kernel<<<p.B, kCells, 0, st>>>(hist, nlive, nch);
+  rows_scatter_kernel<<<dim3(nch, p.B), kOrderChunk, 0, st>>>(key, hist, perm, p.Q);
+  msda_backward_tile_kernel<EPI><<<(unsigned)nb, kTileThreads, smem, st>>>(p, perm, nlive, grad_out, grad_value,
+                                                                           grad_loc, grad_attn);
+  e = cudaFreeAsync(scratch, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cudaFreeAsync: %s", who, cudaGetErrorString(e));
+  return check_launch(who);
+}
+
 }  // namespace
 }  // namespace vidar
 
@@ -1128,6 +1582,8 @@ extern "C" int vidar_msda_rows_backward(const float* value, const int64_t* spati
   p.na_bytes = 0xffffffffu;
   if (slab_ok(p))
     return launch_slab_backward<false, true>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, (cudaStream_t)stream, who);
+  if (tile_backward_ok(p))
+    return launch_rows_backward_tiled<false>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, (cudaStream_t)stream, who);
   VIDAR_ROWS_LAUNCH(msda_backward_kernel, false, p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight);
   return check_launch(who);
 }
@@ -1170,6 +1626,8 @@ extern "C" int vidar_msda_sca_rows_backward(const float* value, const int64_t* s
   p.na_bytes = 0xffffffffu;
   if (slab_ok(p))
     return launch_slab_backward<true, true>(p, grad_slots, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
+  if (tile_backward_ok(p))
+    return launch_rows_backward_tiled<true>(p, grad_slots, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
   VIDAR_ROWS_LAUNCH(msda_backward_kernel, true, p, grad_slots, grad_value, grad_offsets, grad_logits);
   return check_launch(who);
 }
