@@ -15,6 +15,9 @@ Two independent statements are given:
   * `msda_explicit`     -- the per-corner formulation the CUDA kernels follow
     (SURVEY.md A.1: pixel = loc*size - 0.5, four individually zero-padded corners,
     analytic gradients), in numpy float64.
+On top of `msda_grid_sample`, `msda_rows` / `msda_sca_rows` state SpatialCrossAttention's row map (per-camera
+visible-pillar lists scattered into the BEV slots), the operation of the vidar_msda_rows_* / vidar_msda_sca_rows_*
+entry points.
 Pinning: tests/test_oracle_msda.py checks both against each other and against the
 same-lineage implementation shipped in `transformers`
 (`transformers.models.deformable_detr.modeling_deformable_detr`), which is present in this
@@ -57,6 +60,77 @@ def msda_grid_sample_backward(value, spatial_shapes, sampling_locations, attenti
     out = msda_grid_sample(v, spatial_shapes, loc, aw)
     out.backward(grad_output.to(dtype))
     return v.grad, loc.grad, aw.grad
+
+
+def _rows_into_slots(slots, group, bs, rows_out, idx, count, inv):
+    """Add the live rows of one launch group into slots [bs, Qd, H*C].  rows_out [bs*ncl, rows, H*C]: row j of
+    batch element n = b*ncl + camera.  Rows that are not live (j >= count[cam], or (j // 64) % S outside
+    [s_lo, s_hi)) add nothing; the others go to pillar idx[cam, j] (j without a list), scaled by inv[b, q]."""
+    cam0, ncl, S, lo, hi = group
+    dev = rows_out.device
+    rows = rows_out.shape[1]
+    j = torch.arange(rows, device=dev)
+    n = torch.arange(bs * ncl, device=dev)
+    b, cam = n // ncl, cam0 + n % ncl
+    live = (((j // 64) % S >= lo) & ((j // 64) % S < hi)).expand(bs * ncl, rows)
+    if count is not None:
+        live = live & (j[None] < count.to(dev).long()[cam][:, None])
+    q = idx.to(dev)[cam][:, :rows].long() if idx is not None else j.expand(bs * ncl, rows)
+    bb = b[:, None].expand(bs * ncl, rows)
+    out = rows_out[live]
+    if inv is not None:
+        out = out * inv.to(device=dev, dtype=out.dtype)[bb[live], q[live]][:, None]
+    return slots.index_put((bb[live], q[live]), out, accumulate=True)
+
+
+def msda_rows(plan, bs, Qd, spatial_shapes, idx, count, inv, groups):
+    """The row map of `MSDARowsFunction` (SpatialCrossAttention's rebatch + scatter-add around the op) in
+    differentiable torch: autograd gives every gradient, on any device and dtype.
+    plan [(cam0, ncl, S, s_lo, s_hi)]; groups [(value [bs*ncl, K, H, C], loc [bs*ncl, rows, H, L, P, 2],
+    attn [bs*ncl, rows, H, L, P])] per launch group; idx [cams, Qd] | None; count [cams] | None;
+    inv [bs, Qd] | None  ->  slots [bs, Qd, H*C]."""
+    H, C = groups[0][0].shape[2:]
+    slots = groups[0][0].new_zeros(bs, Qd, H * C)
+    for group, (v, loc, aw) in zip(plan, groups):
+        slots = _rows_into_slots(slots, group, bs, msda_grid_sample(v, spatial_shapes, loc, aw), idx, count, inv)
+    return slots
+
+
+def sca_locations(spatial_shapes, offsets, ref):
+    """MSDeformableAttention3D's sampling locations in its own fp32 statements (spatial_cross_attention.py:356-371):
+    offsets [..., H, L, P, 2] / (W_l, H_l) + ref [..., D, 2] at Z-anchor p % D.  Returned in offsets' dtype with
+    d(loc)/d(offsets) = 1 / (W_l, H_l), but with the fp32 value, which the fused kernels reproduce bit for bit."""
+    shapes = torch.as_tensor(spatial_shapes).to(offsets.device)
+    L, P, D = offsets.shape[-3], offsets.shape[-2], ref.shape[-2]
+    lead = offsets.shape[:-4]
+    H = offsets.shape[-4]
+    wh32 = torch.stack([shapes[:, 1], shapes[:, 0]], -1).float()
+    o32 = offsets.detach().float()
+    r32 = ref.detach().float().reshape(*lead, 1, 1, 1, D, 2)
+    loc32 = ((o32 / wh32.view(L, 1, 2)).view(*lead, H, L, P // D, D, 2) + r32).view(*lead, H, L, P, 2)
+    wh = wh32.to(offsets.dtype).view(L, 1, 2)
+    return loc32.to(offsets.dtype) + (offsets - offsets.detach()) / wh
+
+
+def msda_sca_rows(plan, bs, spatial_shapes, idx, count, inv, ref_cam, offsets, logits, values):
+    """The fused row map of `SCARowsFunction`: offsets [bs, Qd, H, L, P, 2] and logits [bs, Qd, H, L*P] are dense
+    per pillar and gathered through idx for every (camera, row); ref_cam [cams, bs, Qd, D, 2].  Locations from
+    `sca_locations`, softmax and sampling in the inputs' dtype.  values[g] [bs*ncl, K, H, C] -> slots [bs, Qd, H*C];
+    autograd gives the per-pillar offset / logit gradients summed over cameras."""
+    _, Qd, H, L, P, _ = offsets.shape
+    C = values[0].shape[-1]
+    slots = offsets.new_zeros(bs, Qd, H * C)
+    for (cam0, ncl, S, lo, hi), v in zip(plan, values):
+        n = torch.arange(bs * ncl, device=offsets.device)
+        b, cam = n // ncl, cam0 + n % ncl
+        q = idx.to(offsets.device)[cam].long() if idx is not None else torch.arange(Qd, device=offsets.device).expand(bs * ncl, Qd)
+        q = q.clamp(0, Qd - 1)            # list entries past count are undefined; those rows are masked below
+        bb = b[:, None].expand_as(q)
+        loc = sca_locations(spatial_shapes, offsets[bb, q], ref_cam.to(offsets.device)[cam[:, None], bb, q])
+        w = logits[bb, q].softmax(-1).view(bs * ncl, Qd, H, L, P)
+        slots = _rows_into_slots(slots, (cam0, ncl, S, lo, hi), bs, msda_grid_sample(v, spatial_shapes, loc, w),
+                                 idx, count, inv)
+    return slots
 
 
 def msda_explicit(value, spatial_shapes, level_start_index, sampling_locations,

@@ -215,7 +215,8 @@ def test_fused_sca_epilogue_rejects_other_shapes(cuda):
 @pytest.mark.parametrize("mode,fwd", [("1", "0"), ("2", "1")], ids=["slab-plain", "slab-tma+fwd"])
 def test_slab_variants(cuda, mode, fwd):
     """The persistent shared-memory variants (csrc/msda_slab.cuh; off by default, selected by environment
-    variables read once per process) against the oracle, in a subprocess: SCA shape, plain op."""
+    variables read once per process) against the oracle, in a subprocess: SCA shape, plain op and both row-map
+    functions."""
     import os
     import subprocess
     import sys
@@ -240,6 +241,9 @@ for mode_, Q in (("local", 333), ("stress", 150)):
     parity.close(ga, rga, "grad_attn")
     keep = parity.off_kink(d["loc"], d["shapes"])
     parity.close(gl, rgl, "grad_loc", keep=keep.unsqueeze(-1).expand_as(rgl))
+# the row map (vidar_msda_rows_* / vidar_msda_sca_rows_*) on the same variants
+from tests.test_msda_rows_gpu import slab_row_cases
+slab_row_cases(dev)
 print("SLAB-OK")
 """
     env = dict(os.environ, VIDAR_MSDA_SLAB=mode, VIDAR_MSDA_SLAB_FWD=fwd, PYTHONPATH=root)
