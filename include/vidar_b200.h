@@ -329,6 +329,7 @@ int vidar_latent_render_backward(const float* occ, const float* feat, const floa
 /* The same four kernels, one phase per call, on a range [cell0, cell0+ncells) of the
  * bs*Hb*Wb BEV cells (row-major): when the cells are sharded over GPUs the host places a
  * collective on the small maps between the phases (vidar_b200/modules/latent_rendering.py).
+ * A range with cell0 < 0, ncells < 0 or cell0 + ncells > bs*Hb*Wb is rejected.
  * Outputs are indexed by GLOBAL cell; scatter targets (grad_*) are caller-zeroed full maps
  * that receive this range's contributions. */
 int vidar_latent_prob_forward(const float* occ, float* prob, float* aux, int bs, int D, int Hb,

@@ -455,7 +455,7 @@ latent_pool_bwd_kernel(LrDims L, const float* __restrict__ prob, const float* __
 }
 
 int check_lr(LrDims& L, int bs, int D, int G, int Hb, int Wb, int grid_num, float grid_step, float eps,
-             int act, int& vec, const char* who, long long cell0 = 0, long long ncells = -1) {
+             int act, int& vec, const char* who, long long cell0, long long ncells) {
   VIDAR_REQUIRE(bs > 0 && D > 0 && G > 0 && Hb > 1 && Wb > 1 && grid_num > 0,
                 "%s: bad sizes bs=%d D=%d G=%d Hb=%d Wb=%d grid_num=%d", who, bs, D, G, Hb, Wb, grid_num);
   VIDAR_REQUIRE(act == 0 || act == 1, "Only support exp or sigmoid activation_fn for now.");
@@ -467,9 +467,8 @@ int check_lr(LrDims& L, int bs, int D, int G, int Hb, int Wb, int grid_num, floa
   vec = (D % 4 == 0 && G <= 4) ? 4 : 1;   // a lane keeps VEC*G accumulators in registers
   const int half = (Hb < Wb ? Hb : Wb) / 2;
   const long long total = (long long)bs * Hb * Wb;
-  if (ncells < 0) ncells = total - cell0;
-  VIDAR_REQUIRE(cell0 >= 0 && ncells >= 0 && cell0 + ncells <= total, "%s: bad cell range [%lld, +%lld) of %lld",
-                who, cell0, ncells, total);
+  VIDAR_REQUIRE(cell0 >= 0 && ncells >= 0 && cell0 <= total && ncells <= total - cell0,
+                "%s: bad cell range [%lld, +%lld) of %lld", who, cell0, ncells, total);
   L = LrDims{bs, D, G, Hb, Wb, grid_num, act, (float)((double)grid_step / (double)half), eps, cell0, ncells};
   return VIDAR_OK;
 }
@@ -548,7 +547,8 @@ extern "C" int vidar_latent_render_forward(const float* occ, const float* feat, 
                                            float grid_step, float eps, int act, void* stream) {
   LrDims L;
   int vec;
-  int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, act, vec, "LatentRendering.forward");
+  int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, act, vec, "LatentRendering.forward", 0,
+                    (long long)bs * Hb * Wb);
   if (rc) return rc;
   VIDAR_REQUIRE(occ && feat && prob && pooled, "LatentRendering.forward: null pointer argument");
   rc = prob_fwd(L, vec, occ, prob, aux, (cudaStream_t)stream);
@@ -563,7 +563,8 @@ extern "C" int vidar_latent_render_backward(const float* occ, const float* feat,
                                             int grid_num, float grid_step, float eps, int act, void* stream) {
   LrDims L;
   int vec;
-  int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, act, vec, "LatentRendering.backward");
+  int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, act, vec, "LatentRendering.backward", 0,
+                    (long long)bs * Hb * Wb);
   if (rc) return rc;
   VIDAR_REQUIRE(occ && feat && prob && grad_prob && grad_pooled && grad_prob_total && grad_occ && grad_feat,
                 "LatentRendering.backward: null pointer argument");
