@@ -14,6 +14,13 @@ char* err_buf();
 int set_error(int code, const char* fmt, ...);
 extern std::atomic<int64_t> g_launches;
 
+// Stream-ordered scratch (cudaMallocFromPoolAsync / cudaFreeAsync) for the MSDA row order and the LatentRendering
+// cell order comes from this memory pool of the library, one per device.  It keeps what it has allocated (release
+// threshold = max): eager training does not pay a fresh physical allocation per backward, and the device's default
+// pool, which the rest of the process may use, keeps its settings.  No host sync, and a CUDA graph captures the
+// allocations as nodes, so the C signatures need no workspace argument.
+cudaError_t scratch_pool(cudaMemPool_t* pool);
+
 inline int check_launch(const char* what) {
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();

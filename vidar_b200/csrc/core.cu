@@ -2,6 +2,8 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <mutex>
+
 #include "common.cuh"
 
 namespace vidar {
@@ -19,6 +21,34 @@ int set_error(int code, const char* fmt, ...) {
   vsnprintf(err_buf(), 512, fmt, ap);
   va_end(ap);
   return code;
+}
+
+cudaError_t scratch_pool(cudaMemPool_t* pool) {
+  static std::mutex mu;
+  static cudaMemPool_t pools[128] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 128) return cudaErrorInvalidDevice;
+  std::lock_guard<std::mutex> lock(mu);
+  if (!pools[dev]) {
+    cudaMemPoolProps props = {};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = dev;
+    cudaMemPool_t p = nullptr;
+    e = cudaMemPoolCreate(&p, &props);
+    if (e != cudaSuccess) return e;
+    uint64_t keep = UINT64_MAX;
+    e = cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &keep);
+    if (e != cudaSuccess) {
+      cudaMemPoolDestroy(p);
+      return e;
+    }
+    pools[dev] = p;
+  }
+  *pool = pools[dev];
+  return cudaSuccess;
 }
 
 }  // namespace vidar

@@ -25,7 +25,13 @@
 // behind a mask.  Products / sums over waypoints are finished with warp shuffles; only
 // prob (D floats) and pooled (D*g floats) are written per cell.  Backward kernels recompute
 // the forward quantities and scatter with vector reductions.
+// Backward dispatch, by shape: the phase 2 backward with VEC 4 and G 1 (every D in {4, 8, 16, 32} with one
+// feature channel per height, the shipped configuration) runs in angular bundles that sum their scatter in
+// shared memory (latent_pool_bwd_bundle_kernel); other VEC / G and the phase 1 backward use the per-cell kernels.
+#include <limits.h>
 #include <math.h>
+
+#include <cub/device/device_radix_sort.cuh>
 
 #include "common.cuh"
 
@@ -43,21 +49,39 @@ struct Bil {
   float w[4];    // nw, ne, sw, se
 };
 
-__device__ __forceinline__ Bil bilinear_setup(float gx, float gy, int Hb, int Wb) {
-  Bil b;
+struct BilXY {
+  int x0, y0;    // pixel of the nw corner (may lie outside the map)
+  float w[4];    // nw, ne, sw, se
+};
+
+__device__ __forceinline__ BilXY bilinear_xy(float gx, float gy, int Hb, int Wb) {
+  BilXY q;
   // grid_sample: ((g + 1) * size - 1) / 2 ; the division by 2 is exact, so x 0.5 gives the same bits
   const float ix = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)Wb), 1.f), 0.5f);
   const float iy = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)Hb), 1.f), 0.5f);
   const float fx = floorf(ix), fy = floorf(iy);
-  const int x0 = (int)fx, y0 = (int)fy;
+  q.x0 = (int)fx;
+  q.y0 = (int)fy;
   const float wx1 = ix - fx, wy1 = iy - fy;
   const float wx0 = (fx + 1.f) - ix, wy0 = (fy + 1.f) - iy;
 #pragma unroll
+  for (int j = 0; j < 4; ++j) q.w[j] = ((j & 1) ? wx1 : wx0) * ((j & 2) ? wy1 : wy0);
+  return q;
+}
+
+// corner j of a footprint: pixel index, or -1 outside the map
+__device__ __forceinline__ int corner_pixel(int x0, int y0, int j, int Hb, int Wb) {
+  const int xx = x0 + (j & 1), yy = y0 + (j >> 1);
+  return (xx >= 0 && xx < Wb && yy >= 0 && yy < Hb) ? yy * Wb + xx : -1;
+}
+
+__device__ __forceinline__ Bil bilinear_setup(float gx, float gy, int Hb, int Wb) {
+  const BilXY q = bilinear_xy(gx, gy, Hb, Wb);
+  Bil b;
+#pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const int xx = x0 + (j & 1), yy = y0 + (j >> 1);
-    const bool in = xx >= 0 && xx < Wb && yy >= 0 && yy < Hb;
-    b.o[j] = in ? yy * Wb + xx : -1;
-    b.w[j] = ((j & 1) ? wx1 : wx0) * ((j & 2) ? wy1 : wy0);
+    b.o[j] = corner_pixel(q.x0, q.y0, j, Hb, Wb);
+    b.w[j] = q.w[j];
   }
   return b;
 }
@@ -454,6 +478,265 @@ latent_pool_bwd_kernel(LrDims L, const float* __restrict__ prob, const float* __
   }
 }
 
+// ---------------------------------------------------------------- phase 2 backward in angular bundles (VEC 4, G 1)
+// latent_pool_bwd_kernel sends one 16-byte reduction per (cell, waypoint, corner, float4, map): 18.3 M 64-byte
+// lines per map at 200 x 200 with grid_num 256.  Every ray starts at the BEV centre and waypoint k of
+// every ray lies ~k px from it, so the cells sorted by the direction of their ray and cut into bundles of
+// kBundle consecutive cells put their kBundle footprints of one waypoint inside a kBox x kBox pixel box
+// (a 4 x 4 box holds every bundle of 32 at 200 x 200).  A bundle kernel sums the bundle's contributions to
+// each box pixel in shared memory, in a fixed cell order, and sends one reduction per touched pixel and map:
+// 0.67 M lines per map at the bench shape.  A corner outside its box (bundles across the +-pi cut, the centre
+// cell, small BEVs, a bundle's cells of a second batch element) is reduced straight to global memory as in the
+// per-cell kernel.  The phase 1 backward keeps its per-cell kernel: its rays end at their own cell, so a
+// bundle of cells at every radius along one direction spends most of its waypoints on finished cells, and the
+// bundled form measured slower than the per-cell one (DESIGN.md 4.3).
+constexpr int kBundle = 32;                                 // cells per bundle = lanes of a warp
+constexpr int kBundleThreads = 256;
+constexpr int kChunk = kBundleThreads / kBundle;            // waypoints staged in shared memory at a time
+constexpr int kBox = 4;
+constexpr int kAngleBits = 20;                              // angle bins of the cell order
+constexpr int kNoCorner = -(1 << 29);                       // footprint slot of a (waypoint, cell) with no sample
+
+// Cell order, key: batch element (relative to the range's first) above the angle bin of the cell's direction from
+// the BEV centre, taken from its integer position so that it is exact on any BEV shape.
+__global__ void __launch_bounds__(256) latent_order_key_kernel(LrDims L, unsigned long long* __restrict__ key,
+                                                                int* __restrict__ idx) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L.ncells) return;
+  const int HW = L.Hb * L.Wb;
+  const long long cell = L.cell0 + i;
+  const int u = (int)(cell % HW), iy = u / L.Wb, ix = u % L.Wb;
+  const float a = atan2f((float)(2 * iy + 1 - L.Hb), (float)(2 * ix + 1 - L.Wb));   // [-pi, pi]
+  const float pi = 3.14159265358979f;
+  const int bin = min(max((int)((a + pi) * ((float)(1 << kAngleBits) / (2.f * pi))), 0), (1 << kAngleBits) - 1);
+  key[i] = ((unsigned long long)(cell / HW - L.cell0 / HW) << kAngleBits) | (unsigned)bin;
+  idx[i] = (int)i;
+}
+
+// Shared memory of a bundle CTA: the fixed part, then per-height coefficient rows and the staged vectors.
+struct BundleSmem {
+  Cell cg[kBundle];
+  int kend[kBundle], kchk[kBundle], bat[kBundle];   // bat: batch element, -1 past the range
+  int2 xy[kChunk][kBundle];                         // nw corner pixel of (waypoint, cell); kNoCorner = no sample
+  float4 w[kChunk][kBundle];                        // bilinear weights
+  int2 box[kChunk];                                 // box origin of each waypoint; INT_MAX = empty
+  unsigned who[kChunk][kBox * kBox];                // cells with a corner on each box pixel
+  unsigned direct[kChunk];                          // cells with a corner the box does not cover
+};
+// then the gN, gS rows [2][kBundle][D] and the grad_feat, grad_prob_map vectors [2][kChunk][kBundle][D]
+inline size_t bundle_smem_bytes(int D) {
+  return sizeof(BundleSmem) + sizeof(float) * (size_t)D * kBundle * (2 + 2 * kChunk);
+}
+
+// latent_pool_bwd_kernel<4, 1> on the cells of `order`, one CTA per kBundle consecutive ones.  map0 = prob,
+// grad_in = grad_pooled, out0 = grad_feat, out1 = grad_prob_map; aux0 / aux1 = the forward's S and pooled, or
+// NULL to re-march.  prologue: a warp per cell forms gN and gS as latent_pool_bwd_kernel does.  Then per chunk of
+// kChunk waypoints:
+//   A1  thread = (waypoint, cell): waypoint, mask, bilinear footprint; the box origin is the warp's minimum
+//       corner; ballots give each box pixel's cells and the cells with a corner outside the box.
+//   A2  thread = (waypoint, cell, float4): gathers of prob and feat, gN pg and gS + gN f into shared memory.
+//   B   corners outside the box are reduced to global memory; thread = (waypoint, box pixel, float4) sums the
+//       pixel's cells in cell order and sends one reduction per touched pixel and map.
+__global__ void __launch_bounds__(kBundleThreads, 4)
+latent_pool_bwd_bundle_kernel(LrDims L, const int* __restrict__ order, const float* __restrict__ map0,
+                              const float* __restrict__ feat, const float* __restrict__ grad_in,
+                              float* __restrict__ out0, float* __restrict__ out1, const float* __restrict__ aux0,
+                              const float* __restrict__ aux1) {
+  constexpr int VEC = 4;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  BundleSmem& sm = *reinterpret_cast<BundleSmem*>(smem_raw);
+  float* rows = reinterpret_cast<float*>(smem_raw + sizeof(BundleSmem));   // [rows][kBundle][D]
+  float* vec = rows + 2 * kBundle * L.D;                                    // [2][kChunk][kBundle][D]
+  const int D = L.D, LPW = D / VEC, WPI = 32 / LPW, HW = L.Hb * L.Wb;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int slot = lane / LPW, ch = (lane % LPW) * VEC;
+
+  // ---- prologue: warp per cell
+  for (int c = warp; c < kBundle; c += kBundleThreads / 32) {
+    const long long pos = (long long)blockIdx.x * kBundle + c;
+    if (pos >= L.ncells) {
+      if (lane == 0) { sm.kend[c] = 0; sm.bat[c] = -1; }
+      continue;
+    }
+    const long long cell = L.cell0 + __ldg(order + pos);
+    const int b = (int)(cell / HW), u = (int)(cell % HW);
+    const Cell cg = cell_geometry(L, u / L.Wb, u % L.Wb);
+    const size_t o = ((size_t)b * HW + u) * D + ch;
+    {   // pooled_c = N_c / (S_d + eps)
+      float S[VEC], N[VEC];
+      if (aux0) {
+        V<VEC>::ld(aux0 + o, S);
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) N[v] = __ldg(aux1 + o + v) * (S[v] + L.eps);
+      } else {
+        pool_accumulate<VEC, 1>(L, cg, map0 + (size_t)b * HW * D, feat + (size_t)b * HW * D, ch, slot, WPI, S, N);
+#pragma unroll
+        for (int v = 0; v < VEC; ++v)
+          for (int off = LPW; off < 32; off <<= 1) {
+            S[v] += __shfl_xor_sync(0xffffffffu, S[v], off);
+            N[v] += __shfl_xor_sync(0xffffffffu, N[v], off);
+          }
+      }
+      float gN[VEC], gS[VEC];
+#pragma unroll
+      for (int v = 0; v < VEC; ++v) {
+        const float inv = 1.f / (S[v] + L.eps);
+        const float gpc = __ldg(grad_in + o + v);
+        gN[v] = gpc * inv;
+        gS[v] = 0.f;
+        gS[v] -= gpc * N[v] * inv * inv;
+      }
+      if (slot == 0) {
+        V<VEC>::st(rows + c * D + ch, gN);
+        V<VEC>::st(rows + (kBundle + c) * D + ch, gS);
+      }
+      if (lane == 0) {
+        sm.kend[c] = march_end(L, cg.boundary);
+        sm.kchk[c] = march_check(L, cg.boundary);
+      }
+    }
+    if (lane == 0) {
+      sm.cg[c] = cg;
+      sm.bat[c] = b;
+    }
+  }
+  __syncthreads();
+  int kmax = 0;
+  for (int c = 0; c < kBundle; ++c) kmax = max(kmax, sm.kend[c]);
+  const int b0 = sm.bat[0];
+  float* const o0 = out0 + (size_t)b0 * HW * D;
+  float* const o1 = out1 + (size_t)b0 * HW * D;
+
+  for (int k0 = 0; k0 < kmax; k0 += kChunk) {
+    // ---- A1: thread = (waypoint kk = warp, cell c = lane)
+    {
+      const int kk = warp, c = lane, k = k0 + kk;
+      float gx, gy;
+      const bool live = k < sm.kend[c] && waypoint(L, sm.cg[c], k, sm.kchk[c], sm.cg[c].boundary, gx, gy);
+      int2 xy = make_int2(kNoCorner, kNoCorner);
+      if (live) {
+        const BilXY q = bilinear_xy(gx, gy, L.Hb, L.Wb);
+        xy = make_int2(q.x0, q.y0);
+        sm.w[kk][c] = make_float4(q.w[0], q.w[1], q.w[2], q.w[3]);
+      }
+      sm.xy[kk][c] = xy;
+      const bool boxed = live && sm.bat[c] == b0;
+      const int bx = __reduce_min_sync(0xffffffffu, boxed ? xy.x : INT_MAX);
+      const int by = __reduce_min_sync(0xffffffffu, boxed ? xy.y : INT_MAX);
+      if (lane == 0) sm.box[kk] = make_int2(bx, by);
+      // cells of each box pixel: bit c of who[kk][p] = corner (p % kBox - dx, p / kBox - dy) of cell c
+      const int dx = boxed ? xy.x - bx : 0, dy = boxed ? xy.y - by : 0;
+      bool direct = live && !boxed;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        direct |= boxed && corner_pixel(xy.x, xy.y, j, L.Hb, L.Wb) >= 0 &&
+                  (dx + (j & 1) >= kBox || dy + (j >> 1) >= kBox);
+      const unsigned dm = __ballot_sync(0xffffffffu, direct);
+      if (lane == 0) sm.direct[kk] = dm;
+#pragma unroll
+      for (int p = 0; p < kBox * kBox; ++p) {
+        const int px = p % kBox - dx, py = p / kBox - dy;
+        const bool in = boxed && px >= 0 && px <= 1 && py >= 0 && py <= 1;
+        const unsigned m = __ballot_sync(0xffffffffu, in);
+        if (lane == p) sm.who[kk][p] = m;
+      }
+    }
+    __syncthreads();
+    // ---- A2: thread = (waypoint, cell, float4); lanes of one cell adjacent, so a corner is one 64-byte line
+#pragma unroll 4
+    for (int i = threadIdx.x; i < kChunk * kBundle * LPW; i += kBundleThreads) {
+      const int l = i % LPW, c = (i / LPW) % kBundle, kk = i / (LPW * kBundle);
+      const int2 xy = sm.xy[kk][c];
+      if (xy.x == kNoCorner) continue;
+      const int b = sm.bat[c], chl = l * VEC;
+      const float4 w4 = sm.w[kk][c];
+      const float wj[4] = {w4.x, w4.y, w4.z, w4.w};
+      int oj[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) oj[j] = corner_pixel(xy.x, xy.y, j, L.Hb, L.Wb);
+      float v0[VEC], v1[VEC];
+      {
+        const float* pmap = map0 + (size_t)b * HW * D;
+        const float* fmap = feat + (size_t)b * HW * D;
+        float pg[VEC], f[VEC];
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) { pg[v] = 0.f; f[v] = 0.f; }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          if (oj[j] >= 0) {
+            float t[VEC], s[VEC];
+            V<VEC>::ld(pmap + (size_t)oj[j] * D + chl, t);
+            V<VEC>::ld(fmap + (size_t)oj[j] * D + chl, s);
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) { pg[v] += t[v] * wj[j]; f[v] += s[v] * wj[j]; }
+          }
+        }
+        const float* gN = rows + c * D + chl;
+        const float* gS = rows + (kBundle + c) * D + chl;
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) {
+          v0[v] = gN[v] * pg[v];                 // grad_feat
+          v1[v] = gS[v] + gN[v] * f[v];          // grad_prob_map
+        }
+      }
+      float* vs = vec + ((size_t)kk * kBundle + c) * D + chl;
+      V<VEC>::st(vs, v0);
+      V<VEC>::st(vs + (size_t)kChunk * kBundle * D, v1);
+    }
+    __syncthreads();
+    // ---- corners the box does not cover, reduced straight to global memory (kept out of A2 so that its gathers
+    //      are not ordered behind reductions)
+    for (int i = threadIdx.x; i < kChunk * kBundle * LPW; i += kBundleThreads) {
+      const int l = i % LPW, c = (i / LPW) % kBundle, kk = i / (LPW * kBundle);
+      if (!((sm.direct[kk] >> c) & 1u)) continue;
+      const int2 xy = sm.xy[kk][c], box = sm.box[kk];
+      const int b = sm.bat[c], chl = l * VEC;
+      const float4 w4 = sm.w[kk][c];
+      const float wj[4] = {w4.x, w4.y, w4.z, w4.w};
+      const float* vs = vec + ((size_t)kk * kBundle + c) * D + chl;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int o = corner_pixel(xy.x, xy.y, j, L.Hb, L.Wb);
+        const int dx = xy.x + (j & 1) - box.x, dy = xy.y + (j >> 1) - box.y;
+        if (o < 0 || (b == b0 && dx < kBox && dy < kBox)) continue;
+        float t[VEC];
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) t[v] = vs[v] * wj[j];
+        V<VEC>::red(out0 + ((size_t)b * HW + o) * D + chl, t);
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) t[v] = vs[(size_t)kChunk * kBundle * D + v] * wj[j];
+        V<VEC>::red(out1 + ((size_t)b * HW + o) * D + chl, t);
+      }
+    }
+    // ---- B: thread = (waypoint, box pixel, float4)
+    for (int i = threadIdx.x; i < kChunk * kBox * kBox * LPW; i += kBundleThreads) {
+      const int l = i % LPW, p = (i / LPW) % (kBox * kBox), kk = i / (LPW * kBox * kBox);
+      unsigned m = sm.who[kk][p];
+      if (!m) continue;
+      const int2 box = sm.box[kk];
+      const int px = box.x + p % kBox, py = box.y + p / kBox;
+      if (px < 0 || px >= L.Wb || py < 0 || py >= L.Hb) continue;
+      float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
+      const float* vk = vec + (size_t)kk * kBundle * D + l * VEC;
+      for (; m; m &= m - 1) {             // the pixel's cells in cell order
+        const int c = __ffs(m) - 1;
+        const int2 xy = sm.xy[kk][c];
+        const int dx = px - xy.x, dy = py - xy.y;
+        const float4 w4 = sm.w[kk][c];
+        const float w = dy ? (dx ? w4.w : w4.z) : (dx ? w4.y : w4.x);
+        const float4 v0 = *reinterpret_cast<const float4*>(vk + c * D);
+        a0.x += v0.x * w; a0.y += v0.y * w; a0.z += v0.z * w; a0.w += v0.w * w;
+        const float4 v1 = *reinterpret_cast<const float4*>(vk + (size_t)kChunk * kBundle * D + c * D);
+        a1.x += v1.x * w; a1.y += v1.y * w; a1.z += v1.z * w; a1.w += v1.w * w;
+      }
+      const size_t o = (size_t)(py * L.Wb + px) * D + l * VEC;
+      red_add_v4(o0 + o, a0);
+      red_add_v4(o1 + o, a1);
+    }
+    __syncthreads();
+  }
+}
+
 int check_lr(LrDims& L, int bs, int D, int G, int Hb, int Wb, int grid_num, float grid_step, float eps,
              int act, int& vec, const char* who, long long cell0, long long ncells) {
   VIDAR_REQUIRE(bs > 0 && D > 0 && G > 0 && Hb > 1 && Wb > 1 && grid_num > 0,
@@ -475,6 +758,46 @@ int check_lr(LrDims& L, int bs, int D, int G, int Hb, int Wb, int grid_num, floa
 
 inline unsigned lr_blocks(const LrDims& L) {
   return (unsigned)((L.ncells + kCellsPerBlock - 1) / kCellsPerBlock);
+}
+
+// Phase 2 backward in bundles: cell order (key kernel + CUB's stable radix sort) and the bundle kernel.  The order's scratch (two keys and two
+// indices per cell, the sort's temp storage) is stream-ordered from the library's pool.
+int pool_bwd_bundled(const LrDims& L, const float* map0, const float* feat, const float* grad_in, float* out0, float* out1,
+               const float* aux0, const float* aux1, cudaStream_t st, const char* who) {
+  VIDAR_REQUIRE(L.ncells < INT_MAX, "%s: %lld cells, at most 2^31 - 1", who, L.ncells);
+  const int n = (int)L.ncells, HW = L.Hb * L.Wb;
+  const long long nbat = (L.cell0 + L.ncells - 1) / HW - L.cell0 / HW + 1;
+  int bits = kAngleBits;
+  while ((1LL << (bits - kAngleBits)) < nbat) ++bits;
+  const size_t smem = bundle_smem_bytes(L.D);
+  if (cudaFuncSetAttribute(latent_pool_bwd_bundle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+      cudaSuccess)
+    return set_error(VIDAR_E_CUDA, "%s: cannot opt in to %zu bytes of shared memory", who, smem);
+  using Key = unsigned long long;
+  size_t tmp = 0;
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, tmp, (const Key*)nullptr, (Key*)nullptr, (const int*)nullptr,
+                                                  (int*)nullptr, n, 0, bits, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cell order: %s", who, cudaGetErrorString(e));
+  const size_t off = ((sizeof(Key) + sizeof(int)) * 2 * (size_t)n + 255) & ~(size_t)255;
+  cudaMemPool_t pool;
+  e = scratch_pool(&pool);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: scratch memory pool: %s", who, cudaGetErrorString(e));
+  unsigned char* s = nullptr;
+  e = cudaMallocFromPoolAsync((void**)&s, off + tmp, pool, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cudaMallocFromPoolAsync: %s", who, cudaGetErrorString(e));
+  Key* k0 = reinterpret_cast<Key*>(s);
+  Key* k1 = k0 + n;
+  int* i0 = reinterpret_cast<int*>(k1 + n);
+  int* i1 = i0 + n;
+  latent_order_key_kernel<<<(n + 255) / 256, 256, 0, st>>>(L, k0, i0);
+  e = cub::DeviceRadixSort::SortPairs(s + off, tmp, k0, k1, i0, i1, n, 0, bits, st);
+  if (e == cudaSuccess)
+    latent_pool_bwd_bundle_kernel<<<(unsigned)((n + kBundle - 1) / kBundle), kBundleThreads, smem, st>>>(
+        L, i1, map0, feat, grad_in, out0, out1, aux0, aux1);
+  const cudaError_t ef = cudaFreeAsync(s, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cell order: %s", who, cudaGetErrorString(e));
+  if (ef != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cudaFreeAsync: %s", who, cudaGetErrorString(ef));
+  return VIDAR_OK;
 }
 
 }  // namespace
@@ -528,7 +851,13 @@ static int pool_bwd(const LrDims& L, int vec, int G, const float* prob, const fl
   if (L.ncells == 0) return VIDAR_OK;
   const size_t n = (size_t)L.bs * L.Hb * L.Wb * L.D;
   const float* as = (aux && pooled) ? aux + 2 * n : nullptr;
-  LR_DISPATCH_VG(latent_pool_bwd_kernel, L, prob, feat, grad_pooled, grad_prob_map, grad_feat, as, pooled);
+  if (vec == 4 && G == 1) {
+    const int rc = pool_bwd_bundled(L, prob, feat, grad_pooled, grad_feat, grad_prob_map, as, pooled, st,
+                                    "LatentRendering.pool_backward");
+    if (rc) return rc;
+  } else {
+    LR_DISPATCH_VG(latent_pool_bwd_kernel, L, prob, feat, grad_pooled, grad_prob_map, grad_feat, as, pooled);
+  }
   return check_launch("LatentRendering.pool_backward");
 }
 

@@ -1293,37 +1293,6 @@ inline bool tile_backward_ok(const MsdaParams& p) {
   return p.C == 32 && p.P == kTilePoints && p.LP == 32 && p.K < (1 << (32 - kRecBits));
 }
 
-// The row order's scratch comes from a memory pool of this library that keeps what it has allocated (release
-// threshold = max): eager training does not pay a fresh physical allocation per backward, and the device's
-// default pool, which the rest of the process may use, keeps its settings.
-inline cudaError_t scratch_pool(cudaMemPool_t* pool) {
-  static std::mutex mu;
-  static cudaMemPool_t pools[128] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 128) return cudaErrorInvalidDevice;
-  std::lock_guard<std::mutex> lock(mu);
-  if (!pools[dev]) {
-    cudaMemPoolProps props = {};
-    props.allocType = cudaMemAllocationTypePinned;
-    props.location.type = cudaMemLocationTypeDevice;
-    props.location.id = dev;
-    cudaMemPool_t p = nullptr;
-    e = cudaMemPoolCreate(&p, &props);
-    if (e != cudaSuccess) return e;
-    uint64_t keep = UINT64_MAX;
-    e = cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &keep);
-    if (e != cudaSuccess) {
-      cudaMemPoolDestroy(p);
-      return e;
-    }
-    pools[dev] = p;
-  }
-  *pool = pools[dev];
-  return cudaSuccess;
-}
-
 // Row order + tile kernel.  The order's scratch (two ints per row and a cell histogram per 1024 rows) is
 // stream-ordered (cudaMallocFromPoolAsync / cudaFreeAsync): no host sync, and a CUDA graph captures it as
 // allocation nodes, so the C signature needs no workspace argument.
