@@ -404,6 +404,55 @@ int vidar_nn_backward(const float* p1, const float* p2, const int64_t* lengths1,
                       const int64_t* lengths2, const int64_t* idx, const float* grad_dists,
                       float* grad_p1, float* grad_p2, int N, int P1, int P2, int D, void* stream);
 
+/* Segmented, masked NN (D = 3): segment s pairs the queries [q_off[s], q_off[s+1]) of q [Pq, 3] with the
+ * candidates [c_off[s], c_off[s+1]) of c [Pc, 3]; q_off / c_off [S+1] int64 on the device.  q_mask / c_mask
+ * (uint8, NULL = all kept): a zero entry is neither query nor candidate.  Per query: dists [Pq] the squared
+ * distance to the nearest kept candidate of its segment (ties: smallest index), idx [Pq] its index within the
+ * candidate segment, or VIDAR_NN_MASKED (masked query) / VIDAR_NN_EMPTY (no kept candidate at a finite
+ * distance), with dists 0.  max_q / max_c: host-known upper bounds of the segment lengths (size the grid).
+ * scratch: Pq uint64 (fully overwritten). */
+#define VIDAR_NN_MASKED (-1)
+#define VIDAR_NN_EMPTY (-2)
+int vidar_nn_segments_forward(const float* q, const float* c, const int64_t* q_off, const int64_t* c_off,
+                              const unsigned char* q_mask, const unsigned char* c_mask, float* dists,
+                              int64_t* idx, unsigned long long* scratch, int S, long long Pq, int max_q,
+                              int max_c, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * (iv) ViDAR's evaluation metrics -- Chamfer distance inside the point-cloud range and L1 / AbsRel ray errors
+ *   (bevformer/detectors/vidar.py:452-497, utils/e2e_predictor_utils.py:146-183, utils/eval_utils.py:17-225)
+ *   N = samples x frames clouds, n = b * F + f.  pred [Pp, 3], gt [Pg, 3] flat fp32, cloud n at rows
+ *   [pred_off[n], pred_off[n+1]) / [gt_off[n], gt_off[n+1]) (int64 [N+1], device); origin [N, 3].
+ * ---------------------------------------------------------------------------------- */
+
+/* Fills the 3N-segment search layout:
+ *   qbuf [Pp + 2Pg, 3] = pred xyz | gt xyz | gt spherical,  q_mask [Pp + 2Pg]
+ *   cbuf [Pg + 2Pp, 3] = gt xyz | pred xyz | pred spherical, c_mask [Pg + 2Pp]
+ *   q_off, c_off [3N+1]: segment n = forward Chamfer, N+n = backward Chamfer, 2N+n = spherical search.
+ * xyz masks: inside pc_range_host (6 floats, HOST memory, inclusive); spherical points (atan2(x, y),
+ * atan2(z, y), 1) of point - origin, masked where |point - origin| <= 1e-2. */
+int vidar_eval_prologue(const float* pred, const float* gt, const float* origin, const int64_t* pred_off,
+                        const int64_t* gt_off, const float* pc_range_host, float* qbuf, float* cbuf,
+                        unsigned char* q_mask, unsigned char* c_mask, int64_t* q_off, int64_t* c_off,
+                        int N, long long Pp, long long Pg, void* stream);
+
+/* Ray errors and the deterministic per-cloud reduction over the NN results of the 3N segments
+ * (vidar_nn_segments_forward on the prologue's layout; dists / idx [Pp + 2Pg]).
+ *   partials: 3N * ceil(max_len / 256) * 4 doubles of scratch, max_len >= every cloud's size
+ *   out [N, VIDAR_EVAL_FIELDS] fp64: sum l1, sum absrel, count (gt points kept), sum forward d, pred points
+ *       inside, sum backward d, gt points inside, flags (VIDAR_EVAL_* bits)
+ *   rays [Pg, 9] (NULL = skip): interpolated point, clamped gt, clamped interpolated point (NaN for masked gt) */
+#define VIDAR_EVAL_FIELDS 8
+#define VIDAR_EVAL_GT_DEGENERATE 1       /* a gt ray outside PC_RANGE ends at its origin (RuntimeError) */
+#define VIDAR_EVAL_GT_OUTSIDE 2          /* a clamped gt ray never touches the volume (AssertionError) */
+#define VIDAR_EVAL_INTERP_DEGENERATE 4   /* the same two failures of an interpolated point */
+#define VIDAR_EVAL_INTERP_OUTSIDE 8
+#define VIDAR_EVAL_NO_PRED 16            /* gt points kept but no pred point kept */
+int vidar_eval_metrics(const float* pred, const float* gt, const float* origin, const int64_t* pred_off,
+                       const int64_t* gt_off, const int64_t* q_off, const unsigned char* q_mask,
+                       const float* dists, const int64_t* idx, double* partials, double* out, float* rays,
+                       int N, int max_len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,22 @@ namespace {
 constexpr int kNnThreads = 256;
 constexpr int kNnTile = 1024;
 
+// The inner loop shared by the batched and the segmented search: scan `cnt` candidates of a shared-memory
+// tile whose first point has index `base`, keeping the first strictly smaller squared distance.
+template <int D>
+__device__ __forceinline__ void nn_scan_tile(const float (&a)[D], const float* tile, int cnt, int base, float& bd,
+                                             int& bi) {
+  for (int j = 0; j < cnt; ++j) {
+    float dist = 0.f;
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+      const float diff = a[d] - tile[j * D + d];
+      dist = __fadd_rn(dist, __fmul_rn(diff, diff));     // `dist += diff * diff`, no contraction
+    }
+    if (dist < bd) { bd = dist; bi = base + j; }
+  }
+}
+
 template <int D>
 __global__ void __launch_bounds__(kNnThreads)
 nn_forward_kernel(const float* __restrict__ p1, const float* __restrict__ p2,
@@ -43,17 +59,7 @@ nn_forward_kernel(const float* __restrict__ p1, const float* __restrict__ p2,
     __syncthreads();
     for (int e = threadIdx.x; e < cnt * D; e += kNnThreads) tile[e] = p2[((size_t)n * P2 + t0) * D + e];
     __syncthreads();
-    if (live) {
-      for (int j = 0; j < cnt; ++j) {
-        float dist = 0.f;
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          const float diff = a[d] - tile[j * D + d];
-          dist = __fadd_rn(dist, __fmul_rn(diff, diff));     // `dist += diff * diff`, no contraction
-        }
-        if (dist < bd) { bd = dist; bi = t0 + j; }
-      }
-    }
+    if (live) nn_scan_tile<D>(a, tile, cnt, t0, bd, bi);
   }
   if (live) {
     const unsigned long long key = ((unsigned long long)__float_as_uint(bd) << 32) | (unsigned)bi;
@@ -97,10 +103,87 @@ __global__ void nn_backward_kernel(const float* __restrict__ p1, const float* __
   }
 }
 
+// Segmented search: segment s pairs queries [q_off[s], q_off[s+1]) with candidates [c_off[s], c_off[s+1]),
+// blockIdx.z = s, so ragged clouds of one call share a launch.  A masked candidate enters the tile as +inf and
+// can never be strictly nearer than the running best (valid points are finite); a masked query writes nothing.
+constexpr unsigned long long kNnNone = ~0ull;
+
+__global__ void __launch_bounds__(kNnThreads)
+nn_segments_kernel(const float* __restrict__ q, const float* __restrict__ c, const int64_t* __restrict__ q_off,
+                   const int64_t* __restrict__ c_off, const unsigned char* __restrict__ q_mask,
+                   const unsigned char* __restrict__ c_mask, unsigned long long* __restrict__ best, int splits) {
+  __shared__ float tile[kNnTile * 3];
+  const int s = blockIdx.z;
+  const int64_t q0 = q_off[s], c0 = c_off[s];
+  const int Lq = (int)(q_off[s + 1] - q0), Lc = (int)(c_off[s + 1] - c0);
+  const int i = blockIdx.x * kNnThreads + threadIdx.x;
+  if ((int)blockIdx.x * kNnThreads >= Lq) return;
+  const int chunk = (Lc + splits - 1) / splits;
+  const int j0 = blockIdx.y * chunk, j1 = min(Lc, j0 + chunk);
+  if (j0 >= j1) return;
+  float a[3];
+  const bool live = i < Lq && (!q_mask || q_mask[q0 + i]);
+#pragma unroll
+  for (int d = 0; d < 3; ++d) a[d] = live ? q[(q0 + i) * 3 + d] : 0.f;
+  float bd = INFINITY;
+  int bi = 0;
+  for (int t0 = j0; t0 < j1; t0 += kNnTile) {
+    const int cnt = min(kNnTile, j1 - t0);
+    __syncthreads();
+    for (int e = threadIdx.x; e < cnt * 3; e += kNnThreads) {
+      const int64_t g = c0 + t0 + e / 3;
+      tile[e] = (!c_mask || c_mask[g]) ? c[(c0 + t0) * 3 + e] : INFINITY;
+    }
+    __syncthreads();
+    if (live) nn_scan_tile<3>(a, tile, cnt, t0, bd, bi);
+  }
+  if (live && bd < INFINITY) atomicMin(best + q0 + i, ((unsigned long long)__float_as_uint(bd) << 32) | (unsigned)bi);
+}
+
+__global__ void nn_segments_unpack_kernel(const unsigned long long* __restrict__ best,
+                                          const unsigned char* __restrict__ q_mask, float* __restrict__ dists,
+                                          int64_t* __restrict__ idx, long long Pq) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= Pq) return;
+  const unsigned long long key = best[t];
+  const bool masked = q_mask && !q_mask[t];
+  const bool ok = !masked && key != kNnNone;
+  dists[t] = ok ? __uint_as_float((unsigned)(key >> 32)) : 0.f;
+  idx[t] = ok ? (int64_t)(unsigned)(key & 0xffffffffu) : (masked ? VIDAR_NN_MASKED : VIDAR_NN_EMPTY);
+}
+
 }  // namespace
 }  // namespace vidar
 
 using namespace vidar;
+
+extern "C" int vidar_nn_segments_forward(const float* q, const float* c, const int64_t* q_off, const int64_t* c_off,
+                                         const unsigned char* q_mask, const unsigned char* c_mask, float* dists,
+                                         int64_t* idx, unsigned long long* scratch, int S, long long Pq,
+                                         int max_q, int max_c, void* stream) {
+  VIDAR_REQUIRE(q_off && c_off, "nn_segments: null pointer argument");
+  VIDAR_REQUIRE(S > 0 && S <= 65535 && Pq >= 0 && max_q >= 0 && max_c >= 0,
+                "nn_segments: bad sizes S=%d Pq=%lld max_q=%d max_c=%d", S, Pq, max_q, max_c);
+  VIDAR_REQUIRE(Pq == 0 || (q && dists && idx && scratch), "nn_segments: null query / output buffer");
+  VIDAR_REQUIRE(max_c == 0 || c, "nn_segments: null candidate buffer");
+  if (Pq == 0) return VIDAR_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaMemsetAsync(scratch, 0xff, sizeof(unsigned long long) * (size_t)Pq, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "nn_segments: memset: %s", cudaGetErrorString(e));
+  if (max_q > 0 && max_c > 0) {
+    const int bx = (max_q + kNnThreads - 1) / kNnThreads;
+    // the same occupancy rule as vidar_nn_forward, with the longest segments standing for all of them
+    int splits = (4 * num_sms() + bx * S - 1) / (bx * S);
+    const int max_splits = (max_c + kNnTile - 1) / kNnTile;
+    if (splits > max_splits) splits = max_splits;
+    if (splits < 1) splits = 1;
+    nn_segments_kernel<<<dim3(bx, splits, S), kNnThreads, 0, st>>>(q, c, q_off, c_off, q_mask, c_mask, scratch, splits);
+    int rc = check_launch("nn_segments");
+    if (rc) return rc;
+  }
+  nn_segments_unpack_kernel<<<(unsigned)((Pq + 255) / 256), 256, 0, st>>>(scratch, q_mask, dists, idx, Pq);
+  return check_launch("nn_segments(unpack)");
+}
 
 extern "C" int vidar_nn_forward(const float* p1, const float* p2, const int64_t* lengths1,
                                 const int64_t* lengths2, float* dists, int64_t* idx,
