@@ -24,6 +24,16 @@ def test_product_does_not_import_oracle_or_reference():
     assert not bad, f"product files reference oracle/ or /root/reference: {bad}"
 
 
+def test_native_library_reads_no_environment():
+    """What libvidar_b200.so computes and which kernels it launches depend only on its arguments."""
+    bad = []
+    for path in _py_and_cu(os.path.join(ROOT, "vidar_b200", "csrc")):
+        with open(path) as fh:
+            if re.search(r"\bgetenv\b", fh.read()):
+                bad.append(path)
+    assert not bad, f"native sources read environment variables: {bad}"
+
+
 def test_no_cpu_fallback_on_cpu_tensors():
     import pytest
     import torch

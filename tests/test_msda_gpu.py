@@ -210,42 +210,3 @@ def test_fused_sca_epilogue_rejects_other_shapes(cuda):
     with pytest.raises(RuntimeError, match="num_levels \\* num_points == 32"):
         msda.MSDeformAttn3DFusedFunction.apply(v, shapes.to(cuda), lsi.to(cuda), torch.zeros(1, 5, 4, 2, device=cuda),
                                                torch.zeros(1, 5, 8, 1, 4, 2, device=cuda), torch.zeros(1, 5, 8, 4, device=cuda))
-
-
-@pytest.mark.parametrize("mode,fwd", [("1", "0"), ("2", "1")], ids=["slab-plain", "slab-tma+fwd"])
-def test_slab_variants(cuda, mode, fwd):
-    """The persistent shared-memory variants (csrc/msda_slab.cuh; off by default, selected by environment
-    variables read once per process) against the oracle, in a subprocess: SCA shape, plain op and both row-map
-    functions."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = r"""
-import torch
-from oracle import msda_ref
-from tests import parity
-from tests.inputs import SCA_LEVELS, msda_inputs
-from vidar_b200 import msda
-dev = torch.device("cuda:0")
-for mode_, Q in (("local", 333), ("stress", 150)):
-    d = msda_inputs(2, Q, 8, 32, SCA_LEVELS, 8, seed=7, mode=mode_)
-    g = {k: v.to(dev) for k, v in d.items()}
-    out = msda.ext_module.ms_deform_attn_forward(g["value"], g["shapes"], g["lsi"], g["loc"], g["attn"], im2col_step=64)
-    gv, gl, ga = torch.zeros_like(g["value"]), torch.full_like(g["loc"], 7.0), torch.full_like(g["attn"], 7.0)
-    msda.ext_module.ms_deform_attn_backward(g["value"], g["shapes"], g["lsi"], g["loc"], g["attn"], g["grad_out"], gv, gl, ga, im2col_step=64)
-    rout = msda_ref.msda_grid_sample(d["value"].double(), d["shapes"], d["loc"].double(), d["attn"].double())
-    rgv, rgl, rga = msda_ref.msda_grid_sample_backward(d["value"], d["shapes"], d["loc"], d["attn"], d["grad_out"])
-    parity.close(out, rout, "out")
-    parity.close(gv, rgv, "grad_value")
-    parity.close(ga, rga, "grad_attn")
-    keep = parity.off_kink(d["loc"], d["shapes"])
-    parity.close(gl, rgl, "grad_loc", keep=keep.unsqueeze(-1).expand_as(rgl))
-# the row map (vidar_msda_rows_* / vidar_msda_sca_rows_*) on the same variants
-from tests.test_msda_rows_gpu import slab_row_cases
-slab_row_cases(dev)
-print("SLAB-OK")
-"""
-    env = dict(os.environ, VIDAR_MSDA_SLAB=mode, VIDAR_MSDA_SLAB_FWD=fwd, PYTHONPATH=root)
-    r = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "SLAB-OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]

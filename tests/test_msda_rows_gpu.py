@@ -9,8 +9,7 @@ slot gradient times 1 / #cameras, and zero for rows outside the launch (dead lis
 
 The cases reach every backward branch of vidar_msda_rows_backward / vidar_msda_sca_rows_backward: the tile kernel
 (C = 32, 8 points on 4 levels, K < 2^19) and msda_backward_kernel<CV, .., IDX> otherwise (C = 16 / 64, other L*P,
-K >= 2^19), with the forward at all three head widths.  test_msda_gpu.py::test_slab_variants runs the slab
-variants on the row map."""
+K >= 2^19), with the forward at all three head widths."""
 import pytest
 import torch
 
@@ -538,17 +537,3 @@ def test_rows_backward_scratch_reuse(cuda):
     for Qd, shapes, grp, inv, g, leaves, slots in runs:
         ref = _oracle_rows(sca.unit_plan(1, 0, cams), 1, Qd, shapes, None, None, inv, [grp], g, per_camera=True)
         _close_rows(slots, [[t.grad for t in leaves]], ref, shapes, [grp], tag=f"{Qd} rows: ")
-
-
-def slab_row_cases(dev):
-    """One row-map case of each function against the oracle (run by test_msda_gpu.py::test_slab_variants with the
-    slab variants selected)."""
-    cams, Qd = 2, 700
-    shapes, lsi, grp = _inputs(dev, cams, Qd, "stress", seed=130)
-    idx, count = _lists(dev, cams, Qd, 131), torch.tensor([650, 333], dtype=torch.int32, device=dev)
-    _check(dev, [(0, cams, 2, 1, 2)], 1, Qd, [grp], shapes, lsi, idx=idx, count=count, inv=_inv(dev, 1, Qd, 132),
-           plain=False)
-    _check(dev, sca.unit_plan(1, 0, cams), 1, Qd, [grp], shapes, lsi, inv=_inv(dev, 1, Qd, 133), plain=False)
-    _check_sca(dev, 3, Qd, [(0, 3, 2, 0, 1)], idx=_lists(dev, 3, Qd, 134),
-               count=torch.tensor([700, 420, 99], dtype=torch.int32, device=dev), inv=_inv(dev, 2, Qd, 135), seed=136,
-               bs=2)

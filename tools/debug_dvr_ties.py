@@ -11,7 +11,7 @@ dev = torch.device("cuda:0")
 s, o, p, t = (torch.from_numpy(a).to(dev) for a in (sigma, origin, points, tindex))
 grid = list(sigma.shape[1:])
 ref = build_ref.load("ref_dvr")
-out = {"eps": os.environ.get("VIDAR_DVR_TIE_EPS", "default")}
+out = {}
 bad = lambda a, b: np.flatnonzero(np.abs(a - b) > 1e-5 * np.maximum(1.0, np.abs(b)))
 for name, f_gpu, f_orc, f_ref in (
         ("fwd_test", lambda: render.dvr.render_forward(s, o, p, t, grid, "test")[0], lambda: dvr_ref.render_forward(sigma, origin, points, tindex, None, "test")[0],

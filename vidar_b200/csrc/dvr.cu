@@ -32,7 +32,6 @@
 // Launch: 64-thread blocks (30k rays -> 469 blocks over 132 SMs; the reference's
 // 1024-thread blocks give 30 blocks), one ray per thread, neighbouring rays in a warp.
 #include <float.h>
-#include <stdlib.h>
 #include <math.h>
 
 #include "common.cuh"
@@ -455,7 +454,7 @@ __global__ void __launch_bounds__(kWarpRaysPerBlock * 32)
 render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
                    const float* __restrict__ points, const float* __restrict__ tindex,
                    float* __restrict__ pred_dist, float* __restrict__ gt_dist,
-                   float* __restrict__ grad_sigma, int mode, int cap, double kTieEps, WarpRayExtra ex) {
+                   float* __restrict__ grad_sigma, int mode, int cap, double tie_eps, WarpRayExtra ex) {
   using TR = Traits<V>;
   constexpr bool GRAD = MODE != 0;
   constexpr bool MERGE = TR::kMerge;
@@ -550,7 +549,7 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
         if (a != ax && moves[a] && gi[a] < hi[a] && (gi[a] > 0 || gi[ax] > 0) &&
-            fabs(tm[a] - tcur) <= kTieEps * fabs(tcur))
+            fabs(tm[a] - tcur) <= tie_eps * fabs(tcur))
           tie = true;
       }
       const bool inside = v[0] >= 0 && v[0] < G.X && v[1] >= 0 && v[1] < G.Y && v[2] >= 0 && v[2] < G.Z;
@@ -561,9 +560,9 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
           const double cx = fma(last, r.dx, (double)r.vx0), cy = fma(last, r.dy, (double)r.vy0),
                        cz = fma(last, r.dz, (double)r.vz0);
           if (last > 0.0) {
-            tie = tie || fabs(fabs(cx - floor(cx)) - 0.5) <= kTieEps * fmax(1.0, fabs(cx)) ||
-                  fabs(fabs(cy - floor(cy)) - 0.5) <= kTieEps * fmax(1.0, fabs(cy)) ||
-                  fabs(fabs(cz - floor(cz)) - 0.5) <= kTieEps * fmax(1.0, fabs(cz));
+            tie = tie || fabs(fabs(cx - floor(cx)) - 0.5) <= tie_eps * fmax(1.0, fabs(cx)) ||
+                  fabs(fabs(cy - floor(cy)) - 0.5) <= tie_eps * fmax(1.0, fabs(cy)) ||
+                  fabs(fabs(cz - floor(cz)) - 0.5) <= tie_eps * fmax(1.0, fabs(cz));
           }
           px = (int)round(cx); px = px < G.X ? px : G.X - 1; px = px >= 0 ? px : 0;
           py = (int)round(cy); py = py < G.Y ? py : G.Y - 1; py = py >= 0 ? py : 0;
@@ -834,14 +833,8 @@ bool warp_ray_config(const Grid& G, K kernel, int& cap, size_t& smem) {
 }
 
 // relative distance below which two crossing times / a path coordinate and a .5 tie count as a near-tie
-// (render_warp_kernel); VIDAR_DVR_TIE_EPS overrides for experiments
-inline double tie_eps() {
-  static const double v = [] {
-    const char* e = getenv("VIDAR_DVR_TIE_EPS");
-    return e ? atof(e) : 1e-9;
-  }();
-  return v;
-}
+// (render_warp_kernel): such rays take the serial traversal, whose decisions are the reference's
+constexpr double kTieEps = 1e-9;
 
 inline dim3 ray_grid(const Grid& G, int per_block) {
   return dim3((unsigned)((G.M + per_block - 1) / per_block), (unsigned)G.N);
@@ -880,7 +873,7 @@ extern "C" int vidar_dvr_render_forward(const float* sigma, const float* origin,
   if (warp_ray_config(G, render_warp_kernel<V_DVR_FWD, 0>, cap, smem)) {
     render_warp_kernel<V_DVR_FWD, 0><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem,
                                        (cudaStream_t)stream>>>(G, sigma, origin, points, tindex, pred_dist,
-                                                               gt_dist, nullptr, train_phase, cap, tie_eps(), WarpRayExtra{});
+                                                               gt_dist, nullptr, train_phase, cap, kTieEps, WarpRayExtra{});
   } else {
     forward_kernel<V_DVR_FWD><<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
         G, sigma, origin, points, tindex, pred_dist, gt_dist, train_phase);
@@ -904,7 +897,7 @@ extern "C" int vidar_dvr_render(const float* sigma, const float* origin, const f
   if (warp_ray_config(G, render_warp_kernel<V_DVR_RENDER, 1>, cap, smem)) {
     render_warp_kernel<V_DVR_RENDER, 1><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem,
                                           (cudaStream_t)stream>>>(G, sigma, origin, points, tindex, pred_dist,
-                                                                  gt_dist, grad_sigma, loss_type, cap, tie_eps(), WarpRayExtra{});
+                                                                  gt_dist, grad_sigma, loss_type, cap, kTieEps, WarpRayExtra{});
   } else {
     render_grad_kernel<<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
         G, sigma, origin, points, tindex, pred_dist, gt_dist, grad_sigma, loss_type);
@@ -926,7 +919,7 @@ extern "C" int vidar_dvxlr_forward(const float* sigma, const float* origin, cons
   if (warp_ray_config(G, render_warp_kernel<V_DVXLR, 0>, cap, smem)) {
     // one ray per warp; consecutive records of one (rounded) voxel merge into a segment by a warp scan
     render_warp_kernel<V_DVXLR, 0><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, pred_dist, gt_dist, nullptr, 1, cap, tie_eps(), WarpRayExtra{});
+        G, sigma, origin, points, tindex, pred_dist, gt_dist, nullptr, 1, cap, kTieEps, WarpRayExtra{});
   } else {
     forward_kernel<V_DVXLR><<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
         G, sigma, origin, points, tindex, pred_dist, gt_dist, 1);
@@ -997,7 +990,7 @@ extern "C" int vidar_dvxlr_backward_fused(const float* sigma, const float* origi
   size_t smem;
   if (warp_ray_config(G, render_warp_kernel<V_DVXLR, 2>, cap, smem)) {
     render_warp_kernel<V_DVXLR, 2><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, nullptr, nullptr, grad_sigma, 1, cap, tie_eps(),
+        G, sigma, origin, points, tindex, nullptr, nullptr, grad_sigma, 1, cap, kTieEps,
         WarpRayExtra{grad_pred, grad_ray_pred, grad_sigma_regul, max_d});
   } else {
     dvxlr_fused_bwd_kernel<<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(

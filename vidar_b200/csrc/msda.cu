@@ -21,10 +21,7 @@
 // Work order: for L*P >= 32 a block is 8 consecutive queries of one (b, h) and
 // neighbouring blocks are the other heads of the same queries, so the lines a block
 // touches are neighbours in the image (L1/L2 locality).
-#include <stdlib.h>
-#include <string.h>
-
-#include <mutex>
+#include <type_traits>
 
 #include <cub/block/block_radix_sort.cuh>
 #include <cub/block/block_scan.cuh>
@@ -809,7 +806,8 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
                           const float* __restrict__ grad_out, float* __restrict__ grad_value,
                           float* __restrict__ grad_loc, float* __restrict__ grad_attn) {
   constexpr int CV = 8, NG = 4, P = kTilePoints, NT = kTileThreads, RW = kTileRows / (NT / 32);   // RW rows per warp
-  extern __shared__ __align__(16) unsigned char tile_smem[];
+  // 128-byte aligned: keeps the dynamic region at the offset this kernel was tuned and measured with
+  extern __shared__ __align__(128) unsigned char tile_smem[];
   TileSmem& sm = *reinterpret_cast<TileSmem*>(tile_smem);
   TileSmemEpi& se = *reinterpret_cast<TileSmemEpi*>(tile_smem + sizeof(TileSmem));
   __shared__ TileKeys tk;
@@ -1033,8 +1031,6 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
   }
 }
 
-#include "msda_slab.cuh"
-
 // ---- generic fallback (any C): one thread per (item, channel); scalar atomics.
 __global__ void msda_forward_generic_kernel(const MsdaParams p, float* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1107,17 +1103,10 @@ __global__ void msda_backward_generic_kernel(const MsdaParams p, const float* __
 }
 
 // FORWARD only: per-head level slabs larger than this are read with L1::no_allocate (see ldg4_na), so at
-// the SpatialCrossAttention shape everything but the 48 KB 15x25 level streams (tools/exp_msda.py sweeps the
-// threshold).  The backward keeps plain loads: they share the LSU -> XBAR request path with the reductions,
-// and a no-allocate miss cannot merge with a neighbouring warp's pending miss.
-// VIDAR_MSDA_STREAM_BYTES overrides the forward threshold (experiments; 0xffffffff = off).
-inline unsigned stream_threshold() {
-  static const unsigned v = [] {
-    const char* e = getenv("VIDAR_MSDA_STREAM_BYTES");
-    return e ? (unsigned)strtoul(e, nullptr, 0) : 100000u;
-  }();
-  return v;
-}
+// the SpatialCrossAttention shape everything but the 48 KB 15x25 level streams (a sweep of the threshold at that
+// shape chose it).  The backward keeps plain loads (na_bytes = 0xffffffff): they share the LSU -> XBAR request
+// path with the reductions, and a no-allocate miss cannot merge with a neighbouring warp's pending miss.
+constexpr unsigned kStreamBytes = 100000u;
 
 int fill_params(MsdaParams& p, const float* value, const int64_t* shapes, const int64_t* lsi,
                 const float* loc, const float* attn, int B, int K, int H, int C, int L, int Q,
@@ -1146,7 +1135,7 @@ int fill_params(MsdaParams& p, const float* value, const int64_t* shapes, const 
   p.idx = nullptr; p.count = nullptr; p.inv = nullptr;
   p.ncl = B; p.cam0 = 0; p.bs = 1; p.Qd = Q;
   p.S = 1; p.s_lo = 0; p.s_hi = 1;
-  p.na_bytes = stream_threshold();
+  p.na_bytes = kStreamBytes;
   return VIDAR_OK;
 }
 
@@ -1179,112 +1168,55 @@ inline long long num_blocks(const MsdaParams& p) {
   return (warps + kWarpsPerBlock - 1) / kWarpsPerBlock;
 }
 
-
-// ---- slab (persistent, shared-memory) variants: host side --------------------------------------
-// VIDAR_MSDA_SLAB: 0 = off (default), 1 = slab kernels with plain staging / flush, 2 = with TMA.  Both
-// variants were measured slower than the default kernels at the SpatialCrossAttention shape: the
-// shared-memory hand-over costs more than the 25 % of reduction lines it removes (a barrier per 16-query tile,
-// ~10 issue slots per record, half the L1), with or without TMA.  They stay selectable (and parity-tested,
-// tests/test_msda_gpu.py::test_slab_variants) but off.
-inline int slab_mode() {
-  static const int v = [] {
-    const char* e = getenv("VIDAR_MSDA_SLAB");
-    return e ? atoi(e) : 0;
-  }();
-  return v;
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-inline EncodeTiledFn encode_tiled() {
-  static const EncodeTiledFn fn = [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess) {
-      cudaGetLastError();
-      f = nullptr;
+// The vector kernels at head width p.C (CV = C / 4 lanes per head vector).  The plain op (!EPI && !IDX) packs
+// several items into a warp when L*P is small (set_ipw): the small kernel once every lane group gets an item of
+// its own, MULTI below that.  The row map (IDX) keeps fill_rows' one item per warp.
+template <bool EPI, bool IDX>
+int launch_vec_forward(MsdaParams& p, float* out, cudaStream_t st, const char* who) {
+  if (!IDX) set_ipw(p, p.C / 4);
+  const long long nb = num_blocks(p);
+  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
+  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
+  const auto launch = [&](auto cv) {
+    constexpr int CV = decltype(cv)::value;
+    if constexpr (!EPI && !IDX) {
+      if (p.ipw >= 32 / CV) msda_forward_small_kernel<CV><<<grid, block, 0, st>>>(p, out);
+      else if (p.ipw > 1) msda_forward_kernel<CV, true><<<grid, block, 0, st>>>(p, out);
+      else msda_forward_kernel<CV, false><<<grid, block, 0, st>>>(p, out);
+    } else {
+      msda_forward_kernel<CV, false, EPI, IDX><<<grid, block, 0, st>>>(p, out);
     }
-    return (EncodeTiledFn)f;
-  }();
-  return fn;
-}
-
-// 2-D map over a [rows = B*K, cols = H*C] fp32 matrix (value or grad_value) with a [kSlabBoxRows x 32] box:
-// a head's 128-byte column slice of 128 consecutive pixel rows.
-inline bool make_slab_map(CUtensorMap* m, const float* base, long long rows, int cols) {
-  memset(m, 0, sizeof(*m));
-  EncodeTiledFn enc = encode_tiled();
-  if (!enc || ((uintptr_t)base & 15u) || (cols & 3)) return false;
-  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(float)};
-  const cuuint32_t box[2] = {32u, (cuuint32_t)kSlabBoxRows};
-  const cuuint32_t estr[2] = {1u, 1u};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-inline bool slab_ok(const MsdaParams& p) {
-  return slab_mode() > 0 && p.C == 32 && p.LP == 32 && p.P % 4 == 0 && p.L >= 1 && (p.pix_stride & (p.pix_stride - 1)) == 0 &&
-         vec_ok(p) && (long long)p.B * p.H < (1 << 20);
-}
-
-inline void slab_geo(const MsdaParams& p, SlabGeo& sg, int& grid) {
-  const int slots = 2 * num_sms();
-  const int nh = p.B * p.H;
-  sg.first_it = (p.LP - p.P) / 4;
-  sg.pix_shift = 0;
-  while ((1 << sg.pix_shift) < p.pix_stride) ++sg.pix_shift;
-  sg.tiles = (p.Q + kSlabWarps - 1) / kSlabWarps;
-  sg.parts = slots / nh > 1 ? slots / nh : 1;
-  if (sg.parts > sg.tiles) sg.parts = sg.tiles > 0 ? sg.tiles : 1;
-  sg.use_tma = 0;
-  const long long units = (long long)nh * sg.parts;
-  grid = (int)(units < slots ? units : slots);
-}
-
-constexpr size_t kSlabBwdSmem = (size_t)kSlabMaxRows * 128 + 2 * kSlabRecords * 4 + 2 * kSlabRecords * 4 + 2 * kSlabRecords * 2;
-constexpr size_t kSlabFwdSmem = (size_t)kSlabMaxRows * 128;
-
-template <bool EPI, bool IDX>
-int launch_slab_backward(MsdaParams& p, const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
-                         cudaStream_t st, const char* who) {
-  SlabGeo sg;
-  int grid;
-  slab_geo(p, sg, grid);
-  CUtensorMap map;
-  sg.use_tma = (slab_mode() >= 2 && make_slab_map(&map, grad_value, (long long)p.B * p.K, p.pix_stride)) ? 1 : 0;
-  if (!sg.use_tma) memset(&map, 0, sizeof(map));
-  auto k = msda_backward_slab_kernel<EPI, IDX>;
-  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSlabBwdSmem) != cudaSuccess)
-    return set_error(VIDAR_E_CUDA, "%s: cannot opt in to %zu bytes of shared memory", who, kSlabBwdSmem);
-  k<<<grid, kSlabWarps * 32, kSlabBwdSmem, st>>>(p, sg, map, grad_out, grad_value, grad_loc, grad_attn);
+  };
+  if (p.C == 32) launch(std::integral_constant<int, 8>{});
+  else if (p.C == 16) launch(std::integral_constant<int, 4>{});
+  else launch(std::integral_constant<int, 16>{});
   return check_launch(who);
 }
 
 template <bool EPI, bool IDX>
-int launch_slab_forward(MsdaParams& p, float* out, cudaStream_t st, const char* who) {
-  SlabGeo sg;
-  int grid;
-  slab_geo(p, sg, grid);
-  CUtensorMap map;
-  sg.use_tma = (slab_mode() >= 2 && make_slab_map(&map, p.value, (long long)p.B * p.K, p.pix_stride)) ? 1 : 0;
-  if (!sg.use_tma) memset(&map, 0, sizeof(map));
-  auto k = msda_forward_slab_kernel<EPI, IDX>;
-  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSlabFwdSmem) != cudaSuccess)
-    return set_error(VIDAR_E_CUDA, "%s: cannot opt in to %zu bytes of shared memory", who, kSlabFwdSmem);
-  k<<<grid, kSlabWarps * 32, kSlabFwdSmem, st>>>(p, sg, map, out);
+int launch_vec_backward(MsdaParams& p, const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
+                        cudaStream_t st, const char* who) {
+  if (!IDX) set_ipw(p, p.C / 4);
+  const long long nb = num_blocks(p);
+  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
+  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
+  const auto launch = [&](auto cv) {
+    constexpr int CV = decltype(cv)::value;
+    if constexpr (!EPI && !IDX) {
+      if (p.ipw >= 32 / CV)
+        msda_backward_small_kernel<CV><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+      else if (p.ipw > 1)
+        msda_backward_kernel<CV, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+      else
+        msda_backward_kernel<CV, false><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+    } else {
+      msda_backward_kernel<CV, false, EPI, IDX><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+    }
+  };
+  if (p.C == 32) launch(std::integral_constant<int, 8>{});
+  else if (p.C == 16) launch(std::integral_constant<int, 4>{});
+  else launch(std::integral_constant<int, 16>{});
   return check_launch(who);
-}
-
-// VIDAR_MSDA_SLAB_FWD=1: the forward also runs its slab variant (off by default, see DESIGN.md 4.1)
-inline bool slab_forward_on() {
-  static const bool v = [] {
-    const char* e = getenv("VIDAR_MSDA_SLAB_FWD");
-    return e && atoi(e) != 0;
-  }();
-  return v;
 }
 
 // The tile-aggregating rows backward: C = 32, 8 points on each of 4 levels (SpatialCrossAttention).
@@ -1349,27 +1281,11 @@ extern "C" int vidar_msda_forward(const float* value, const int64_t* spatial_sha
   if (rc) return rc;
   VIDAR_REQUIRE(out, "ms_deform_attn_forward: null output");
   cudaStream_t st = (cudaStream_t)stream;
-  if (slab_ok(p) && slab_forward_on()) return launch_slab_forward<false, false>(p, out, st, "ms_deform_attn_forward");
-  if (vec_ok(p)) {
-    const int CV = C / 4;
-    set_ipw(p, CV);
-    const long long nb = num_blocks(p);
-    VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_forward: problem too large");
-    const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
-#define VIDAR_FWD(CVV)                                                                     \
-  if (p.ipw >= 32 / CVV) msda_forward_small_kernel<CVV><<<grid, block, 0, st>>>(p, out);  \
-  else if (p.ipw > 1) msda_forward_kernel<CVV, true><<<grid, block, 0, st>>>(p, out);     \
-  else msda_forward_kernel<CVV, false><<<grid, block, 0, st>>>(p, out)
-    if (CV == 8) { VIDAR_FWD(8); }
-    else if (CV == 4) { VIDAR_FWD(4); }
-    else { VIDAR_FWD(16); }
-#undef VIDAR_FWD
-  } else {
-    const long long n = p.items * C;
-    const long long nb = (n + 255) / 256;
-    VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_forward: problem too large");
-    msda_forward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, out);
-  }
+  if (vec_ok(p)) return launch_vec_forward<false, false>(p, out, st, "ms_deform_attn_forward");
+  const long long n = p.items * C;
+  const long long nb = (n + 255) / 256;
+  VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_forward: problem too large");
+  msda_forward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, out);
   return check_launch("ms_deform_attn_forward");
 }
 
@@ -1387,38 +1303,16 @@ extern "C" int vidar_msda_backward(const float* value, const int64_t* spatial_sh
                 "ms_deform_attn_backward: null gradient pointer");
   p.na_bytes = 0xffffffffu;
   cudaStream_t st = (cudaStream_t)stream;
-  if (slab_ok(p))
-    return launch_slab_backward<false, false>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight, st,
-                                              "ms_deform_attn_backward");
-  if (vec_ok(p)) {
-    const int CV = C / 4;
-    set_ipw(p, CV);
-    const long long nb = num_blocks(p);
-    VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_backward: problem too large");
-    const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
-#define VIDAR_BWD(CVV)                                                                        \
-  if (p.ipw >= 32 / CVV)                                                                      \
-    msda_backward_small_kernel<CVV><<<grid, block, 0, st>>>(p, grad_out, grad_value,         \
-                                                            grad_sampling_loc, grad_attn_weight); \
-  else if (p.ipw > 1)                                                                         \
-    msda_backward_kernel<CVV, true><<<grid, block, 0, st>>>(p, grad_out, grad_value,          \
-                                                            grad_sampling_loc, grad_attn_weight); \
-  else                                                                                        \
-    msda_backward_kernel<CVV, false><<<grid, block, 0, st>>>(p, grad_out, grad_value,         \
-                                                             grad_sampling_loc, grad_attn_weight)
-    if (CV == 8) { VIDAR_BWD(8); }
-    else if (CV == 4) { VIDAR_BWD(4); }
-    else { VIDAR_BWD(16); }
-#undef VIDAR_BWD
-  } else {
-    cudaError_t e = cudaMemsetAsync(grad_sampling_loc, 0, sizeof(float) * 2 * (size_t)p.items * p.LP, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(grad_attn_weight, 0, sizeof(float) * (size_t)p.items * p.LP, st);
-    if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "ms_deform_attn_backward: memset: %s", cudaGetErrorString(e));
-    const long long n = p.items * C;
-    const long long nb = (n + 255) / 256;
-    VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_backward: problem too large");
-    msda_backward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight);
-  }
+  if (vec_ok(p))
+    return launch_vec_backward<false, false>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight, st,
+                                             "ms_deform_attn_backward");
+  cudaError_t e = cudaMemsetAsync(grad_sampling_loc, 0, sizeof(float) * 2 * (size_t)p.items * p.LP, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(grad_attn_weight, 0, sizeof(float) * (size_t)p.items * p.LP, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "ms_deform_attn_backward: memset: %s", cudaGetErrorString(e));
+  const long long n = p.items * C;
+  const long long nb = (n + 255) / 256;
+  VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_backward: problem too large");
+  msda_backward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight);
   return check_launch("ms_deform_attn_backward");
 }
 
@@ -1444,16 +1338,7 @@ extern "C" int vidar_msda_sca_forward(const float* value, const int64_t* spatial
   rc = check_sca(p, ref_points, D, who);
   if (rc) return rc;
   VIDAR_REQUIRE(out, "%s: null output", who);
-  if (slab_ok(p) && slab_forward_on()) return launch_slab_forward<true, false>(p, out, (cudaStream_t)stream, who);
-  set_ipw(p, C / 4);
-  const long long nb = num_blocks(p);
-  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
-  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (C == 32) msda_forward_kernel<8, false, true><<<grid, block, 0, st>>>(p, out);
-  else if (C == 16) msda_forward_kernel<4, false, true><<<grid, block, 0, st>>>(p, out);
-  else msda_forward_kernel<16, false, true><<<grid, block, 0, st>>>(p, out);
-  return check_launch(who);
+  return launch_vec_forward<true, false>(p, out, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_sca_backward(const float* value, const int64_t* spatial_shapes,
@@ -1469,16 +1354,7 @@ extern "C" int vidar_msda_sca_backward(const float* value, const int64_t* spatia
   if (rc) return rc;
   VIDAR_REQUIRE(grad_out && grad_value && grad_offsets && grad_logits, "%s: null gradient pointer", who);
   p.na_bytes = 0xffffffffu;
-  if (slab_ok(p)) return launch_slab_backward<true, false>(p, grad_out, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
-  set_ipw(p, C / 4);
-  const long long nb = num_blocks(p);
-  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
-  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (C == 32) msda_backward_kernel<8, false, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_offsets, grad_logits);
-  else if (C == 16) msda_backward_kernel<4, false, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_offsets, grad_logits);
-  else msda_backward_kernel<16, false, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_offsets, grad_logits);
-  return check_launch(who);
+  return launch_vec_backward<true, false>(p, grad_out, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
 }
 
 // ---- row-indirect entry points: SpatialCrossAttention's rebatch / scatter-add fused into the op ------
@@ -1502,17 +1378,6 @@ static int fill_rows(MsdaParams& p, const int32_t* idx, const int32_t* count, co
   return VIDAR_OK;
 }
 
-#define VIDAR_ROWS_LAUNCH(KERNEL, EPI_, ...)                                                     \
-  do {                                                                                           \
-    const long long nb = num_blocks(p);                                                          \
-    VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);                              \
-    const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);                                   \
-    cudaStream_t st = (cudaStream_t)stream;                                                      \
-    if (p.C == 32) KERNEL<8, false, EPI_, true><<<grid, block, 0, st>>>(__VA_ARGS__);            \
-    else if (p.C == 16) KERNEL<4, false, EPI_, true><<<grid, block, 0, st>>>(__VA_ARGS__);       \
-    else KERNEL<16, false, EPI_, true><<<grid, block, 0, st>>>(__VA_ARGS__);                     \
-  } while (0)
-
 extern "C" int vidar_msda_rows_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
                                        const float* sampling_loc, const float* attn_weight, const int32_t* idx,
                                        const int32_t* count, const float* inv_count, float* slots, int bs, int ncl,
@@ -1529,9 +1394,7 @@ extern "C" int vidar_msda_rows_forward(const float* value, const int64_t* spatia
   // the streaming hint helps the plain forward but not this one, whose epilogue also sends 245 MB
   // of slot reductions through L2: plain loads here
   p.na_bytes = 0xffffffffu;
-  if (slab_ok(p) && slab_forward_on()) return launch_slab_forward<false, true>(p, slots, (cudaStream_t)stream, who);
-  VIDAR_ROWS_LAUNCH(msda_forward_kernel, false, p, slots);
-  return check_launch(who);
+  return launch_vec_forward<false, true>(p, slots, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_rows_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -1549,12 +1412,10 @@ extern "C" int vidar_msda_rows_backward(const float* value, const int64_t* spati
   if (rc) return rc;
   VIDAR_REQUIRE(grad_slots && grad_value && grad_sampling_loc && grad_attn_weight, "%s: null gradient pointer", who);
   p.na_bytes = 0xffffffffu;
-  if (slab_ok(p))
-    return launch_slab_backward<false, true>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, (cudaStream_t)stream, who);
+  cudaStream_t st = (cudaStream_t)stream;
   if (tile_backward_ok(p))
-    return launch_rows_backward_tiled<false>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, (cudaStream_t)stream, who);
-  VIDAR_ROWS_LAUNCH(msda_backward_kernel, false, p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight);
-  return check_launch(who);
+    return launch_rows_backward_tiled<false>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, st, who);
+  return launch_vec_backward<false, true>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, st, who);
 }
 
 extern "C" int vidar_msda_sca_rows_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -1572,9 +1433,7 @@ extern "C" int vidar_msda_sca_rows_forward(const float* value, const int64_t* sp
   if (rc) return rc;
   VIDAR_REQUIRE(slots, "%s: null output", who);
   p.na_bytes = 0xffffffffu;
-  if (slab_ok(p) && slab_forward_on()) return launch_slab_forward<true, true>(p, slots, (cudaStream_t)stream, who);
-  VIDAR_ROWS_LAUNCH(msda_forward_kernel, true, p, slots);
-  return check_launch(who);
+  return launch_vec_forward<true, true>(p, slots, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_sca_rows_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -1593,11 +1452,8 @@ extern "C" int vidar_msda_sca_rows_backward(const float* value, const int64_t* s
   if (rc) return rc;
   VIDAR_REQUIRE(grad_slots && grad_value && grad_offsets && grad_logits, "%s: null gradient pointer", who);
   p.na_bytes = 0xffffffffu;
-  if (slab_ok(p))
-    return launch_slab_backward<true, true>(p, grad_slots, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
+  cudaStream_t st = (cudaStream_t)stream;
   if (tile_backward_ok(p))
-    return launch_rows_backward_tiled<true>(p, grad_slots, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
-  VIDAR_ROWS_LAUNCH(msda_backward_kernel, true, p, grad_slots, grad_value, grad_offsets, grad_logits);
-  return check_launch(who);
+    return launch_rows_backward_tiled<true>(p, grad_slots, grad_value, grad_offsets, grad_logits, st, who);
+  return launch_vec_backward<true, true>(p, grad_slots, grad_value, grad_offsets, grad_logits, st, who);
 }
-#undef VIDAR_ROWS_LAUNCH
