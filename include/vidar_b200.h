@@ -240,6 +240,8 @@ int vidar_dvxlr_backward_fused(const float* sigma, const float* origin, const fl
  *   (projects/mmdet3d_plugin/bevformer/dense_heads/vidar_head_base.py:420-509, 586-592, 706-738)
  *   sigma  [F, Z, Y, X]  the F frame volumes of one batch element
  *   origin [F, 3], points [R, 3] (voxel units), frame [R] int32 frame of each ray (NULL = 0)
+ *   A ray whose frame is outside [0, F) (e.g. -1 for a padded row) is invalid: valid 0, ce / lse / dist / depth 0,
+ *   logits -inf, no gradient; only its frame entry is read.
  *   Per ray: sample 0 = the GT point (with_gt), then num_way waypoints at
  *   o + u*(k+0.5)*step; K = num_way + with_gt samples; logit = trilinear grid_sample
  *   (align_corners=False, zeros) or -inf where any normalised coordinate leaves (-1,1).
@@ -452,6 +454,38 @@ int vidar_eval_metrics(const float* pred, const float* gt, const float* origin, 
                        const int64_t* gt_off, const int64_t* q_off, const unsigned char* q_mask,
                        const float* dists, const int64_t* idx, double* partials, double* out, float* rays,
                        int N, int max_len, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * (v) The head's dense loss term 'loss.dense_voxel' (dense_heads/vidar_head_base.py:594-659, get_rendered_pcds
+ *   :344-389): Chamfer distance between the decoded dense rays and the GT cloud of every (sample, frame) pair,
+ *   S = bs * F pairs, n = b * F + f, in a fixed number of launches and without a host sync.
+ *   dist      [bs, F*R0]     decoded ray lengths, frame-major: rays f*R0 .. (f+1)*R0-1 belong to frame f
+ *   points    [bs, F*R0, 3]  ray end points (voxel units);  origin [bs, To, 3], To >= F (voxel units)
+ *   gt        [bs, M, 3], gt_tindex [bs, M] (float frame, -1 = padding, any order; NULL when M = 0)
+ *   weights_host [F] per-frame loss weights, weight_sum = sum of all loss weights (HOST); loss divides by
+ *   weight_sum * bs.  pc_range_host: 6 floats (HOST), used when within_grid (the reference's
+ *   get_inside_mask on the voxel-unit end points).  W, H, Z: the grid size (gt box 0 < x < W-1, ...).
+ *   Pred cloud of n: rays with dist > 0, point (o + unit(p - o) * dist - o) * 0.1; gt cloud of n: rows with
+ *   gt_tindex == f strictly inside the box, (g - o) * 0.1, in row order (it decides NN ties).
+ * Forward outputs (Pq = bs*F*R0 + bs*M; all but loss are also inputs of the backward):
+ *   qbuf, cbuf [Pq, 3]; q_mask, c_mask [Pq]; q_off, c_off [2S+1] int64; idx [Pq] int64: the search layout
+ *   (segments 0..S-1 pred -> gt, S..2S-1 gt -> pred) and each query's nearest neighbour
+ *   pairs [S, 4] fp64: sum pred->gt squared distances, pred points, sum gt->pred, gt points
+ *   loss [1]: sum_n w_f * (mean pred->gt + mean gt->pred) / 2 / (weight_sum * bs) over pairs with gt points;
+ *   NaN when a pair has gt points but no pred point.  Fixed-order fp64 sums: the same bits on every call.
+ * Scratch from the library's memory pool.  Backward: grad_dist [bs, F*R0] fully overwritten (0 for rays
+ * outside the pred cloud), grad_loss [1] the upstream gradient (device). */
+int vidar_dense_chamfer_forward(const float* dist, const float* points, const float* origin, const float* gt,
+                                const float* gt_tindex, const float* weights_host, const float* pc_range_host,
+                                float weight_sum, float* qbuf, float* cbuf, unsigned char* q_mask,
+                                unsigned char* c_mask, int64_t* q_off, int64_t* c_off, int64_t* idx, double* pairs,
+                                float* loss, int bs, int F, int R0, int To, int M, int W, int H, int Z,
+                                int within_grid, void* stream);
+int vidar_dense_chamfer_backward(const float* points, const float* origin, const float* qbuf, const float* cbuf,
+                                 const unsigned char* q_mask, const int64_t* q_off, const int64_t* c_off,
+                                 const int64_t* idx, const double* pairs, const float* weights_host,
+                                 float weight_sum, const float* grad_loss, float* grad_dist, int bs, int F, int R0,
+                                 int To, int M, void* stream);
 
 #ifdef __cplusplus
 }

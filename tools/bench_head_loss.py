@@ -1,0 +1,121 @@
+"""Time ViDARRayHead.loss forward + backward at the pre-training head shape, with the dense Chamfer term batched
+(`fuse_dense_chamfer = True`, the default) and through the per-pair loop it replaced, alternating in one process.
+
+    python tools/bench_head_loss.py [--steps 20] [--warmup 3] [--gt 10000 30000]
+
+Shape: bs 1, 4 valid frames, 200 x 200 x 16 sigma, ray_grid_num 512, 10 000 dense rays per frame (the 50 x 50 x 4
+dense grid), CE + dense (use_dist_loss=False, the vidar_pretrain configuration).  Both paths get the same inputs
+and the same pre-drawn Gumbel noise, so their outputs are compared at the timed size.  Per path: median time of
+loss + backward by CUDA events, vidar_b200 kernel launches per call, and host syncs per call counted in a separate
+pass under torch.cuda.set_sync_debug_mode("warn").  The card's name and power limit are read in the same run.
+Prints one JSON line per GT size."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import warnings
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from vidar_b200 import _lib  # noqa: E402
+from vidar_b200.head import ViDARRayHead  # noqa: E402
+
+F, H, W, Z, NUM_WAY = 4, 200, 200, 16, 512
+PC_RANGE = [-51.2, -51.2, -5.0, 51.2, 51.2, 3.0]
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                       text=True).stdout.strip().splitlines()
+    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
+
+
+def inputs(gt_per_frame, seed=0):
+    dev = torch.device("cuda")
+    g = torch.Generator().manual_seed(seed)
+    preds = torch.randn(F, 1, 1, H * W, Z, generator=g).to(dev)
+    n = gt_per_frame * F
+    lo, hi = torch.tensor(PC_RANGE[:3]), torch.tensor(PC_RANGE[3:])
+    xyz = lo + (hi - lo) * torch.rand(n, 3, generator=g)
+    t = torch.randint(0, F, (n, 1), generator=g).float()
+    gt = [torch.cat([xyz, torch.rand(n, 1, generator=g), t], 1).to(dev)]
+    origin = torch.randn(1, F, 3, generator=g).to(dev)
+    R = (H // 4) * (W // 4) * (Z // 4) * F
+    noise = {"dense": (-torch.empty(1, R, NUM_WAY).exponential_(generator=g).log()).to(dev)}
+    kw = dict(start_idx=0, tgt_bev_h=H, tgt_bev_w=W, tgt_pc_range=PC_RANGE, pred_frame_num=F,
+              batched_origin_points=origin, gumbels=noise)
+    return preds, gt, kw
+
+
+def call(head, preds, gt, kw):
+    p = preds.clone().requires_grad_(True)
+    out = head.loss(dict(next_bev_preds=p, valid_frames=list(range(F))), gt, **kw)
+    sum(out.values()).backward()
+    return out, p.grad
+
+
+def count_syncs(head, preds, gt, kw):
+    torch.cuda.synchronize()
+    with warnings.catch_warnings(record=True) as rec:
+        warnings.simplefilter("always")
+        torch.cuda.set_sync_debug_mode("warn")
+        try:
+            call(head, preds, gt, kw)
+        finally:
+            torch.cuda.set_sync_debug_mode("default")
+    torch.cuda.synchronize()
+    syncs = [w for w in rec if "called a synchronizing CUDA operation" in str(w.message)]
+    return len(syncs), sorted({f"{os.path.relpath(w.filename, ROOT)}:{w.lineno}" for w in syncs})
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--gt", type=int, nargs="+", default=[10000, 30000])
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_head_loss needs a CUDA device")
+    heads = {}
+    for fused in (True, False):
+        h = ViDARRayHead(ray_grid_num=NUM_WAY, loss_weight=np.ones((F, 1)))
+        h.fuse_dense_chamfer = fused
+        heads["batched" if fused else "per_pair"] = h
+    name = card()
+    for n_gt in a.gt:
+        preds, gt, kw = inputs(n_gt)
+        res = {k: dict(ms=[]) for k in heads}
+        outs = {}
+        for k, h in heads.items():
+            for _ in range(a.warmup):
+                call(h, preds, gt, kw)
+            n0 = _lib.launch_count()
+            outs[k] = call(h, preds, gt, kw)
+            torch.cuda.synchronize()
+            res[k]["launches"] = _lib.launch_count() - n0
+        for _ in range(a.steps):
+            for k, h in heads.items():                 # alternate the two paths
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                call(h, preds, gt, kw)
+                e1.record()
+                e1.synchronize()
+                res[k]["ms"].append(e0.elapsed_time(e1))
+        for k, h in heads.items():
+            res[k]["syncs"], res[k]["sync_sites"] = count_syncs(h, preds, gt, kw)
+            res[k]["median_ms"] = round(float(np.median(res[k].pop("ms"))), 3)
+        (ob, gb), (op, gp) = outs["batched"], outs["per_pair"]
+        ob, op = ({k: float(v.detach()) for k, v in o.items()} for o in (ob, op))
+        cmp = {k: dict(batched=ob[k], per_pair=op[k], rel_diff=abs(ob[k] - op[k]) / max(abs(op[k]), 1e-30)) for k in ob}
+        cmp["grad_max_abs_diff_over_max"] = float((gb - gp).abs().max() / gp.abs().max())
+        print(json.dumps(dict(tool="bench_head_loss", card=name, bs=1, frames=F, sigma=[H, W, Z], ray_grid_num=NUM_WAY,
+                              dense_rays_per_frame=(H // 4) * (W // 4) * (Z // 4), gt_per_frame=n_gt, steps=a.steps,
+                              paths=res, compare=cmp)), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -61,4 +61,29 @@ __device__ __forceinline__ void red_add_f32(float* p, float v) {
   asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
 }
 
+// Segment of a flat index: the largest n with off[n] <= p, for off[0] <= p < off[N] (empty segments are skipped).
+__device__ __forceinline__ int find_segment(const int64_t* __restrict__ off, int N, int64_t p) {
+  int lo = 0, hi = N;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= p) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// Fixed-order fp64 sum over a block of kThreads threads (warp tree, then the warps in order); the result is valid
+// in thread 0.  `red`: kThreads / 32 doubles of shared memory.
+template <int kThreads>
+__device__ __forceinline__ double block_sum(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < kThreads / 32; ++w) s += red[w];
+  return s;
+}
+
 }  // namespace vidar

@@ -29,15 +29,6 @@ __constant__ float kSlack[6] = {(float)(-70.0 - 0.02), (float)(-70.0 - 0.02), (f
                              (float)(70.0 + 0.02), (float)(70.0 + 0.02), (float)(4.5 + 0.02)};
 constexpr float kMaxValue = 1e8f;
 
-__device__ __forceinline__ int find_segment(const int64_t* __restrict__ off, int N, int64_t p) {
-  int lo = 0, hi = N;               // largest n with off[n] <= p  (p < off[N])
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= p) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 __device__ __forceinline__ float norm3(float x, float y, float z) {      // sqrt(x*x + y*y + z*z), numpy order
   return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
 }
@@ -193,18 +184,6 @@ __global__ void eval_prologue_kernel(const float* __restrict__ pred, const float
   else q_mask[Pp + Pg + p] = far;
 }
 
-__device__ __forceinline__ double block_sum(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < kEvalThreads / 32; ++w) s += red[w];
-  return s;
-}
-
 // Per (block, segment) partials: [a, b, c, flags].  Forward / backward Chamfer segments: a = sum of squared NN
 // distances of the kept queries, b = their count.  Ray segments (one thread per gt point): a = sum l1,
 // b = sum absrel, c = kept gt points (`count`), flags = VIDAR_EVAL_* of the failures the reference raises.
@@ -270,9 +249,9 @@ eval_partials_kernel(const float* __restrict__ pred, const float* __restrict__ g
       }
     }
   }
-  a = block_sum(a, red);
-  b = block_sum(b, red);
-  c = block_sum(c, red);
+  a = block_sum<kEvalThreads>(a, red);
+  b = block_sum<kEvalThreads>(b, red);
+  c = block_sum<kEvalThreads>(c, red);
   flags = __reduce_or_sync(0xffffffffu, flags);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = (double)flags;

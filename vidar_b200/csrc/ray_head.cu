@@ -39,6 +39,7 @@ struct Sample {
 struct RaySetup {
   float ox, oy, oz, gx, gy, gz, ux, uy, uz;
   int f;
+  bool live;          // frame in [0, F): a ray of another frame (e.g. -1 for padding) is skipped, nothing is read
 };
 
 __device__ __forceinline__ RaySetup load_ray(const RayDims& D, const float* __restrict__ origin,
@@ -46,6 +47,8 @@ __device__ __forceinline__ RaySetup load_ray(const RayDims& D, const float* __re
                                              const int32_t* __restrict__ frame, int r) {
   RaySetup s;
   s.f = frame ? frame[r] : 0;
+  s.live = s.f >= 0 && s.f < D.F;
+  if (!s.live) return s;
   const float* o = origin + (size_t)s.f * 3;
   s.ox = o[0]; s.oy = o[1]; s.oz = o[2];
   s.gx = points[(size_t)r * 3]; s.gy = points[(size_t)r * 3 + 1]; s.gz = points[(size_t)r * 3 + 2];
@@ -146,7 +149,14 @@ ray_sample_kernel(RayDims D, const float* __restrict__ sigma, const float* __res
   const RaySetup s = load_ray(D, origin, points, frame, r);
   const float* vol = sigma + (size_t)s.f * D.Z * D.Y * D.X;
   const int K = D.num_way + D.with_gt;
-  if (valid && lane == 0) valid[r] = (!D.with_gt || gt_inside(D, s)) ? 1.f : 0.f;
+  if (valid && lane == 0) valid[r] = (s.live && (!D.with_gt || gt_inside(D, s))) ? 1.f : 0.f;
+  if (!s.live) {
+    for (int k = lane; k < K; k += 32) {
+      if (logits) logits[(size_t)r * K + k] = -INFINITY;
+      if (length) length[(size_t)r * K + k] = 0.f;
+    }
+    return;
+  }
   for (int k = lane; k < K; k += 32) {
     const Sample q = make_sample(D, s, k);
     float v = -INFINITY;
@@ -164,6 +174,7 @@ ray_sample_bwd_kernel(RayDims D, const float* __restrict__ origin, const float* 
   const int lane = threadIdx.x & 31;
   if (r >= D.R) return;
   const RaySetup s = load_ray(D, origin, points, frame, r);
+  if (!s.live) return;
   float* gvol = grad_sigma + (size_t)s.f * D.Z * D.Y * D.X;
   const int K = D.num_way + D.with_gt;
   for (int k = lane; k < K; k += 32) {
@@ -187,7 +198,7 @@ ray_ce_fwd_kernel(RayDims D, const float* __restrict__ sigma, const float* __res
   const int lane = threadIdx.x & 31;
   if (r >= D.R) return;
   const RaySetup s = load_ray(D, origin, points, frame, r);
-  if (!gt_inside(D, s)) {   // the reference drops the ray (:464-467)
+  if (!s.live || !gt_inside(D, s)) {   // the reference drops the ray (:464-467)
     if (lane == 0) { ce[r] = 0.f; lse_out[r] = 0.f; valid[r] = 0.f; }
     return;
   }
@@ -220,7 +231,7 @@ ray_ce_bwd_kernel(RayDims D, const float* __restrict__ sigma, const float* __res
   const float g = grad_ce ? grad_ce[r] : 1.f;
   if (g == 0.f) return;
   const RaySetup s = load_ray(D, origin, points, frame, r);
-  if (!gt_inside(D, s)) return;
+  if (!s.live || !gt_inside(D, s)) return;
   const size_t voff = (size_t)s.f * D.Z * D.Y * D.X;
   const float* vol = sigma + voff;
   float* gvol = grad_sigma + voff;
@@ -256,7 +267,7 @@ ray_gumbel_fwd_kernel(RayDims D, const float* __restrict__ sigma, const float* _
   const int lane = threadIdx.x & 31;
   if (r >= D.R) return;
   const RaySetup s = load_ray(D, origin, points, frame, r);
-  if (!gt_inside(D, s)) {
+  if (!s.live || !gt_inside(D, s)) {
     if (lane == 0) { dist[r] = 0.f; lse_out[r] = 0.f; p_out[r] = 0.f; }
     return;
   }
@@ -304,7 +315,7 @@ ray_gumbel_bwd_kernel(RayDims D, const float* __restrict__ sigma, const float* _
   const float g = grad_dist[r] * pred;
   if (g == 0.f) return;
   const RaySetup s = load_ray(D, origin, points, frame, r);
-  if (!gt_inside(D, s)) return;
+  if (!s.live || !gt_inside(D, s)) return;
   const size_t voff = (size_t)s.f * D.Z * D.Y * D.X;
   const float* vol = sigma + voff;
   float* gvol = grad_sigma + voff;
@@ -329,6 +340,13 @@ ray_argmax_kernel(RayDims D, const float* __restrict__ sigma, const float* __res
   const int lane = threadIdx.x & 31;
   if (r >= D.R) return;
   const RaySetup s = load_ray(D, origin, points, frame, r);
+  if (!s.live) {
+    if (lane == 0) {
+      depth[r] = 0.f;
+      if (index) index[r] = 0.f;
+    }
+    return;
+  }
   const float* vol = sigma + (size_t)s.f * D.Z * D.Y * D.X;
   float best = -INFINITY, best_len = 0.f;
   int best_k = 0x7fffffff;

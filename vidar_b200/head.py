@@ -14,10 +14,12 @@ arguments, returned keys and arithmetic
 
 What runs where: the CE term never materialises the [levels, rays, 513] logits
 (`ray_head.ce_regularization_loss`, one fused kernel per frame set); the dense term's gumbel decode
-is fused with the sampler as well (`ray_head.gumbel_distance`); the distance term samples through
-`ray_head.get_grid_features` (CUDA sampler) and then follows the reference's torch statements; Chamfer uses the nearest-neighbour kernel (`chamfer.knn_points`) in
-place of mmdet3d's O(N*M) distance matrix (`chamfer_distance`, criterion 'l2', reduction 'mean':
-the mean squared NN distance each way); decoding is `ray_head.decode_ray_depth`.
+is fused with the sampler as well (`ray_head.gumbel_distance`), and its Chamfer distance over every
+(sample, frame) pair is one batched op (`ray_head.dense_chamfer_loss`: segmented nearest-neighbour search in
+place of mmdet3d's O(N*M) distance matrix, `chamfer_distance` with criterion 'l2', reduction 'mean': the mean
+squared NN distance each way).  With CE + dense (use_dist_loss=False) `loss` runs forward and backward without
+a host sync.  The distance term samples through `ray_head.get_grid_features` (CUDA sampler) and then follows
+the reference's torch statements; decoding is `ray_head.decode_ray_depth`.
 CUDA only, like everything else in this package.
 """
 import numpy as np
@@ -59,6 +61,7 @@ class ViDARRayHead:
         assert self.loss_weight.shape[-1] == 1
         self.eval_within_grid = eval_within_grid
         self.fuse_dense_decode = True     # False: dense term through the materialising sampler + torch statements
+        self.fuse_dense_chamfer = True    # False: the reference's per-pair Chamfer loop (boolean masks, host syncs)
 
     # ------------------------------------------------------------------ ground truth (:219-276)
     def _process_gt_points(self, bev_preds, gt_points, batched_origin_points, valid_frames, start_idx,
@@ -82,8 +85,8 @@ class ViDARRayHead:
             order = torch.argsort(key, stable=True)
             keep = (key[order] < len(frames))
             srt = cur[order]
-            pts[b, : cur.shape[0]] = torch.where(keep[:, None], srt[:, :3].to(pts.dtype), pts.new_tensor(float("nan")))
-            tindex[b, : cur.shape[0]] = torch.where(keep, srt[:, -1].to(pts.dtype) - start_idx, pts.new_tensor(-1.0))
+            pts[b, : cur.shape[0]] = torch.where(keep[:, None], srt[:, :3].to(pts.dtype), float("nan"))
+            tindex[b, : cur.shape[0]] = torch.where(keep, srt[:, -1].to(pts.dtype) - start_idx, -1.0)
         if batched_origin_points is None:
             batched_origin_points = torch.zeros((bs, len(valid_frames), 3), dtype=bev_preds.dtype, device=bev_preds.device)
         origin_grids = bev_geometry.coords_to_voxel_grids(batched_origin_points, bev_h=bev_h, bev_w=bev_w,
@@ -190,22 +193,31 @@ class ViDARRayHead:
                 d_feat = d_feat[0][..., 1:].contiguous()
                 d_len = d_len[..., 1:].contiguous()
                 dense_dist = self._custom_gumbel_softmax_distance(d_feat, d_len, gumbels.get("dense"))
-            voxel_pcd = self.get_rendered_pcds(origin_grids, voxel_grids, voxel_tindex, dense_dist, dense_dist, tgt_pc_range)
-            dense = 0
-            for b in range(bs):
-                for f in range(valid_frame_num):
-                    pred = voxel_pcd[b][f].view(1, -1, 3)
-                    gt = gt_grids[b][gt_tindex[b] == f].view(1, -1, 3)
-                    m = ((gt[..., 0] < tgt_bev_w - 1) & (gt[..., 0] > 0) & (gt[..., 1] < tgt_bev_h - 1) & (gt[..., 1] > 0)
-                         & (gt[..., 2] < num_height_pred - 1) & (gt[..., 2] > 0))
-                    gt = gt.squeeze(0)[m.squeeze(0)][None]
-                    pred = (pred - origin_grids[b, f:f + 1]) * 0.1
-                    gt = (gt - origin_grids[b, f:f + 1]) * 0.1
-                    if gt.shape[1] == 0:
-                        continue
-                    loss_src, loss_tgt = chamfer_l2_mean(pred, gt)
-                    dense = dense + ((loss_src + loss_tgt) / 2.) * loss_weight[f, 0]
-            dense = dense / (loss_weight.sum() * bs)
+            if self.fuse_dense_chamfer:
+                # every (sample, frame) pair in one op: no boolean masks, no host sync
+                dense = ray_head.dense_chamfer_loss(
+                    dense_dist.contiguous(), voxel_grids.contiguous(), origin_grids.float().contiguous(),
+                    gt_grids.float().contiguous(), gt_tindex.float().contiguous(),
+                    (tgt_bev_w, tgt_bev_h, num_height_pred), [loss_weight[f, 0] for f in range(valid_frame_num)],
+                    float(loss_weight.sum()), self.eval_within_grid, tgt_pc_range)
+            else:
+                voxel_pcd = self.get_rendered_pcds(origin_grids, voxel_grids, voxel_tindex, dense_dist, dense_dist,
+                                                   tgt_pc_range)
+                dense = 0
+                for b in range(bs):
+                    for f in range(valid_frame_num):
+                        pred = voxel_pcd[b][f].view(1, -1, 3)
+                        gt = gt_grids[b][gt_tindex[b] == f].view(1, -1, 3)
+                        m = ((gt[..., 0] < tgt_bev_w - 1) & (gt[..., 0] > 0) & (gt[..., 1] < tgt_bev_h - 1)
+                             & (gt[..., 1] > 0) & (gt[..., 2] < num_height_pred - 1) & (gt[..., 2] > 0))
+                        gt = gt.squeeze(0)[m.squeeze(0)][None]
+                        pred = (pred - origin_grids[b, f:f + 1]) * 0.1
+                        gt = (gt - origin_grids[b, f:f + 1]) * 0.1
+                        if gt.shape[1] == 0:
+                            continue
+                        loss_src, loss_tgt = chamfer_l2_mean(pred, gt)
+                        dense = dense + ((loss_src + loss_tgt) / 2.) * loss_weight[f, 0]
+                dense = dense / (loss_weight.sum() * bs)
             loss_dict["loss.dense_voxel"] = dense * self.dense_loss_weight
         return loss_dict
 

@@ -10,11 +10,17 @@ projects/mmdet3d_plugin/bevformer/dense_heads/vidar_head_base.py:
                                  computed by the FUSED sampler+cross-entropy kernels: the
                                  [lvl, R, 513] logits are never materialised;
   decode_ray_depth(...)       == the per-(batch, frame) body of get_point_cloud_prediction
-                                 (:706-738): arg-max waypoint -> distance.
+                                 (:706-738): arg-max waypoint -> distance;
+  dense_chamfer_loss(...)     == the Chamfer loop of the `use_dense_loss` branch of ViDARHeadBase.loss
+                                 (:638-659) over every (sample, frame) pair in one batched op
+                                 (csrc/dense_chamfer.cu), no host sync.
 
 Low-level autograd ops: `ray_sample` (logits/lengths, differentiable w.r.t. sigma) and `ray_ce`.
 All tensors must be CUDA; there is no PyTorch fallback.
 """
+import ctypes as C
+
+import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
 
@@ -171,6 +177,20 @@ def ray_argmax(sigma, origin, points, frame, num_way, step):
     return depth, index
 
 
+def _host_weights(loss_weights, device):
+    """[frame, level] loss weights as a device tensor, by a pinned non-blocking copy (no host sync)."""
+    host = torch.from_numpy(np.ascontiguousarray(loss_weights, dtype=np.float32)).pin_memory()
+    return host.to(device, non_blocking=True)
+
+
+def _ray_frames(gt_tindex, num_frames):
+    """int32 frame of every ray: its tindex when that is a frame in [0, num_frames), else -1 (skipped by the
+    kernels).  No compaction, so no host sync."""
+    t = gt_tindex
+    keep = (t >= 0) & (t < num_frames) & (t == t.floor())     # `cur_tindex == frame_idx`
+    return torch.where(keep, t, -1.0).to(torch.int32).contiguous()
+
+
 def _frame_sorted_rays(gt_grids, gt_tindex, num_frames):
     """Rays of one batch element grouped by frame (frame-major, original order inside a frame,
     like the reference's double loop) -> (points [R,3], frame int32 [R])."""
@@ -223,15 +243,17 @@ def ce_regularization_loss(batched_origin_grids, batched_gt_grids, batched_gt_ti
     """`regularization.loss` of ViDARHeadBase.loss (:586-592) without materialising the logits:
     sum(ce * w) / clamp(sum(w), min=1) over intermediate levels and valid rays."""
     bs, F = intermediate_sigma[0].shape[:2]
-    lw = torch.as_tensor(loss_weights, dtype=torch.float32, device=batched_gt_grids.device)
+    lw = _host_weights(loss_weights, batched_gt_grids.device)
     num = batched_gt_grids.new_zeros(())
     den = batched_gt_grids.new_zeros(())
     for b in range(bs):
-        pts, frame = _frame_sorted_rays(batched_gt_grids[b], batched_gt_tindex[b], F)
+        # every row, rays of no predicted frame (padding, frame -1) contribute valid = 0
+        pts = batched_gt_grids[b].float().contiguous()
+        frame = _ray_frames(batched_gt_tindex[b], F)
         origin = batched_origin_grids[b, :F].contiguous().float()
         for lvl, sig in enumerate(intermediate_sigma):
             ce, valid = ray_ce(sig[b], origin, pts, frame, ray_grid_num, ray_grid_step)
-            w = lw[frame.long(), lvl] * valid
+            w = lw[frame.clamp(min=0).long(), lvl] * valid
             num = num + (ce * w).sum()
             den = den + w.sum()
     return num / torch.clamp(den, min=1)
@@ -253,3 +275,80 @@ def decode_ray_depth(sigma, origin_grids, gt_grids, gt_tindex, ray_grid_step, ra
     pred[idx] = depth
     gt[idx] = torch.sqrt(((pts - origin_grids[frame.long()]) ** 2).sum(-1))
     return pred, gt
+
+
+class _DenseChamfer(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, dist, points, origin, gt, gt_tindex, grid, weights, weight_sum, within_grid, pc_range):
+        dev = dist.device
+        bs, FR = dist.shape
+        F = len(weights)
+        R0 = FR // F
+        To, M = origin.shape[1], gt.shape[1]
+        W, H, Z = (int(v) for v in grid)
+        Pq = bs * FR + bs * M
+        S = bs * F
+        qbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
+        cbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
+        q_mask = torch.empty(Pq, dtype=torch.uint8, device=dev)
+        c_mask = torch.empty(Pq, dtype=torch.uint8, device=dev)
+        seg_off = torch.empty((2, 2 * S + 1), dtype=torch.int64, device=dev)
+        idx = torch.empty(Pq, dtype=torch.int64, device=dev)
+        pairs = torch.empty((S, 4), dtype=torch.float64, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        w = (C.c_float * F)(*weights)
+        rng = (C.c_float * 6)(*[float(v) for v in pc_range])
+        P = _lib.ptr
+        _call(_lib.lib().vidar_dense_chamfer_forward, dev, P(dist), P(points), P(origin), P(gt), P(gt_tindex),
+              C.cast(w, C.c_void_p), C.cast(rng, C.c_void_p), float(weight_sum), P(qbuf), P(cbuf), P(q_mask),
+              P(c_mask), P(seg_off[0]), P(seg_off[1]), P(idx), P(pairs), P(loss), bs, F, R0, To, M, W, H, Z,
+              int(bool(within_grid)))
+        ctx.save_for_backward(points, origin, qbuf, cbuf, q_mask, seg_off, idx, pairs)
+        ctx.meta = (tuple(weights), float(weight_sum), bs, F, R0, To, M)
+        ctx.mark_non_differentiable(pairs)
+        return loss, pairs
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_loss, _gp):
+        points, origin, qbuf, cbuf, q_mask, seg_off, idx, pairs = ctx.saved_tensors
+        weights, weight_sum, bs, F, R0, To, M = ctx.meta
+        g = grad_loss.float().contiguous()
+        grad_dist = torch.empty((bs, F * R0), dtype=torch.float32, device=qbuf.device)
+        w = (C.c_float * F)(*weights)
+        P = _lib.ptr
+        _call(_lib.lib().vidar_dense_chamfer_backward, qbuf.device, P(points), P(origin), P(qbuf), P(cbuf),
+              P(q_mask), P(seg_off[0]), P(seg_off[1]), P(idx), P(pairs), C.cast(w, C.c_void_p), weight_sum, P(g),
+              P(grad_dist), bs, F, R0, To, M)
+        return grad_dist, None, None, None, None, None, None, None, None, None
+
+
+def dense_chamfer_loss(dist, points, origin, gt, gt_tindex, grid, frame_weights, weight_sum, eval_within_grid=False,
+                       pc_range=None, return_pairs=False):
+    """`loss.dense_voxel` before its `dense_loss_weight` (vidar_head_base.py:594-659), every (sample, frame) pair
+    at once, differentiable in `dist`.
+
+    dist [bs, F*R0] decoded lengths (`gumbel_distance`), points [bs, F*R0, 3] frame-major ray end points, origin
+    [bs, >=F, 3], gt [bs, M, 3] and gt_tindex [bs, M] (float, -1 = padding, any order), all voxel units on one CUDA
+    device; grid = (W, H, Z); frame_weights: F host floats (loss_weight[f, 0]); weight_sum: loss_weight.sum(), the
+    loss divides by weight_sum * bs; pc_range: metres, used by eval_within_grid like get_rendered_pcds.
+    Returns the 0-dim loss (and, with return_pairs, [bs*F, 4] float64 per pair: sum pred->gt squared distances,
+    pred points, sum gt->pred, gt points)."""
+    _lib.require_cuda(dist=dist, points=points, origin=origin, gt=gt, gt_tindex=gt_tindex)
+    frame_weights = [float(v) for v in frame_weights]
+    F = len(frame_weights)
+    if dist.dim() != 2 or F == 0 or dist.shape[1] % F:
+        raise RuntimeError(f"dist must be [bs, F*R0] with F = {F} frame weights, got {tuple(dist.shape)}")
+    bs, FR = dist.shape
+    M = gt.shape[1] if gt.dim() == 3 else -1
+    if (tuple(points.shape) != (bs, FR, 3) or origin.dim() != 3 or origin.shape[0] != bs or origin.shape[1] < F
+            or origin.shape[2] != 3 or tuple(gt.shape) != (bs, M, 3) or tuple(gt_tindex.shape) != (bs, M)):
+        raise RuntimeError("expected points [bs, F*R0, 3], origin [bs, >=F, 3], gt [bs, M, 3], gt_tindex [bs, M]")
+    for name, t in (("dist", dist), ("points", points), ("origin", origin), ("gt", gt), ("gt_tindex", gt_tindex)):
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must be float32")
+    if eval_within_grid and pc_range is None:
+        raise RuntimeError("eval_within_grid needs pc_range")
+    loss, pairs = _DenseChamfer.apply(dist, points, origin, gt, gt_tindex, grid, frame_weights, weight_sum,
+                                      eval_within_grid, pc_range if pc_range is not None else [0.0] * 6)
+    return (loss, pairs) if return_pairs else loss
