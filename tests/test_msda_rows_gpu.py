@@ -3,7 +3,8 @@ sca.MSDARowsFunction (rows -> BEV slots, the benchmark's MSDA stage) against ora
 sca.SCARowsFunction (SpatialCrossAttention's fused path) against msda_ref.msda_sca_rows.  The slots and every
 gradient are held to tests/parity.py; grad_sampling_loc / grad_offsets skip samples on a pixel-centre line.
 
-They are also compared with the plain ops at 1e-5 (tighter than parity, shared arithmetic): per launch group
+They are also compared with the plain ops at 1e-5 (tighter than parity, shared arithmetic; where the rows take the
+tile kernel, grad_sampling_loc / grad_attn_weight must be bit-identical): per launch group
 `ms_deform_attn` / MSDeformAttn3DFusedFunction runs on the same rows with each row's grad_out set to its pillar's
 slot gradient times 1 / #cameras, and zero for rows outside the launch (dead list entries, other sub-slices).
 
@@ -97,9 +98,16 @@ def _check(dev, plan, bs, Qd, groups, shapes, lsi, idx=None, count=None, inv=Non
         rv, rl, ra = (t.detach().clone().requires_grad_(True) for t in (v, loc, aw))
         out = msda.MultiScaleDeformableAttnFunction_fp32.apply(rv, shapes, lsi, rl, ra, 64)
         out.backward(go.reshape(out.shape))
+        # the tile kernel's location / attention gradients are msda_backward_kernel's arithmetic: bit-identical.
+        # `tile` restates tile_backward_ok in csrc/msda.cu, which picks the tile kernel; keep the two in step.
+        K, C_, L, P_ = v.shape[1], v.shape[3], loc.shape[3], loc.shape[4]
+        tile = C_ == 32 and P_ == 8 and L * P_ == 32 and K < 2 ** 19
         for name, got_, want in (("grad_value", got[k][0], rv.grad), ("grad_loc", got[k][1], rl.grad),
                                  ("grad_attn", got[k][2], ra.grad)):
-            _close(f"group {k} {name}", got_, want)
+            if tile and name != "grad_value":
+                assert torch.equal(got_, want), f"group {k} {name}: tile kernel differs from ms_deform_attn"
+            else:
+                _close(f"group {k} {name}", got_, want)
 
 
 def _inputs(dev, n, rows, mode, seed, levels=SCA_LEVELS, heads=H, dim=C, points=P):

@@ -55,7 +55,6 @@ struct MsdaParams {
   const float* inv;    // [bs, Qd] output scale 1 / #cameras seeing the pillar, or nullptr
   int ncl, cam0, bs, Qd;   // cameras in this launch, first camera, batch size, pillars per batch element
   int S, s_lo, s_hi;   // the launch covers rows with (j / 64) % S in [s_lo, s_hi)   (rank sub-slices)
-  unsigned na_bytes;  // levels whose per-head slab (H_l*W_l*C*4 bytes) exceeds this stream past L1 (no_allocate)
 };
 
 // Decode one sample: pixel coordinates -> clamped base pixel, corner mask, fractions.
@@ -87,11 +86,36 @@ __device__ __forceinline__ void decode_sample(float lx, float ly, int Hl, int Wl
   }
 }
 
+// Bilinear corner weights of a decoded sample, pre-multiplied by its attention weight aw.  Invalid corners get
+// weight 0; their (clamped) address aliases a valid corner's pixel.
+__device__ __forceinline__ void corner_weights(int meta, float lh, float lw, float aw, float& w1, float& w2,
+                                               float& w3, float& w4) {
+  const float hh = 1.f - lh, hw = 1.f - lw;
+  w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
+  w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
+  w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
+  w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+}
+
+// Float offsets of a decoded sample's four corners inside its slab.  decode_sample's base and row step are in units
+// of `unit` floats (1 when it scaled them to floats, the pixel stride when it left them in pixels); the column step
+// is one pixel stride `pix`.
+__device__ __forceinline__ uint4 corner_offsets(int base, int meta, unsigned unit, unsigned pix) {
+  const unsigned o1 = (unsigned)base * unit;
+  const unsigned o2 = o1 + ((meta & 16) ? pix : 0u);
+  const unsigned o3 = o1 + (unsigned)(meta >> 5) * unit;
+  return make_uint4(o1, o2, o3, o3 + (o2 - o1));
+}
+
 // Cache policy of the gather.  The fine pyramid levels have (almost) no reuse inside an SM -- a
 // 24x24-pixel window per anchor and two samples in it -- while one head's coarse levels (15x25: 48 KB,
 // 29x50: 186 KB) are re-read by every query: fine-level lines are loaded with L1::no_allocate so they
-// do not evict the coarse slabs (kHintBit of a sample's meta word selects the policy).
+// do not evict the coarse slabs (kHintBit of a sample's meta word selects the policy).  msda_forward_kernel
+// decides where the policy applies.
 constexpr int kHintBit = 1 << 30;
+// Per-head level slabs (H_l*W_l*C*4 bytes) larger than this stream, so at the SpatialCrossAttention shape everything
+// but the 48 KB 15x25 level does (a sweep of the threshold at that shape chose it).
+constexpr unsigned kStreamBytes = 100000u;
 __device__ __forceinline__ float4 ldg4_na(const float* p) {
   float4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
@@ -118,6 +142,56 @@ __device__ __forceinline__ float4 f4_scale(float s, const float4& v) {
   return make_float4(__fmul_rn(s, v.x), __fmul_rn(s, v.y), __fmul_rn(s, v.z), __fmul_rn(s, v.w));
 }
 
+// Forward: sum of the NG groups' float4 partial head vectors over the warp (every group ends with the total).
+template <int CV>
+__device__ __forceinline__ float4 group_sum(float4 acc) {
+#pragma unroll
+  for (int off = CV; off < 32; off <<= 1) {
+    acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
+    acc.y += __shfl_xor_sync(0xffffffffu, acc.y, off);
+    acc.z += __shfl_xor_sync(0xffffffffu, acc.z, off);
+    acc.w += __shfl_xor_sync(0xffffffffu, acc.w, off);
+  }
+  return acc;
+}
+
+// Backward: (d1..d4) are this lane's channel share of sum_c g*v_k for the four corners of its group's sample.  A
+// transposed reduction over the CV lanes of the group takes 4 shuffles; afterwards lane class
+// (cl & CV/2, cl & CV/4) = (0,0):d1 (0,1):d2 (1,0):d3 (1,1):d4.  Returns, in every lane, the four sums of the group
+// whose first lane is `back`, for the lane that decoded that group's sample to keep.
+template <int CV>
+__device__ __forceinline__ float4 reduce_corners(float d1, float d2, float d3, float d4, int cl, int back) {
+  const bool up1 = (cl & (CV / 2)) != 0;
+  const float e0 = __shfl_xor_sync(0xffffffffu, up1 ? d1 : d3, CV / 2);
+  const float e1 = __shfl_xor_sync(0xffffffffu, up1 ? d2 : d4, CV / 2);
+  const float k0 = (up1 ? d3 : d1) + e0;    // lower half: d1   upper half: d3
+  const float k1 = (up1 ? d4 : d2) + e1;    // lower half: d2   upper half: d4
+  const bool up2 = (cl & (CV / 4)) != 0;
+  const float eb = __shfl_xor_sync(0xffffffffu, up2 ? k0 : k1, CV / 4);
+  float k = (up2 ? k1 : k0) + eb;
+#pragma unroll
+  for (int off = CV / 8; off >= 1; off >>= 1) k += __shfl_xor_sync(0xffffffffu, k, off);
+  const float t1 = __shfl_sync(0xffffffffu, k, back);
+  const float t2 = __shfl_sync(0xffffffffu, k, back + CV / 4);
+  const float t3 = __shfl_sync(0xffffffffu, k, back + CV / 2);
+  const float t4 = __shfl_sync(0xffffffffu, k, back + CV / 2 + CV / 4);
+  return make_float4(t1, t2, t3, t4);
+}
+
+// Backward, in the lane that decoded the sample: its corner sums r (sum_c g*v_k) -> the gradients of its attention
+// weight (ga) and of its location (gx, gy).  An out-of-image corner contributes v = 0 to every gradient (mmcv
+// col2im_bilinear).
+__device__ __forceinline__ void sample_grads(int meta, float lh, float lw, float aw, float fW, float fH,
+                                             const float4& r, float& ga, float& gx, float& gy) {
+  const float hh = 1.f - lh, hw = 1.f - lw;
+  const float r1 = (meta & 1) ? r.x : 0.f, r2 = (meta & 2) ? r.y : 0.f;
+  const float r3 = (meta & 4) ? r.z : 0.f, r4 = (meta & 8) ? r.w : 0.f;
+  const bool ok = (meta & 15) != 0;
+  ga = ok ? (hh * hw) * r1 + (hh * lw) * r2 + (lh * hw) * r3 + (lh * lw) * r4 : 0.f;
+  gx = ok ? fW * aw * (hh * (r2 - r1) + lh * (r4 - r3)) : 0.f;
+  gy = ok ? fH * aw * (hw * (r3 - r1) + lw * (r4 - r2)) : 0.f;
+}
+
 
 // EPI (MSDeformableAttention3D, spatial_cross_attention.py:339-371 folded into the kernel): lane s
 // holds sample s = l*P + p of one (b,q,h); the attention weight is the softmax of the 32 logits
@@ -134,6 +208,9 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+__device__ __forceinline__ float2 epi_loc(float2 off, float Wl, float Hl, float2 r) {
+  return make_float2(__fadd_rn(__fdiv_rn(off.x, Wl), r.x), __fadd_rn(__fdiv_rn(off.y, Hl), r.y));
+}
 __device__ __forceinline__ void epi_decode(const MsdaParams& p, size_t refrow, int s, float Wl, float Hl,
                                            const float* loc0, const float* att0, float2& xy, float& aw) {
   const float logit = __ldg(att0 + s);
@@ -142,8 +219,7 @@ __device__ __forceinline__ void epi_decode(const MsdaParams& p, size_t refrow, i
   const float2 off = __ldg(reinterpret_cast<const float2*>(loc0) + s);
   const int z = (s % p.P) % p.D;
   const float2 r = __ldg(reinterpret_cast<const float2*>(p.ref) + refrow + z);   // refrow: anchor 0 of this row
-  xy.x = __fadd_rn(__fdiv_rn(off.x, Wl), r.x);
-  xy.y = __fadd_rn(__fdiv_rn(off.y, Hl), r.y);
+  xy = epi_loc(off, Wl, Hl, r);
 }
 
 // Which (b,q,h) items does this warp own?  Returns false if none.
@@ -188,6 +264,21 @@ struct Row {
   size_t refrow;     // float2 index of the row's Z-anchor 0 in p.ref
   float inv;         // output scale
 };
+// Is list entry j of batch element n one of this launch's rows?  (below its camera's live count, in the launch's
+// sub-slice.)  Signed indexing: with unsigned arithmetic here rows_key_kernel<false> spills at its 32 registers.
+__device__ __forceinline__ bool row_live(const MsdaParams& p, int n, int j) {
+  if (p.count && j >= __ldg(p.count + p.cam0 + n % p.ncl)) return false;
+  if (p.S > 1) {
+    const int sl = (j >> 6) % p.S;
+    if (sl < p.s_lo || sl >= p.s_hi) return false;
+  }
+  return true;
+}
+// float2 index of Z-anchor 0 of camera c's row for pillar q of batch element b in reference_points_cam
+// [cams, bs, Qd, D, 2]
+__device__ __forceinline__ size_t anchor_row(const MsdaParams& p, size_t c, size_t b, size_t q) {
+  return ((c * p.bs + b) * p.Qd + q) * p.D;
+}
 template <bool IDX>
 __device__ __forceinline__ bool resolve_row(const MsdaParams& p, long long item0, Row& r) {
   if (!IDX) {
@@ -202,15 +293,11 @@ __device__ __forceinline__ bool resolve_row(const MsdaParams& p, long long item0
   const unsigned j = nj % (unsigned)p.Q, n = nj / (unsigned)p.Q;
   const unsigned cl = n % (unsigned)p.ncl, b = n / (unsigned)p.ncl;
   const unsigned c = (unsigned)p.cam0 + cl;
-  if (p.count && (int)j >= __ldg(p.count + c)) return false;
-  if (p.S > 1) {
-    const int sl = (int)((j >> 6) % (unsigned)p.S);
-    if (sl < p.s_lo || sl >= p.s_hi) return false;
-  }
+  if (!row_live(p, (int)n, (int)j)) return false;
   const unsigned q = p.idx ? (unsigned)__ldg(p.idx + (size_t)c * p.Qd + j) : j;
   const size_t bq = (size_t)b * p.Qd + q;
   r.dense = (long long)(bq * p.H + h);
-  r.refrow = (((size_t)c * p.bs + b) * p.Qd + q) * p.D;             // reference_points_cam [cams, bs, Qd, D, 2]
+  r.refrow = anchor_row(p, c, b, q);
   r.inv = p.inv ? __ldg(p.inv + bq) : 1.f;
   return true;
 }
@@ -222,13 +309,7 @@ __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
 template <int CV>
 __device__ __forceinline__ void store_item(const MsdaParams& p, float* __restrict__ out,
                                            long long item, float4 acc, int g, int cl) {
-#pragma unroll
-  for (int off = CV; off < 32; off <<= 1) {
-    acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
-    acc.y += __shfl_xor_sync(0xffffffffu, acc.y, off);
-    acc.z += __shfl_xor_sync(0xffffffffu, acc.z, off);
-    acc.w += __shfl_xor_sync(0xffffffffu, acc.w, off);
-  }
+  acc = group_sum<CV>(acc);
   if (g == 0 && item < p.items)
     *reinterpret_cast<float4*>(out + (size_t)item * p.C + cl * 4) = acc;
 }
@@ -239,6 +320,11 @@ __device__ __forceinline__ void store_item(const MsdaParams& p, float* __restric
 template <int CV, bool MULTI, bool EPI = false, bool IDX = false>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 6)
 msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
+  // The streaming hint (kStreamBytes, ldg4_na) applies to this kernel without IDX and nowhere else.  The backward
+  // keeps plain loads: they share the LSU -> XBAR request path with the reductions, and a no-allocate miss cannot
+  // merge with a neighbouring warp's pending miss.  The rows forward (IDX) keeps them too: its epilogue also sends
+  // 245 MB of slot reductions through L2.
+  constexpr bool NA = !IDX;
   constexpr int NG = 32 / CV;       // sample groups per warp
   constexpr int ITERS = 32 / NG;    // == CV
   const int lane = threadIdx.x & 31;
@@ -253,13 +339,15 @@ msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
   const int nchunks = MULTI ? 1 : (span + 31) >> 5;
   // fused prologue + IDX: offsets / logits exist once per pillar (dense); otherwise per row
   const long long prow = (EPI && IDX) ? row.dense : item0;
-  const float* loc0 = p.loc + (size_t)prow * p.LP * 2;
-  const float* att0 = p.attn + (size_t)prow * p.LP;
   const float* vb = p.value + slab_offset(p, item0) + cl * 4;   // moves with the item (MULTI)
+  float* slot = IDX ? out + (size_t)row.dense * p.C + cl * 4 : out;   // IDX: this lane's share of the BEV slot
   const unsigned pix = (unsigned)p.pix_stride;
 
   float4 acc = f4_zero();
   for (int chunk = 0; chunk < nchunks; ++chunk) {
+    // derived per chunk, not kept live through the sample loop (the IDX forwards spill at 40 registers otherwise)
+    const float* loc0 = p.loc + (size_t)prow * p.LP * 2;
+    const float* att0 = p.attn + (size_t)prow * p.LP;
     // ---- lane j decodes sample j of the chunk; weights are pre-multiplied by attention
     const int s = chunk * 32 + lane;
     int base = 0, meta = 0;
@@ -279,13 +367,8 @@ msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
       }
       float lh, lw;
       decode_sample(xy.x, xy.y, Hl, Wl, (int)__ldg(p.lsi + l), base, meta, lh, lw, p.pix_stride);
-      if (meta && (unsigned)(Hl * Wl) * (unsigned)p.C * 4u > p.na_bytes) meta |= kHintBit;
-      const float hh = 1.f - lh, hw = 1.f - lw;
-      // invalid corners get weight 0; their (clamped) address aliases a valid corner's pixel
-      w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
-      w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
-      w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
-      w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+      if (NA && meta && (unsigned)(Hl * Wl) * (unsigned)p.C * 4u > kStreamBytes) meta |= kHintBit;
+      corner_weights(meta, lh, lw, aw, w1, w2, w3, w4);
     }
 #pragma unroll
     for (int it = 0; it < ITERS; ++it) {
@@ -308,15 +391,12 @@ msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
       asm volatile("" : "+l"(vbi));   // keep the slab base in a 64-bit register pair
       if (smeta & 15) {
         // four independent 16-byte loads, issued back to back (32-bit offsets, 64-bit base)
-        const unsigned o1 = (unsigned)sbase;                       // float offsets inside the slab
-        const unsigned o2 = o1 + ((smeta & 16) ? pix : 0u);
-        const unsigned o3 = o1 + (unsigned)((smeta & ~kHintBit) >> 5);
-        const unsigned o4 = o3 + (o2 - o1);
-        const bool na = (smeta & kHintBit) != 0;      // warp-uniform when a level's points fill whole iterations
-        const float4 v1 = ldg4_h(vbi + o1, na);
-        const float4 v2 = ldg4_h(vbi + o2, na);
-        const float4 v3 = ldg4_h(vbi + o3, na);
-        const float4 v4 = ldg4_h(vbi + o4, na);
+        const uint4 o = corner_offsets(sbase, smeta & ~kHintBit, 1u, pix);
+        const bool na = NA && (smeta & kHintBit) != 0;   // warp-uniform when a level's points fill whole iterations
+        const float4 v1 = ldg4_h(vbi + o.x, na);
+        const float4 v2 = ldg4_h(vbi + o.y, na);
+        const float4 v3 = ldg4_h(vbi + o.z, na);
+        const float4 v4 = ldg4_h(vbi + o.w, na);
         f4_fma(acc, a1, v1);
         f4_fma(acc, a2, v2);
         f4_fma(acc, a3, v3);
@@ -327,14 +407,8 @@ msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
   if (IDX) {
     // SpatialCrossAttention's scatter-add + count normalisation (spatial_cross_attention.py:164-171) as
     // the epilogue: the head vector goes straight into the BEV slot of its pillar.
-#pragma unroll
-    for (int off = CV; off < 32; off <<= 1) {
-      acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
-      acc.y += __shfl_xor_sync(0xffffffffu, acc.y, off);
-      acc.z += __shfl_xor_sync(0xffffffffu, acc.z, off);
-      acc.w += __shfl_xor_sync(0xffffffffu, acc.w, off);
-    }
-    if (g == 0) red_add_v4(out + (size_t)row.dense * p.C + cl * 4, f4_scale(row.inv, acc));
+    acc = group_sum<CV>(acc);
+    if (g == 0) red_add_v4(slot, f4_scale(row.inv, acc));
     return;
   }
   store_item<CV>(p, out, MULTI ? item0 + p.ipw - 1 : item0, acc, g, cl);
@@ -388,16 +462,11 @@ msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
         aw = __ldg(att0 + s);
       }
       decode_sample(xy.x, xy.y, Hl, Wl, (int)__ldg(p.lsi + l), base, meta, lh, lw, p.pix_stride);
-      if (meta && (unsigned)(Hl * Wl) * (unsigned)p.C * 4u > p.na_bytes) meta |= kHintBit;
       fH = (float)Hl;
       fW = (float)Wl;
-      const float hh = 1.f - lh, hw = 1.f - lw;
-      w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
-      w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
-      w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
-      w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+      corner_weights(meta, lh, lw, aw, w1, w2, w3, w4);
     }
-    float r1 = 0.f, r2 = 0.f, r3 = 0.f, r4 = 0.f;   // this lane's sample: sum_c g*v_k
+    float4 r = f4_zero();   // this lane's sample: sum_c g*v_k
 #pragma unroll
     for (int it = 0; it < ITERS; ++it) {
       if (!MULTI && chunk * 32 + it * NG >= span) break;
@@ -419,58 +488,30 @@ msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
       }
       float d1 = 0.f, d2 = 0.f, d3 = 0.f, d4 = 0.f;
       if (smeta & 15) {
-        const unsigned o1 = (unsigned)sbase;                       // float offsets inside the slab
-        const unsigned o2 = o1 + ((smeta & 16) ? pix : 0u);
-        const unsigned o3 = o1 + (unsigned)((smeta & ~kHintBit) >> 5);
-        const unsigned o4 = o3 + (o2 - o1);
+        const uint4 o = corner_offsets(sbase, smeta, 1u, pix);
         const float* vs = p.value + slab;
         float* gs = grad_value + slab;
         asm volatile("" : "+l"(vs), "+l"(gs));
-        const bool na = (smeta & kHintBit) != 0;
-        const float4 v1 = ldg4_h(vs + o1, na);
-        const float4 v2 = ldg4_h(vs + o2, na);
-        const float4 v3 = ldg4_h(vs + o3, na);
-        const float4 v4 = ldg4_h(vs + o4, na);
+        const float4 v1 = ldg4(vs + o.x);
+        const float4 v2 = ldg4(vs + o.y);
+        const float4 v3 = ldg4(vs + o.z);
+        const float4 v4 = ldg4(vs + o.w);
         // grad_value: top_grad * attn * corner weight as 16-byte vector reductions.  An
         // out-of-image corner has weight 0 and aliases a valid pixel: its reduction adds 0.
-        red_add_v4(gs + o1, f4_scale(a1, go));
-        red_add_v4(gs + o2, f4_scale(a2, go));
-        red_add_v4(gs + o3, f4_scale(a3, go));
-        red_add_v4(gs + o4, f4_scale(a4, go));
+        red_add_v4(gs + o.x, f4_scale(a1, go));
+        red_add_v4(gs + o.y, f4_scale(a2, go));
+        red_add_v4(gs + o.z, f4_scale(a3, go));
+        red_add_v4(gs + o.w, f4_scale(a4, go));
         d1 = f4_dot(go, v1); d2 = f4_dot(go, v2); d3 = f4_dot(go, v3); d4 = f4_dot(go, v4);
       }
-      // ---- transposed reduction of (d1..d4) over the CV lanes of the group: 4 shuffles;
-      //      afterwards lane class (cl & CV/2, cl & CV/4) = (0,0):d1 (0,1):d2 (1,0):d3 (1,1):d4
-      const bool up1 = (cl & (CV / 2)) != 0;
-      const float e0 = __shfl_xor_sync(0xffffffffu, up1 ? d1 : d3, CV / 2);
-      const float e1 = __shfl_xor_sync(0xffffffffu, up1 ? d2 : d4, CV / 2);
-      const float k0 = (up1 ? d3 : d1) + e0;    // lower half: d1   upper half: d3
-      const float k1 = (up1 ? d4 : d2) + e1;    // lower half: d2   upper half: d4
-      const bool up2 = (cl & (CV / 4)) != 0;
-      const float eb = __shfl_xor_sync(0xffffffffu, up2 ? k0 : k1, CV / 4);
-      float k = (up2 ? k1 : k0) + eb;
-#pragma unroll
-      for (int off = CV / 8; off >= 1; off >>= 1) k += __shfl_xor_sync(0xffffffffu, k, off);
-      // ---- hand the four sums back to the lane that decoded the sample (lane it*NG + g')
-      const int back = (lane & (NG - 1)) * CV;
-      const float t1 = __shfl_sync(0xffffffffu, k, back);
-      const float t2 = __shfl_sync(0xffffffffu, k, back + CV / 4);
-      const float t3 = __shfl_sync(0xffffffffu, k, back + CV / 2);
-      const float t4 = __shfl_sync(0xffffffffu, k, back + CV / 2 + CV / 4);
-      if ((lane / NG) == it) { r1 = t1; r2 = t2; r3 = t3; r4 = t4; }
+      // ---- reduce over the group, hand the four sums back to the lane that decoded the sample (lane it*NG + g')
+      const float4 t = reduce_corners<CV>(d1, d2, d3, d4, cl, (lane & (NG - 1)) * CV);
+      if ((lane / NG) == it) r = t;
     }
     // ---- every lane finishes its own sample; coalesced stores
     if (live) {
-      const float hh = 1.f - lh, hw = 1.f - lw;
-      // an out-of-image corner contributes v = 0 to every gradient (mmcv col2im_bilinear)
-      if (!(meta & 1)) r1 = 0.f;
-      if (!(meta & 2)) r2 = 0.f;
-      if (!(meta & 4)) r3 = 0.f;
-      if (!(meta & 8)) r4 = 0.f;
-      const bool ok = (meta & 15) != 0;
-      const float ga = ok ? (hh * hw) * r1 + (hh * lw) * r2 + (lh * hw) * r3 + (lh * lw) * r4 : 0.f;
-      const float gx = ok ? fW * aw * (hh * (r2 - r1) + lh * (r4 - r3)) : 0.f;
-      const float gy = ok ? fH * aw * (hw * (r3 - r1) + lw * (r4 - r2)) : 0.f;
+      float ga, gx, gy;
+      sample_grads(meta, lh, lw, aw, fW, fH, r, ga, gx, gy);
       if (EPI) {
         // through loc = off / (W,H) + ref and w = softmax(logits): grad_off = grad_loc / (W,H),
         // grad_logit = w * (grad_w - sum_j w_j grad_w_j)   (all 32 lanes take part in the sum)
@@ -517,11 +558,7 @@ msda_forward_small_kernel(const MsdaParams p, float* __restrict__ out) {
     const int Hl = (int)__ldg(p.shapes + 2 * l), Wl = (int)__ldg(p.shapes + 2 * l + 1);
     float lh, lw;
     decode_sample(xy.x, xy.y, Hl, Wl, (int)__ldg(p.lsi + l), base, meta, lh, lw, p.pix_stride);
-    const float hh = 1.f - lh, hw = 1.f - lw;
-    w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
-    w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
-    w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
-    w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+    corner_weights(meta, lh, lw, aw, w1, w2, w3, w4);
   }
   const int rounds = p.ipw / NG;
   for (int r = 0; r < rounds; ++r) {
@@ -540,14 +577,11 @@ msda_forward_small_kernel(const MsdaParams p, float* __restrict__ out) {
       const float a3 = __shfl_sync(0xffffffffu, w3, src);
       const float a4 = __shfl_sync(0xffffffffu, w4, src);
       if (smeta & 15) {
-        const unsigned o1 = (unsigned)sbase;
-        const unsigned o2 = o1 + ((smeta & 16) ? pix : 0u);
-        const unsigned o3 = o1 + (unsigned)(smeta >> 5);
-        const unsigned o4 = o3 + (o2 - o1);
-        const float4 v1 = ldg4(vb + o1);
-        const float4 v2 = ldg4(vb + o2);
-        const float4 v3 = ldg4(vb + o3);
-        const float4 v4 = ldg4(vb + o4);
+        const uint4 o = corner_offsets(sbase, smeta, 1u, pix);
+        const float4 v1 = ldg4(vb + o.x);
+        const float4 v2 = ldg4(vb + o.y);
+        const float4 v3 = ldg4(vb + o.z);
+        const float4 v4 = ldg4(vb + o.w);
         f4_fma(acc, a1, v1);
         f4_fma(acc, a2, v2);
         f4_fma(acc, a3, v3);
@@ -583,11 +617,7 @@ msda_backward_small_kernel(const MsdaParams p, const float* __restrict__ grad_ou
     decode_sample(xy.x, xy.y, Hl, Wl, (int)__ldg(p.lsi + l), base, meta, lh, lw, p.pix_stride);
     fH = (float)Hl;
     fW = (float)Wl;
-    const float hh = 1.f - lh, hw = 1.f - lw;
-    w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
-    w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
-    w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
-    w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+    corner_weights(meta, lh, lw, aw, w1, w2, w3, w4);
   }
   float r1 = 0.f, r2 = 0.f, r3 = 0.f, r4 = 0.f;
   const int rounds = p.ipw / NG;
@@ -611,20 +641,19 @@ msda_backward_small_kernel(const MsdaParams p, const float* __restrict__ grad_ou
       const float a4 = __shfl_sync(0xffffffffu, w4, src);
       float d1 = 0.f, d2 = 0.f, d3 = 0.f, d4 = 0.f;
       if (smeta & 15) {
-        const unsigned o1 = (unsigned)sbase;
-        const unsigned o2 = o1 + ((smeta & 16) ? pix : 0u);
-        const unsigned o3 = o1 + (unsigned)(smeta >> 5);
-        const unsigned o4 = o3 + (o2 - o1);
-        const float4 v1 = ldg4(vs + o1);
-        const float4 v2 = ldg4(vs + o2);
-        const float4 v3 = ldg4(vs + o3);
-        const float4 v4 = ldg4(vs + o4);
-        red_add_v4(gs + o1, f4_scale(a1, go));
-        red_add_v4(gs + o2, f4_scale(a2, go));
-        red_add_v4(gs + o3, f4_scale(a3, go));
-        red_add_v4(gs + o4, f4_scale(a4, go));
+        const uint4 o = corner_offsets(sbase, smeta, 1u, pix);
+        const float4 v1 = ldg4(vs + o.x);
+        const float4 v2 = ldg4(vs + o.y);
+        const float4 v3 = ldg4(vs + o.z);
+        const float4 v4 = ldg4(vs + o.w);
+        red_add_v4(gs + o.x, f4_scale(a1, go));
+        red_add_v4(gs + o.y, f4_scale(a2, go));
+        red_add_v4(gs + o.z, f4_scale(a3, go));
+        red_add_v4(gs + o.w, f4_scale(a4, go));
         d1 = f4_dot(go, v1); d2 = f4_dot(go, v2); d3 = f4_dot(go, v3); d4 = f4_dot(go, v4);
       }
+      // reduce_corners written out: through the helper, nvcc contracts the first product of sample_grads' ga sum
+      // on the other side in this kernel, which changes grad_attn in the last bits
       const bool up1 = (cl & (CV / 2)) != 0;
       const float e0 = __shfl_xor_sync(0xffffffffu, up1 ? d1 : d3, CV / 2);
       const float e1 = __shfl_xor_sync(0xffffffffu, up1 ? d2 : d4, CV / 2);
@@ -645,15 +674,8 @@ msda_backward_small_kernel(const MsdaParams p, const float* __restrict__ grad_ou
     }
   }
   if (mine) {
-    const float hh = 1.f - lh, hw = 1.f - lw;
-    if (!(meta & 1)) r1 = 0.f;
-    if (!(meta & 2)) r2 = 0.f;
-    if (!(meta & 4)) r3 = 0.f;
-    if (!(meta & 8)) r4 = 0.f;
-    const bool ok = (meta & 15) != 0;
-    const float ga = ok ? (hh * hw) * r1 + (hh * lw) * r2 + (lh * hw) * r3 + (lh * lw) * r4 : 0.f;
-    const float gx = ok ? fW * aw * (hh * (r2 - r1) + lh * (r4 - r3)) : 0.f;
-    const float gy = ok ? fH * aw * (hw * (r3 - r1) + lw * (r4 - r2)) : 0.f;
+    float ga, gx, gy;
+    sample_grads(meta, lh, lw, aw, fW, fH, make_float4(r1, r2, r3, r4), ga, gx, gy);
     grad_attn[(size_t)item0 * p.LP + lane] = ga;
     reinterpret_cast<float2*>(grad_loc)[(size_t)item0 * p.LP + lane] = make_float2(gx, gy);
   }
@@ -678,16 +700,6 @@ constexpr int kCells = 256;                                  // 16 x 16 image ce
 constexpr int kOrderChunk = 1024;                            // rows per block of the row-order kernels
 static_assert(kTileRecs == 1 << kRecBits, "record index width");
 
-// Is list entry j of batch element n one of this launch's rows?  (the rows resolve_row<true> accepts)
-__device__ __forceinline__ bool row_live(const MsdaParams& p, int n, int j) {
-  if (p.count && j >= __ldg(p.count + p.cam0 + n % p.ncl)) return false;
-  if (p.S > 1) {
-    const int sl = (j >> 6) % p.S;
-    if (sl < p.s_lo || sl >= p.s_hi) return false;
-  }
-  return true;
-}
-
 // Row order, pass 1: each live row's image cell (-1 = not a row of this launch) and the cell histogram of every
 // chunk of kOrderChunk rows.  The cell is taken from the mean of head 0's sampling locations, or with the fused
 // epilogue (EPI) from the mean of the pillar's reference_points_cam Z-anchors.
@@ -701,11 +713,11 @@ rows_key_kernel(const MsdaParams p, int* __restrict__ key, int* __restrict__ his
   if (j < p.Q) {
     int k = -1;
     if (row_live(p, n, j)) {
+      const int c = p.cam0 + n % p.ncl, b = n / p.ncl;
       float sx = 0.f, sy = 0.f, s;
       if (EPI) {
-        const int c = p.cam0 + n % p.ncl, b = n / p.ncl;
         const size_t q = p.idx ? (size_t)__ldg(p.idx + (size_t)c * p.Qd + j) : (size_t)j;
-        const float2* r = reinterpret_cast<const float2*>(p.ref) + (((size_t)c * p.bs + b) * p.Qd + q) * p.D;
+        const float2* r = reinterpret_cast<const float2*>(p.ref) + anchor_row(p, c, b, q);
         for (int i = 0; i < p.D; ++i) {
           const float2 v = __ldg(r + i);
           sx += v.x;
@@ -834,7 +846,7 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
     }
     if (cl == 0) {
       sm.item[r] = r < nrows ? (int)(EPI ? bq * p.H + h : ((size_t)n * p.Q + j) * p.H + h) : -1;
-      if (EPI) se.refrow[r] = (int)((((size_t)c * p.bs + b) * p.Qd + q) * p.D);
+      if (EPI) se.refrow[r] = (int)anchor_row(p, c, b, q);
     }
     sm.go[r * 8 + cl] = go;
   }
@@ -882,19 +894,14 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
           const float2 st = se.stat[r];
           aw = __fdiv_rn(expf(__ldg(p.attn + si) - st.x), st.y);
           const float2 rf = __ldg(reinterpret_cast<const float2*>(p.ref) + se.refrow[r] + (lane & 7) % p.D);
-          xy.x = __fadd_rn(__fdiv_rn(xy.x, fW), rf.x);
-          xy.y = __fadd_rn(__fdiv_rn(xy.y, fH), rf.y);
+          xy = epi_loc(xy, fW, fH, rf);
         } else {
           aw = __ldg(p.attn + si);
         }
         decode_sample(xy.x, xy.y, Hl, Wl, start, base, meta, lh, lw);   // base, dy in pixels
-        const float hh = 1.f - lh, hw = 1.f - lw;
-        w1 = (meta & 1) ? aw * (hh * hw) : 0.f;
-        w2 = (meta & 2) ? aw * (hh * lw) : 0.f;
-        w3 = (meta & 4) ? aw * (lh * hw) : 0.f;
-        w4 = (meta & 8) ? aw * (lh * lw) : 0.f;
+        corner_weights(meta, lh, lw, aw, w1, w2, w3, w4);
       }
-      float r1 = 0.f, r2 = 0.f, r3 = 0.f, r4 = 0.f;
+      float4 rs = f4_zero();
 #pragma unroll
       for (int it = 0; it < CV; ++it) {
         const int src = it * NG + g;
@@ -903,32 +910,15 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
         const float4 go = sm.go[(warp * RW + ck * 4 + (it >> 1)) * 8 + cl];   // row of sample src
         float d1 = 0.f, d2 = 0.f, d3 = 0.f, d4 = 0.f;
         if (smeta & 15) {
-          const unsigned o1 = (unsigned)sbase * pix;
-          const unsigned o2 = o1 + ((smeta & 16) ? pix : 0u);
-          const unsigned o3 = o1 + (unsigned)(smeta >> 5) * pix;
-          const unsigned o4 = o3 + (o2 - o1);
-          d1 = f4_dot(go, ldg4(vs + o1));
-          d2 = f4_dot(go, ldg4(vs + o2));
-          d3 = f4_dot(go, ldg4(vs + o3));
-          d4 = f4_dot(go, ldg4(vs + o4));
+          const uint4 o = corner_offsets(sbase, smeta, pix, pix);
+          d1 = f4_dot(go, ldg4(vs + o.x));
+          d2 = f4_dot(go, ldg4(vs + o.y));
+          d3 = f4_dot(go, ldg4(vs + o.z));
+          d4 = f4_dot(go, ldg4(vs + o.w));
         }
-        // transposed reduction and hand-back, as in msda_backward_kernel
-        const bool up1 = (cl & (CV / 2)) != 0;
-        const float e0 = __shfl_xor_sync(0xffffffffu, up1 ? d1 : d3, CV / 2);
-        const float e1 = __shfl_xor_sync(0xffffffffu, up1 ? d2 : d4, CV / 2);
-        const float k0 = (up1 ? d3 : d1) + e0;
-        const float k1 = (up1 ? d4 : d2) + e1;
-        const bool up2 = (cl & (CV / 4)) != 0;
-        const float eb = __shfl_xor_sync(0xffffffffu, up2 ? k0 : k1, CV / 4);
-        float k = (up2 ? k1 : k0) + eb;
-#pragma unroll
-        for (int off = CV / 8; off >= 1; off >>= 1) k += __shfl_xor_sync(0xffffffffu, k, off);
-        const int back = (lane & (NG - 1)) * CV;
-        const float t1 = __shfl_sync(0xffffffffu, k, back);
-        const float t2 = __shfl_sync(0xffffffffu, k, back + CV / 4);
-        const float t3 = __shfl_sync(0xffffffffu, k, back + CV / 2);
-        const float t4 = __shfl_sync(0xffffffffu, k, back + CV / 2 + CV / 4);
-        if ((lane / NG) == it) { r1 = t1; r2 = t2; r3 = t3; r4 = t4; }
+        // reduction and hand-back, as in msda_backward_kernel
+        const float4 t = reduce_corners<CV>(d1, d2, d3, d4, cl, (lane & (NG - 1)) * CV);
+        if ((lane / NG) == it) rs = t;
       }
       // this sample's 4 corner records: record = (row in tile, point, corner), key = level pixel << kRecBits | record
       const unsigned rec = ((unsigned)(warp * RW + ck * 4) << 5) + lane * 4;
@@ -941,15 +931,8 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
       *reinterpret_cast<uint4*>(&tk.key[rec]) = kk;
       *reinterpret_cast<float4*>(&sm.w[rec]) = make_float4(w1, w2, w3, w4);
       if (live) {
-        const float hh = 1.f - lh, hw = 1.f - lw;
-        if (!(meta & 1)) r1 = 0.f;
-        if (!(meta & 2)) r2 = 0.f;
-        if (!(meta & 4)) r3 = 0.f;
-        if (!(meta & 8)) r4 = 0.f;
-        const bool ok = (meta & 15) != 0;
-        const float ga = ok ? (hh * hw) * r1 + (hh * lw) * r2 + (lh * hw) * r3 + (lh * lw) * r4 : 0.f;
-        const float gx = ok ? fW * aw * (hh * (r2 - r1) + lh * (r4 - r3)) : 0.f;
-        const float gy = ok ? fH * aw * (hw * (r3 - r1) + lw * (r4 - r2)) : 0.f;
+        float ga, gx, gy;
+        sample_grads(meta, lh, lw, aw, fW, fH, rs, ga, gx, gy);
         if (EPI) {
           // offsets are shared by every camera that sees the pillar: accumulate (caller zeroes); the logit
           // gradient waits for the row's other levels
@@ -1102,12 +1085,6 @@ __global__ void msda_backward_generic_kernel(const MsdaParams p, const float* __
   }
 }
 
-// FORWARD only: per-head level slabs larger than this are read with L1::no_allocate (see ldg4_na), so at
-// the SpatialCrossAttention shape everything but the 48 KB 15x25 level streams (a sweep of the threshold at that
-// shape chose it).  The backward keeps plain loads (na_bytes = 0xffffffff): they share the LSU -> XBAR request
-// path with the reductions, and a no-allocate miss cannot merge with a neighbouring warp's pending miss.
-constexpr unsigned kStreamBytes = 100000u;
-
 int fill_params(MsdaParams& p, const float* value, const int64_t* shapes, const int64_t* lsi,
                 const float* loc, const float* attn, int B, int K, int H, int C, int L, int Q,
                 int P, int im2col_step, const char* who) {
@@ -1135,28 +1112,22 @@ int fill_params(MsdaParams& p, const float* value, const int64_t* shapes, const 
   p.idx = nullptr; p.count = nullptr; p.inv = nullptr;
   p.ncl = B; p.cam0 = 0; p.bs = 1; p.Qd = Q;
   p.S = 1; p.s_lo = 0; p.s_hi = 1;
-  p.na_bytes = kStreamBytes;
   return VIDAR_OK;
 }
 
-inline int pick_ipw(int LP, int CV);
 // vector kernels: C in {16,32,64}, 32-bit intra-batch offsets and item counts
 inline bool vec_ok(const MsdaParams& p) {
   return (p.C == 16 || p.C == 32 || p.C == 64) && (long long)p.K * p.H * p.C < (1LL << 25) &&   /* offsets ride in meta bits 5..29 */
          p.items < (1LL << 31) && (long long)p.Q * p.H < (1LL << 31);
 }
-inline void set_ipw(MsdaParams& p, int CV) {
-  p.ipw = pick_ipw(p.LP, CV);
-  p.lp_shift = 0;
-  while ((1 << p.lp_shift) < p.LP) ++p.lp_shift;
-}
 
 // items per warp for the vector kernels: pack several (b,q,h) into one 32-sample chunk
 // when L*P is small (temporal self-attention: L*P = 4).
-inline int pick_ipw(int LP, int CV) {
+inline void set_ipw(MsdaParams& p, int CV) {
   const int NG = 32 / CV;
-  if (LP >= 2 && LP < 32 && 32 % LP == 0 && LP % NG == 0) return 32 / LP;
-  return 1;
+  p.ipw = (p.LP >= 2 && p.LP < 32 && 32 % p.LP == 0 && p.LP % NG == 0) ? 32 / p.LP : 1;
+  p.lp_shift = 0;
+  while ((1 << p.lp_shift) < p.LP) ++p.lp_shift;
 }
 
 inline long long num_blocks(const MsdaParams& p) {
@@ -1166,57 +1137,6 @@ inline long long num_blocks(const MsdaParams& p) {
   }
   const long long warps = (p.items + p.ipw - 1) / p.ipw;
   return (warps + kWarpsPerBlock - 1) / kWarpsPerBlock;
-}
-
-// The vector kernels at head width p.C (CV = C / 4 lanes per head vector).  The plain op (!EPI && !IDX) packs
-// several items into a warp when L*P is small (set_ipw): the small kernel once every lane group gets an item of
-// its own, MULTI below that.  The row map (IDX) keeps fill_rows' one item per warp.
-template <bool EPI, bool IDX>
-int launch_vec_forward(MsdaParams& p, float* out, cudaStream_t st, const char* who) {
-  if (!IDX) set_ipw(p, p.C / 4);
-  const long long nb = num_blocks(p);
-  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
-  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
-  const auto launch = [&](auto cv) {
-    constexpr int CV = decltype(cv)::value;
-    if constexpr (!EPI && !IDX) {
-      if (p.ipw >= 32 / CV) msda_forward_small_kernel<CV><<<grid, block, 0, st>>>(p, out);
-      else if (p.ipw > 1) msda_forward_kernel<CV, true><<<grid, block, 0, st>>>(p, out);
-      else msda_forward_kernel<CV, false><<<grid, block, 0, st>>>(p, out);
-    } else {
-      msda_forward_kernel<CV, false, EPI, IDX><<<grid, block, 0, st>>>(p, out);
-    }
-  };
-  if (p.C == 32) launch(std::integral_constant<int, 8>{});
-  else if (p.C == 16) launch(std::integral_constant<int, 4>{});
-  else launch(std::integral_constant<int, 16>{});
-  return check_launch(who);
-}
-
-template <bool EPI, bool IDX>
-int launch_vec_backward(MsdaParams& p, const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
-                        cudaStream_t st, const char* who) {
-  if (!IDX) set_ipw(p, p.C / 4);
-  const long long nb = num_blocks(p);
-  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
-  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
-  const auto launch = [&](auto cv) {
-    constexpr int CV = decltype(cv)::value;
-    if constexpr (!EPI && !IDX) {
-      if (p.ipw >= 32 / CV)
-        msda_backward_small_kernel<CV><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
-      else if (p.ipw > 1)
-        msda_backward_kernel<CV, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
-      else
-        msda_backward_kernel<CV, false><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
-    } else {
-      msda_backward_kernel<CV, false, EPI, IDX><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
-    }
-  };
-  if (p.C == 32) launch(std::integral_constant<int, 8>{});
-  else if (p.C == 16) launch(std::integral_constant<int, 4>{});
-  else launch(std::integral_constant<int, 16>{});
-  return check_launch(who);
 }
 
 // The tile-aggregating rows backward: C = 32, 8 points on each of 4 levels (SpatialCrossAttention).
@@ -1266,6 +1186,81 @@ int launch_rows_backward_tiled(const MsdaParams& p, const float* grad_out, float
   return check_launch(who);
 }
 
+// Calls f(std::integral_constant<int, CV>{}) for head width C in {16, 32, 64}: CV = C / 4 lanes per head vector.
+template <class F>
+void with_cv(int C, const F& f) {
+  if (C == 32) f(std::integral_constant<int, 8>{});
+  else if (C == 16) f(std::integral_constant<int, 4>{});
+  else f(std::integral_constant<int, 16>{});
+}
+
+// The forward of every entry point, once its arguments are checked.  The plain op (!EPI && !IDX) takes the generic
+// kernel at head widths the vector kernels do not support (the fused epilogue and the row map require them), and
+// packs several items into a warp when L*P is small (set_ipw): the small kernel once every lane group gets an item
+// of its own, MULTI below that.  The row map (IDX) keeps fill_rows' one item per warp.
+template <bool EPI, bool IDX>
+int msda_forward(MsdaParams& p, float* out, cudaStream_t st, const char* who) {
+  VIDAR_REQUIRE(out, "%s: null output", who);
+  if (!EPI && !IDX && !vec_ok(p)) {
+    const long long nb = (p.items * p.C + 255) / 256;
+    VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
+    msda_forward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, out);
+    return check_launch(who);
+  }
+  if (!IDX) set_ipw(p, p.C / 4);
+  const long long nb = num_blocks(p);
+  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
+  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
+  with_cv(p.C, [&](auto cv) {
+    constexpr int CV = decltype(cv)::value;
+    if constexpr (!EPI && !IDX) {
+      if (p.ipw >= 32 / CV) msda_forward_small_kernel<CV><<<grid, block, 0, st>>>(p, out);
+      else if (p.ipw > 1) msda_forward_kernel<CV, true><<<grid, block, 0, st>>>(p, out);
+      else msda_forward_kernel<CV, false><<<grid, block, 0, st>>>(p, out);
+    } else {
+      msda_forward_kernel<CV, false, EPI, IDX><<<grid, block, 0, st>>>(p, out);
+    }
+  });
+  return check_launch(who);
+}
+
+// The backward of every entry point, once its arguments are checked: the kernels the forward picks, or the tile
+// kernel for the row map where tile_backward_ok.
+template <bool EPI, bool IDX>
+int msda_backward(MsdaParams& p, const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
+                  cudaStream_t st, const char* who) {
+  VIDAR_REQUIRE(grad_out && grad_value && grad_loc && grad_attn, "%s: null gradient pointer", who);
+  if (IDX && tile_backward_ok(p))
+    return launch_rows_backward_tiled<EPI>(p, grad_out, grad_value, grad_loc, grad_attn, st, who);
+  if (!EPI && !IDX && !vec_ok(p)) {
+    cudaError_t e = cudaMemsetAsync(grad_loc, 0, sizeof(float) * 2 * (size_t)p.items * p.LP, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(grad_attn, 0, sizeof(float) * (size_t)p.items * p.LP, st);
+    if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: memset: %s", who, cudaGetErrorString(e));
+    const long long nb = (p.items * p.C + 255) / 256;
+    VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
+    msda_backward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+    return check_launch(who);
+  }
+  if (!IDX) set_ipw(p, p.C / 4);
+  const long long nb = num_blocks(p);
+  VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
+  const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
+  with_cv(p.C, [&](auto cv) {
+    constexpr int CV = decltype(cv)::value;
+    if constexpr (!EPI && !IDX) {
+      if (p.ipw >= 32 / CV)
+        msda_backward_small_kernel<CV><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+      else if (p.ipw > 1)
+        msda_backward_kernel<CV, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+      else
+        msda_backward_kernel<CV, false><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+    } else {
+      msda_backward_kernel<CV, false, EPI, IDX><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
+    }
+  });
+  return check_launch(who);
+}
+
 }  // namespace
 }  // namespace vidar
 
@@ -1275,18 +1270,12 @@ extern "C" int vidar_msda_forward(const float* value, const int64_t* spatial_sha
                                   const int64_t* level_start, const float* sampling_loc,
                                   const float* attn_weight, float* out, int B, int K, int H, int C,
                                   int L, int Q, int P, int im2col_step, void* stream) {
+  const char* who = "ms_deform_attn_forward";
   MsdaParams p;
   int rc = fill_params(p, value, spatial_shapes, level_start, sampling_loc, attn_weight, B, K, H,
-                       C, L, Q, P, im2col_step, "ms_deform_attn_forward");
+                       C, L, Q, P, im2col_step, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(out, "ms_deform_attn_forward: null output");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (vec_ok(p)) return launch_vec_forward<false, false>(p, out, st, "ms_deform_attn_forward");
-  const long long n = p.items * C;
-  const long long nb = (n + 255) / 256;
-  VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_forward: problem too large");
-  msda_forward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, out);
-  return check_launch("ms_deform_attn_forward");
+  return msda_forward<false, false>(p, out, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_backward(const float* value, const int64_t* spatial_shapes,
@@ -1295,25 +1284,13 @@ extern "C" int vidar_msda_backward(const float* value, const int64_t* spatial_sh
                                    float* grad_value, float* grad_sampling_loc,
                                    float* grad_attn_weight, int B, int K, int H, int C, int L,
                                    int Q, int P, int im2col_step, void* stream) {
+  const char* who = "ms_deform_attn_backward";
   MsdaParams p;
   int rc = fill_params(p, value, spatial_shapes, level_start, sampling_loc, attn_weight, B, K, H,
-                       C, L, Q, P, im2col_step, "ms_deform_attn_backward");
+                       C, L, Q, P, im2col_step, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(grad_out && grad_value && grad_sampling_loc && grad_attn_weight,
-                "ms_deform_attn_backward: null gradient pointer");
-  p.na_bytes = 0xffffffffu;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (vec_ok(p))
-    return launch_vec_backward<false, false>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight, st,
-                                             "ms_deform_attn_backward");
-  cudaError_t e = cudaMemsetAsync(grad_sampling_loc, 0, sizeof(float) * 2 * (size_t)p.items * p.LP, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(grad_attn_weight, 0, sizeof(float) * (size_t)p.items * p.LP, st);
-  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "ms_deform_attn_backward: memset: %s", cudaGetErrorString(e));
-  const long long n = p.items * C;
-  const long long nb = (n + 255) / 256;
-  VIDAR_REQUIRE(nb < 2147483647LL, "ms_deform_attn_backward: problem too large");
-  msda_backward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight);
-  return check_launch("ms_deform_attn_backward");
+  return msda_backward<false, false>(p, grad_out, grad_value, grad_sampling_loc, grad_attn_weight,
+                                     (cudaStream_t)stream, who);
 }
 
 // ---- MSDeformableAttention3D with the softmax and the sampling-location arithmetic folded in
@@ -1337,8 +1314,7 @@ extern "C" int vidar_msda_sca_forward(const float* value, const int64_t* spatial
   if (rc) return rc;
   rc = check_sca(p, ref_points, D, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(out, "%s: null output", who);
-  return launch_vec_forward<true, false>(p, out, (cudaStream_t)stream, who);
+  return msda_forward<true, false>(p, out, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_sca_backward(const float* value, const int64_t* spatial_shapes,
@@ -1352,9 +1328,7 @@ extern "C" int vidar_msda_sca_backward(const float* value, const int64_t* spatia
   if (rc) return rc;
   rc = check_sca(p, ref_points, D, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(grad_out && grad_value && grad_offsets && grad_logits, "%s: null gradient pointer", who);
-  p.na_bytes = 0xffffffffu;
-  return launch_vec_backward<true, false>(p, grad_out, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
+  return msda_backward<true, false>(p, grad_out, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
 }
 
 // ---- row-indirect entry points: SpatialCrossAttention's rebatch / scatter-add fused into the op ------
@@ -1390,11 +1364,7 @@ extern "C" int vidar_msda_rows_forward(const float* value, const int64_t* spatia
   if (rc) return rc;
   rc = fill_rows(p, idx, count, inv_count, bs, ncl, cam0, Qd, S, s_lo, s_hi, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(slots, "%s: null output", who);
-  // the streaming hint helps the plain forward but not this one, whose epilogue also sends 245 MB
-  // of slot reductions through L2: plain loads here
-  p.na_bytes = 0xffffffffu;
-  return launch_vec_forward<false, true>(p, slots, (cudaStream_t)stream, who);
+  return msda_forward<false, true>(p, slots, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_rows_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -1410,12 +1380,8 @@ extern "C" int vidar_msda_rows_backward(const float* value, const int64_t* spati
   if (rc) return rc;
   rc = fill_rows(p, idx, count, inv_count, bs, ncl, cam0, Qd, S, s_lo, s_hi, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(grad_slots && grad_value && grad_sampling_loc && grad_attn_weight, "%s: null gradient pointer", who);
-  p.na_bytes = 0xffffffffu;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (tile_backward_ok(p))
-    return launch_rows_backward_tiled<false>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, st, who);
-  return launch_vec_backward<false, true>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight, st, who);
+  return msda_backward<false, true>(p, grad_slots, grad_value, grad_sampling_loc, grad_attn_weight,
+                                    (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_sca_rows_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -1431,9 +1397,7 @@ extern "C" int vidar_msda_sca_rows_forward(const float* value, const int64_t* sp
   if (rc) return rc;
   rc = fill_rows(p, idx, count, inv_count, bs, ncl, cam0, Qd, S, s_lo, s_hi, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(slots, "%s: null output", who);
-  p.na_bytes = 0xffffffffu;
-  return launch_vec_forward<true, true>(p, slots, (cudaStream_t)stream, who);
+  return msda_forward<true, true>(p, slots, (cudaStream_t)stream, who);
 }
 
 extern "C" int vidar_msda_sca_rows_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -1450,10 +1414,5 @@ extern "C" int vidar_msda_sca_rows_backward(const float* value, const int64_t* s
   if (rc) return rc;
   rc = fill_rows(p, idx, count, inv_count, bs, ncl, cam0, Qd, S, s_lo, s_hi, who);
   if (rc) return rc;
-  VIDAR_REQUIRE(grad_slots && grad_value && grad_offsets && grad_logits, "%s: null gradient pointer", who);
-  p.na_bytes = 0xffffffffu;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (tile_backward_ok(p))
-    return launch_rows_backward_tiled<true>(p, grad_slots, grad_value, grad_offsets, grad_logits, st, who);
-  return launch_vec_backward<true, true>(p, grad_slots, grad_value, grad_offsets, grad_logits, st, who);
+  return msda_backward<true, true>(p, grad_slots, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
 }
