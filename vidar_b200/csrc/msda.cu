@@ -687,18 +687,25 @@ msda_backward_small_kernel(const MsdaParams p, const float* __restrict__ grad_ou
 // are first put in image order (a stable counting sort by a 16 x 16 cell of the row's mean sampling location), and
 // one CTA then owns a tile of kTileRows ordered rows of one head.  Per pyramid level it gathers and computes the
 // sampling-location / attention gradients as msda_backward_kernel does (same arithmetic), writes one record per
-// corner (level pixel, weight, row) to shared memory, sorts the records by pixel and sums each pixel's run with
-// lane = channel, so a (pixel, head) line is reduced once per tile instead of once per corner.
+// pair of horizontally adjacent corners (left pixel, two weights, row) to shared memory, sorts the records by pixel
+// and sums the runs with lane = channel, so a (pixel, head) line is reduced about once per tile instead of once per
+// corner.
 constexpr int kTileRows = 256;                               // rows per tile
 constexpr int kTilePoints = 8;                               // points per level (P)
-constexpr int kTileRecs = kTileRows * kTilePoints * 4;       // corner records per level
-constexpr int kRecBits = 13;                                 // record index bits: log2(kTileRecs)
+constexpr int kTileRecs = kTileRows * kTilePoints * 2;       // corner-pair records per level (top, bottom)
+constexpr int kRecBits = 12;                                 // record index bits: log2(kTileRecs)
 constexpr int kTileThreads = 512;                            // 16 warps, 16 rows each
 constexpr int kTileItems = kTileRecs / kTileThreads;         // records per thread in the sort
 constexpr int kTileSeg = kTileRecs / (kTileThreads / 8);     // sorted records summed by one 8-lane group
 constexpr int kCells = 256;                                  // 16 x 16 image cells of the row order
 constexpr int kOrderChunk = 1024;                            // rows per block of the row-order kernels
 static_assert(kTileRecs == 1 << kRecBits, "record index width");
+
+// floor(n / d) for n < 2^22 from rd = 1 / d rounded to fp32: n + 0.5 is exact, its quotient lies at least 0.5 / d from
+// an integer, and the two fp32 roundings move it by less than (n + 0.5) / d * 2^-23 < 0.5 / d.
+__device__ __forceinline__ unsigned div_small(unsigned n, float rd) {
+  return (unsigned)__fmul_rn(__fadd_rn(__uint2float_rn(n), 0.5f), rd);
+}
 
 // Row order, pass 1: each live row's image cell (-1 = not a row of this launch) and the cell histogram of every
 // chunk of kOrderChunk rows.  The cell is taken from the mean of head 0's sampling locations, or with the fused
@@ -794,7 +801,7 @@ union __align__(16) TileKeys {
   typename TileSort::TempStorage sort;
 };
 struct TileSmem {                        // dynamic shared memory
-  float w[kTileRecs];                    // record weight attn * bilinear corner weight
+  float w[2 * kTileRecs];                // attn * bilinear weight of record r's left (w[2r]) and right (w[2r+1]) corner
   float4 go[kTileRows * 8];              // row's grad_out head vector, scaled by 1 / #cameras
   int item[kTileRows];                   // row's item index (EPI: its pillar's (b, q, h) index), -1 past the last row
   size_t slab;                           // float offset of the (n, h) slab in value / grad_value
@@ -874,7 +881,9 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
     const int Hl = (int)__ldg(p.shapes + 2 * l), Wl = (int)__ldg(p.shapes + 2 * l + 1);
     const int start = (int)__ldg(p.lsi + l);
     const float fH = (float)Hl, fW = (float)Wl;
-    const int pb = 32 - __clz(Hl * Wl);             // pixel bits of the level's sort key
+    // A record's pixel is a slot h * (Wl + 1) + x' of the level's rows padded by one column in front: x' = w + 1, and
+    // x' = 0 holds only invalid corners.  Slots are below Hl * (Wl + 1) < 2 * K < 2^20, so the key fits 32 bits.
+    const int pb = 32 - __clz(Hl * (Wl + 1));       // pixel bits of the level's sort key
     const unsigned none = (1u << pb) - 1;           // pixel field of an unused record: sorts last
     // ---- row phase: a chunk is 4 rows x this level's 8 points, lane j decodes point j % 8 of row j / 8
 #pragma unroll 1
@@ -920,16 +929,18 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
         const float4 t = reduce_corners<CV>(d1, d2, d3, d4, cl, (lane & (NG - 1)) * CV);
         if ((lane / NG) == it) rs = t;
       }
-      // this sample's 4 corner records: record = (row in tile, point, corner), key = level pixel << kRecBits | record
-      const unsigned rec = ((unsigned)(warp * RW + ck * 4) << 5) + lane * 4;
-      const unsigned px = (unsigned)(base - start), dx = (meta >> 4) & 1, dy = (unsigned)meta >> 5;
-      uint4 kk;
-      kk.x = (((meta & 1) ? px : none) << kRecBits) | rec;
-      kk.y = (((meta & 2) ? px + dx : none) << kRecBits) | (rec + 1);
-      kk.z = (((meta & 4) ? px + dy : none) << kRecBits) | (rec + 2);
-      kk.w = (((meta & 8) ? px + dy + dx : none) << kRecBits) | (rec + 3);
-      *reinterpret_cast<uint4*>(&tk.key[rec]) = kk;
-      *reinterpret_cast<float4*>(&sm.w[rec]) = make_float4(w1, w2, w3, w4);
+      // this sample's 2 corner-pair records: record = (row in tile, point, half), half 0 = corners (1, 2) in row
+      // h_low, 1 = corners (3, 4) in row h_low + 1; key = slot of the pair's left pixel (w_low) << kRecBits | record,
+      // or `none` if neither corner is valid.  The clamped base is (max(h_low, 0), max(w_low, 0)); the mask tells
+      // h_low = -1 (no corner in the top row) and w_low = -1 (no left corner, slot x' = 0).
+      const unsigned rec = ((unsigned)(warp * RW + ck * 4) << 4) + lane * 2;
+      const unsigned px = (unsigned)(base - start), hl = div_small(px, __frcp_rn(fW));
+      const unsigned left = px + hl + ((meta & 5) ? 1u : 0u);
+      uint2 kk;
+      kk.x = (((meta & 3) ? left : none) << kRecBits) | rec;
+      kk.y = (((meta & 12) ? left + ((meta & 3) ? (unsigned)Wl + 1u : 0u) : none) << kRecBits) | (rec + 1);
+      *reinterpret_cast<uint2*>(&tk.key[rec]) = kk;
+      *reinterpret_cast<float4*>(&sm.w[2 * rec]) = make_float4(w1, w2, w3, w4);
       if (live) {
         float ga, gx, gy;
         sample_grads(meta, lh, lw, aw, fW, fH, rs, ga, gx, gy);
@@ -962,40 +973,60 @@ msda_backward_tile_kernel(const MsdaParams p, const int* __restrict__ perm, cons
     }
     __syncthreads();
 
-    // group G (8 lanes x float4 = one head vector) sums the runs of sorted positions [G*kTileSeg, (G+1)*kTileSeg):
-    // one 128-byte reduction per pixel run (a run split between two groups is reduced twice)
+    // group G (8 lanes x float4 = one head vector) sums the records at sorted positions [G*kTileSeg, (G+1)*kTileSeg).
+    // Slot s receives the left corners of pairs keyed s and the right corners of pairs keyed s - 1, which sort next
+    // to each other: the group keeps accumulators for slots cur and cur + 1 and sends one 128-byte reduction per
+    // touched pixel (a pixel whose records straddle two groups is reduced twice)
     float* gl = grad_value + slab + (size_t)start * pix;
     asm volatile("" : "+l"(gl));   // computed here, not kept live through the sort (64-register budget)
     const unsigned* ks = tk.key + (warp * NG + g) * (kTileSeg + 1);
+    const unsigned W1 = (unsigned)Wl + 1u;
+    const float rW1 = __frcp_rn(fW + 1.f);
+    // slot s = h * W1 + x' is pixel h * Wl + x' - 1; slot x' = 0 only ever holds invalid corners (weight 0, and
+    // perhaps an address outside the level) and is never reduced
+    const auto flush = [&](unsigned s, const float4& a) {
+      const unsigned hs = div_small(s, rW1);
+      if (s != hs * W1) red_add_v4(gl + (s - hs - 1u) * pix, a);
+    };
     // records are read 4 at a time so that their shared-memory loads overlap; unused records (pixel `none`, weight 0)
-    // sort last and accumulate into a run that is never reduced
+    // sort last and accumulate into slots that are never reduced
     unsigned cur = none;
-    float4 acc = f4_zero();
+    float4 a0 = f4_zero(), a1 = f4_zero();   // slots cur, cur + 1
     for (int i0 = 0; i0 < kTileSeg; i0 += 4) {
       unsigned kq[4];
-      float wq[4];
+      float2 wq[4];
       float4 gq[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) kq[u] = ks[i0 + u];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const unsigned rec = kq[u] & (kTileRecs - 1);
-        wq[u] = sm.w[rec];
-        gq[u] = sm.go[(rec >> 5) * 8 + cl];
+        wq[u] = reinterpret_cast<const float2*>(sm.w)[rec];
+        gq[u] = sm.go[(rec >> 4) * 8 + cl];
       }
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const unsigned kp = kq[u] >> kRecBits;
         if (kp != cur) {
-          if (cur != none) red_add_v4(gl + cur * pix, acc);
+          // next slot: cur + 1 carries on; any other key ends both
+          const bool next = kp == cur + 1u;
+          if (cur != none) {
+            flush(cur, a0);
+            if (!next) flush(cur + 1u, a1);
+          }
+          a0 = next ? a1 : f4_zero();
+          a1 = f4_zero();
           cur = kp;
-          acc = f4_zero();
         }
-        f4_fma(acc, wq[u], gq[u]);
+        f4_fma(a0, wq[u].x, gq[u]);
+        f4_fma(a1, wq[u].y, gq[u]);
       }
       if (cur == none) break;
     }
-    if (cur != none) red_add_v4(gl + cur * pix, acc);
+    if (cur != none) {
+      flush(cur, a0);
+      flush(cur + 1u, a1);
+    }
     __syncthreads();   // key[] / w[] are rewritten by the next level
   }
   if (EPI) {
@@ -1140,10 +1171,11 @@ inline long long num_blocks(const MsdaParams& p) {
 }
 
 // The tile-aggregating rows backward: C = 32, 8 points on each of 4 levels (SpatialCrossAttention).
-// A level's pixel index and the record index share a 32-bit sort key.
+// A level's padded pixel slot (< 2K) and the record index share a 32-bit sort key.
 inline bool tile_backward_ok(const MsdaParams& p) {
-  return p.C == 32 && p.P == kTilePoints && p.LP == 32 && p.K < (1 << (32 - kRecBits));
+  return p.C == 32 && p.P == kTilePoints && p.LP == 32 && p.K < (1 << 19);
 }
+static_assert(20 + kRecBits <= 32, "sort key width at K < 2^19");
 
 // Row order + tile kernel.  The order's scratch (two ints per row and a cell histogram per 1024 rows) is
 // stream-ordered (cudaMallocFromPoolAsync / cudaFreeAsync): no host sync, and a CUDA graph captures it as
