@@ -487,6 +487,41 @@ int vidar_dense_chamfer_backward(const float* points, const float* origin, const
                                  float weight_sum, const float* grad_loss, float* grad_dist, int bs, int F, int R0,
                                  int To, int M, void* stream);
 
+/* The same Chamfer term over a pair table, one loss per group (ViDARHeadV1: a group per head frame):
+ *   dist [P*R0], points [P*R0, 3]  rays of pair n at n*R0 .. (n+1)*R0-1;  origin [No, 3]
+ *   gt [Sg, M, 3], gt_tindex [Sg, M]  Sg gt samples, frames 0..Fg-1 (float, -1 = padding, any order)
+ *   slot_pair [Sg*Fg] int32 (device): the pair of each (gt sample, frame) slot, -1 = none
+ *   pair_table [P, 3] int32 (device): slot, origin row, group; pairs in increasing slot order
+ *   pair_weight [P], group_norm [groups] (device): loss[g] = sum_{n in g} w_n * (...) / group_norm[g]
+ *   q_off, c_off [2P+1]; pairs [P, 4]; loss [groups]; grad_loss [groups] (device).
+ * vidar_dense_chamfer_forward / _backward are the case P = bs*F, Sg = bs, Fg = F, one group. */
+int vidar_dense_chamfer_groups_forward(const float* dist, const float* points, const float* origin, const float* gt,
+                                       const float* gt_tindex, const int32_t* slot_pair, const int32_t* pair_table,
+                                       const float* pair_weight, const float* group_norm, const float* pc_range_host,
+                                       float* qbuf, float* cbuf, unsigned char* q_mask, unsigned char* c_mask,
+                                       int64_t* q_off, int64_t* c_off, int64_t* idx, double* pairs, float* loss,
+                                       int P, int groups, int R0, int Sg, int Fg, int M, int W, int H, int Z,
+                                       int within_grid, void* stream);
+int vidar_dense_chamfer_groups_backward(const float* points, const float* origin, const float* qbuf,
+                                        const float* cbuf, const unsigned char* q_mask, const int64_t* q_off,
+                                        const int64_t* c_off, const int64_t* idx, const double* pairs,
+                                        const int32_t* pair_table, const float* pair_weight,
+                                        const float* group_norm, const float* grad_loss, float* grad_dist, int P,
+                                        int groups, int R0, int Sg, int Fg, int M, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * (vi) ViDARHeadV1._get_reference_gt_points (dense_heads/vidar_head_v1.py:94-148) for every head frame at once:
+ *   gt [bs, M, Cg]       GT rows (metres), NaN-padded, the frame in the last column
+ *   mats [H*V, bs, 4, 4] src -> tgt transform of each (head frame i, slot v) job and sample; x' = [x y z 1] @ T
+ *   jobs_host [H*V] int32 (HOST): source frame of job (i, v), -1 = none
+ *   voxel_host [9] (HOST): off[3], scale[3], cells[3]; ray = ((x' - off) * scale) * cells
+ * Outputs, segment s = i * bs + b:  rays [H*bs, M, 3] voxel units, tindex [H*bs, M] (v, -1 = padding),
+ * points [H*bs, M, 3] metres (NULL = skip).  Rows of a segment are slot-major, the source rows of a slot in their
+ * order, then padding (NaN).  3 launches, no host sync. */
+int vidar_head_align_gt(const float* gt, const float* mats, const int32_t* jobs_host, const float* voxel_host,
+                        float* rays, float* tindex, float* points, int bs, int M, int Cg, int H, int V,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

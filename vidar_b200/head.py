@@ -18,8 +18,9 @@ is fused with the sampler as well (`ray_head.gumbel_distance`), and its Chamfer 
 (sample, frame) pair is one batched op (`ray_head.dense_chamfer_loss`: segmented nearest-neighbour search in
 place of mmdet3d's O(N*M) distance matrix, `chamfer_distance` with criterion 'l2', reduction 'mean': the mean
 squared NN distance each way).  With CE + dense (use_dist_loss=False) `loss` runs forward and backward without
-a host sync.  The distance term samples through `ray_head.get_grid_features` (CUDA sampler) and then follows
-the reference's torch statements; decoding is `ray_head.decode_ray_depth`.
+a host sync.  `ViDARRayHeadV1` is the same for ViDARHeadV1 (vidar_head_v1.py): every head frame's GT
+alignment and loss in one batched pass.  The distance term samples through `ray_head.get_grid_features` (CUDA
+sampler) and then follows the reference's torch statements; decoding is `ray_head.decode_ray_depth`.
 CUDA only, like everything else in this package.
 """
 import numpy as np
@@ -241,3 +242,260 @@ class ViDARRayHead:
         pred_pcds = self.get_rendered_pcds(batched_origin_points, batched_gt_points, gt_tindex, gt_dist, pred_dist, tgt_pc_range)
         gt_pcds = self.get_rendered_pcds(batched_origin_points, batched_gt_points, gt_tindex, gt_dist, gt_dist, tgt_pc_range)
         return dict(pred_pcds=pred_pcds, gt_pcds=gt_pcds, origin=batched_origin_points)
+
+
+class ViDARRayHeadV1(ViDARRayHead):
+    """The loss / decode half of ViDARHeadV1 (dense_heads/vidar_head_v1.py): the head predicts
+    `1 + pred_history_frame_num + pred_future_frame_num` head frames, each supervised by the GT of its own source
+    frames moved into the target frames' coordinates.
+
+    `loss` with CE + dense (use_dist_loss=False) runs every head frame in one batched pass, in a fixed number of
+    library launches and without a host sync: the GT alignment of every (head frame, slot) job is one op
+    (`ray_head.align_gt`), the CE term one `ray_ce` over [head frames * bs * frames] volumes, the dense term one
+    gumbel decode and one grouped Chamfer op (`ray_head.dense_chamfer_group_loss`, a group per head frame) over the
+    (head frame, sample, frame) pairs of non-zero weight only.  The reference computes the auxiliary head frames'
+    zero-weight frames and multiplies them by zero; those pairs never reach the sampler or the nearest-neighbour
+    search here.  Default Gumbel noise is drawn for the weighted pairs only, so the generator is consumed
+    differently from the reference (pass `gumbels` to pin the noise).
+
+    fuse_head_frames = False (or use_dist_loss) selects the reference's per-head-frame loop over
+    `ViDARRayHead.loss` with a torch restatement of the alignment (boolean masks, host syncs); tests compare the
+    two."""
+
+    def __init__(self, history_queue_length, pred_history_frame_num=0, pred_future_frame_num=0,
+                 per_frame_loss_weight=(1.0,), **kwargs):
+        super().__init__(**kwargs)
+        self.history_queue_length = history_queue_length
+        self.pred_history_frame_num = pred_history_frame_num
+        self.pred_future_frame_num = pred_future_frame_num
+        self.pred_frame_num = 1 + pred_history_frame_num + pred_future_frame_num
+        self.per_frame_loss_weight = per_frame_loss_weight
+        if len(per_frame_loss_weight) != self.pred_frame_num:
+            raise ValueError(f"per_frame_loss_weight needs {self.pred_frame_num} entries, got "
+                             f"{len(per_frame_loss_weight)}")
+        self.fuse_head_frames = True
+
+    # ------------------------------------------------------------------ GT alignment (:94-148)
+    @staticmethod
+    def _transforms(img_metas, src_frames, tgt_frames):
+        """total_cur2ref[src] @ total_ref2cur[tgt] per job and sample -> CPU float32 [jobs, bs, 4, 4], the
+        reference's fp32 CPU matmul."""
+        a = torch.from_numpy(np.array([[m["total_cur2ref_lidar_transform"][s] for m in img_metas]
+                                       for s in src_frames])).float()
+        b = torch.from_numpy(np.array([[m["total_ref2cur_lidar_transform"][t] for m in img_metas]
+                                       for t in tgt_frames])).float()
+        return torch.matmul(a, b)
+
+    @staticmethod
+    def _pack_gt(gt_points, device):
+        """Ragged GT list -> [bs, Mmax, Cg] NaN-padded (shapes are host-known: no sync)."""
+        return torch.nn.utils.rnn.pad_sequence([p.float() for p in gt_points], batch_first=True,
+                                               padding_value=float("nan")).to(device).contiguous()
+
+    @staticmethod
+    def _voxel_table(bev_h, bev_w, pillar_num, pc_range):
+        """bev_geometry.coords_to_voxel_grids as ((x - lo) * scale) * cells with torch's CUDA arithmetic for a
+        tensor divided by a host scalar (a multiply by its fp32 reciprocal)."""
+        r = pc_range
+        span = [r[3] - r[0], r[4] - r[1], r[5] - r[2]]
+        return ([np.float32(r[0]), np.float32(r[1]), np.float32(r[2])]
+                + [np.float32(1.0) / np.float32(s) for s in span] + [np.float32(bev_w), np.float32(bev_h),
+                                                                     np.float32(pillar_num)])
+
+    def _get_reference_gt_points(self, gt_points, src_frame_idx_list, tgt_frame_idx_list, img_metas):
+        """:94-148 -> (batched_gt_points: per sample [n_b, 4] rows (x, y, z, slot), slot-major,
+        batched_origin_points [bs, slots, 3]).  One alignment op; the per-sample row counts come back to the
+        host once (the list's shapes), instead of a boolean mask per (slot, sample)."""
+        dev = gt_points[0].device
+        mats = self._transforms(img_metas, src_frame_idx_list, tgt_frame_idx_list)
+        _, tindex, pts = ray_head.align_gt(self._pack_gt(gt_points, dev), mats.to(dev), [list(src_frame_idx_list)],
+                                           [0.0] * 3 + [1.0] * 3 + [0.0] * 3, with_points=True)
+        counts = (tindex >= 0).sum(1).tolist()
+        rows = [torch.cat([pts[b, :n], tindex[b, :n, None]], 1) for b, n in enumerate(counts)]
+        return rows, mats[:, :, 3, :3].permute(1, 0, 2).contiguous().to(dev)
+
+    def _align_torch(self, gt_points, src_frame_idx_list, tgt_frame_idx_list, img_metas):
+        """The reference's statements (boolean mask per slot and sample), the transform written out in the
+        alignment kernel's order: x' = ((x T0 + y T1) + z T2) + T3.  The reference of the tests."""
+        dev = gt_points[0].device
+        mats = self._transforms(img_metas, src_frame_idx_list, tgt_frame_idx_list).to(dev)
+        per_b = [[] for _ in gt_points]
+        for v, src in enumerate(src_frame_idx_list):
+            for b, p in enumerate(gt_points):
+                q = p[p[:, -1] == src].float()
+                T = mats[v, b]
+                xyz = [((q[:, 0] * T[0, a] + q[:, 1] * T[1, a]) + q[:, 2] * T[2, a]) + T[3, a] for a in range(3)]
+                per_b[b].append(torch.stack(xyz + [torch.full_like(q[:, 0], float(v))], 1))
+        return [torch.cat(r, 0) for r in per_b], mats[:, :, 3, :3].permute(1, 0, 2).contiguous()
+
+    # ------------------------------------------------------------------ loss (:150-219)
+    def _frame_plan(self, pred_dict):
+        valid_frames = np.array(pred_dict["valid_frames"])
+        start_frames = valid_frames + self.history_queue_length - self.pred_history_frame_num
+        tgt_frames = valid_frames + self.history_queue_length
+        if not pred_dict.get("full_prev_bev_exists", True):
+            frame_idx_for_loss = [self.pred_history_frame_num] * self.pred_frame_num
+        else:
+            frame_idx_for_loss = list(range(self.pred_frame_num))
+        return start_frames, tgt_frames, frame_idx_for_loss
+
+    def _head_frame_weight(self, i):
+        if i != self.pred_history_frame_num:     # auxiliary head frames supervise their first frame only
+            return np.array([[1]] + [[0]] * (len(self.loss_weight) - 1))
+        return self.loss_weight
+
+    def loss(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, pred_frame_num,
+             img_metas=None, batched_origin_points=None, gumbels=None):
+        """ViDARHeadV1.loss: keys 'frame.{idx}.{k}.loss'.  `gumbels`: optional list, one entry per loss index,
+        of the `gumbels` dict ViDARRayHead.loss takes for that head frame ({'dense': [bs, frames*R0, K]}); noise of
+        zero-weight pairs is not read."""
+        if not self.fuse_head_frames or self.use_dist_loss:
+            return self._loss_per_head_frame(pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range,
+                                             img_metas, gumbels)
+        bev_preds = pred_dict["next_bev_preds"]
+        V, _, Hf, bs, token_num, Z = bev_preds.shape
+        if Hf != self.pred_frame_num or len(gt_points) != bs:
+            raise ValueError(f"next_bev_preds [frames, inter, {self.pred_frame_num}, bs, tokens, Z] and bs GT "
+                             f"lists expected, got {tuple(bev_preds.shape)} and {len(gt_points)} lists")
+        dev = bev_preds.device
+        start_frames, tgt_frames, frame_idx_for_loss = self._frame_plan(pred_dict)
+        scale = np.zeros(Hf)
+        for idx, i in enumerate(frame_idx_for_loss):
+            if idx == i:
+                scale[i] = self.per_frame_loss_weight[i]
+        active = [i for i in range(Hf) if scale[i] != 0]
+        # slot v of a head frame is the base loss's frame t = v - start_idx when v is one of its frames
+        frames = [f for f in range(start_idx, len(self.loss_weight) - 1) if f < V]
+        slot_t = np.full(V, -1)
+        for f in frames:
+            slot_t[f] = f - start_idx
+        # host tables: per (head frame, sample, slot) the CE frame and weight; the weighted dense pairs
+        S = Hf * bs
+        ray_frame = np.full(S * V, -1)
+        ray_w = np.zeros(S * V)
+        pairs, pair_w, norms = [], [], np.ones(Hf)      # a head frame without pairs keeps norm 1 and loss 0
+        for i in active:
+            lw = self._head_frame_weight(i)
+            norms[i] = np.float32(float(lw.sum())) * np.float32(bs)
+            for b in range(bs):
+                s = i * bs + b
+                for v in range(V):
+                    t = slot_t[v]
+                    if t >= 0 and lw[t, 0] != 0:
+                        ray_frame[s * V + v] = s * V + t
+                        ray_w[s * V + v] = lw[t, 0]
+                for t in range(V):
+                    if lw[t, 0] != 0:
+                        pairs.append((s, t, s * V + t, i))
+                        pair_w.append(lw[t, 0])
+        jobs = np.full((Hf, V), -1)
+        src = np.zeros((Hf, V), dtype=np.int64)
+        for i in range(Hf):
+            src[i] = start_frames + i if i in active else tgt_frames
+            if i in active:
+                jobs[i] = src[i]
+        mats = self._transforms(img_metas, src.ravel(), np.tile(tgt_frames, Hf))           # [Hf*V, bs, 4, 4]
+        nm = mats.numel()
+        host = np.concatenate([mats.numpy().ravel(), ray_frame, ray_w, slot_t]).astype(np.float32)
+        table = ray_head._pinned_upload(host, np.float32, dev)
+        mats_d = table[:nm].view(Hf * V, bs, 4, 4)
+        ray_frame_d = table[nm:nm + S * V]
+        ray_w_d = table[nm + S * V:nm + 2 * S * V]
+        slot_t_d = table[nm + 2 * S * V:]
+
+        # 1. GT of every (head frame, sample), slot-major, in voxel units
+        rays, tv, _ = ray_head.align_gt(self._pack_gt(gt_points, dev), mats_d, jobs,
+                                        self._voxel_table(tgt_bev_h, tgt_bev_w, Z, tgt_pc_range))
+        key = (torch.arange(S, device=dev)[:, None] * V + tv.clamp(min=0).long())
+        live = tv >= 0
+        frame = torch.where(live, ray_frame_d[key], -1.0).to(torch.int32).view(-1).contiguous()
+        w_ray = torch.where(live, ray_w_d[key], 0.0).view(Hf, -1)
+        gt_t = torch.where(live, slot_t_d[tv.clamp(min=0).long()], -1.0).contiguous()
+        origin = mats_d[:, :, 3, :3].view(Hf, V, bs, 3).permute(0, 2, 1, 3).reshape(S * V, 3)
+        origin = bev_geometry.coords_to_voxel_grids(origin, bev_h=tgt_bev_h, bev_w=tgt_bev_w, pillar_num=Z,
+                                                    pc_range=tgt_pc_range).contiguous()
+        # [frames, inter, Hf, bs, tokens, Z] -> volumes [(i * bs + b) * V + v, Z, Y, X] of the last output
+        sigma = (bev_preds[:, -1].float().permute(1, 2, 0, 4, 3).contiguous()
+                 .view(S * V, Z, tgt_bev_h, tgt_bev_w))
+        step, K = self.ray_grid_step, self.ray_grid_num
+        terms = {}
+        if self.use_ce_loss:
+            ce, valid = ray_head.ray_ce(sigma, origin, rays.view(-1, 3), frame, K, step)
+            w = w_ray * valid.view(Hf, -1)
+            terms["regularization.loss"] = (ce.view(Hf, -1) * w).sum(1) / torch.clamp(w.sum(1), min=1)
+        if self.use_dense_loss:
+            dense = sigma.new_zeros(Hf)
+            if pairs:
+                tab = np.array(pairs, dtype=np.int64)
+                P = len(pairs)
+                grid = self._dense_grid(tgt_bev_h, tgt_bev_w, Z, dev)
+                R0 = grid.shape[0]
+                comp = torch.from_numpy(tab[:, 2].astype(np.int32)).pin_memory().to(dev, non_blocking=True)
+                noise = self._pair_noise(gumbels, frame_idx_for_loss, tab, bs, R0, dev)
+                dist = ray_head.gumbel_distance(sigma, origin, grid.repeat(P, 1),
+                                                comp[:, None].expand(P, R0).reshape(-1).contiguous(), K, step, noise)
+                dense = ray_head.dense_chamfer_group_loss(
+                    dist, grid.repeat(P, 1), origin, rays, gt_t, (tgt_bev_w, tgt_bev_h, Z), tab, pair_w, norms,
+                    self.eval_within_grid, tgt_pc_range)
+            terms["loss.dense_voxel"] = dense * self.dense_loss_weight
+        loss_dict = dict()
+        for idx, i in enumerate(frame_idx_for_loss):
+            for k, v in terms.items():
+                loss_dict[f"frame.{idx}.{k}.loss"] = v[i] * (self.per_frame_loss_weight[i] * (idx == i))
+        return loss_dict
+
+    @staticmethod
+    def _dense_grid(bev_h, bev_w, Z, device):
+        """The dense term's ray end points of one sample (vidar_head_base.py:611-619), [R0, 3] voxel units."""
+        interval = 4
+        g = bev_geometry.get_bev_grids_3d(bev_h // interval, bev_w // interval, Z // interval, bs=1, device=device)
+        g[..., 0] = g[..., 0] * bev_w
+        g[..., 1] = g[..., 1] * bev_h
+        g[..., 2] = g[..., 2] * Z
+        return g.view(-1, 3).contiguous()
+
+    def _pair_noise(self, gumbels, frame_idx_for_loss, tab, bs, R0, device):
+        """Gumbel noise [P*R0, K] of the weighted pairs: slices of the per-head-frame noise when given, else drawn
+        with the statement F.gumbel_softmax uses."""
+        P, K = tab.shape[0], self.ray_grid_num
+        if gumbels is None:
+            return -torch.empty((P * R0, K), dtype=torch.float32, device=device).exponential_().log()
+        loss_idx = {i: idx for idx, i in enumerate(frame_idx_for_loss) if idx == i}
+        parts = []
+        for s, t, _, i in tab:
+            parts.append(gumbels[loss_idx[int(i)]]["dense"][int(s) - int(i) * bs, t * R0:(t + 1) * R0])
+        return torch.cat(parts, 0).float().contiguous()
+
+    def _loss_per_head_frame(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas,
+                             gumbels):
+        """The reference's loop (:167-219): one ViDARRayHead.loss per head frame."""
+        bev_preds = pred_dict["next_bev_preds"]
+        start_frames, tgt_frames, frame_idx_for_loss = self._frame_plan(pred_dict)
+        loss_dict = dict()
+        for idx, i in enumerate(frame_idx_for_loss):
+            cur_bev_preds = bev_preds[:, :, i, ...].contiguous()
+            src_frames = start_frames + i
+            cur_gt_points, cur_origin_points = self._align_torch(gt_points, src_frames, tgt_frames, img_metas)
+            cur_loss_dict = ViDARRayHead.loss(
+                self, dict(next_bev_preds=cur_bev_preds, valid_frames=np.arange(0, len(src_frames))), cur_gt_points,
+                start_idx=start_idx, tgt_bev_h=tgt_bev_h, tgt_bev_w=tgt_bev_w, tgt_pc_range=tgt_pc_range,
+                pred_frame_num=len(self.loss_weight) - 1, img_metas=img_metas,
+                batched_origin_points=cur_origin_points, loss_weight=self._head_frame_weight(i),
+                gumbels=gumbels[idx] if gumbels is not None else None)
+            cur_frame_loss_weight = self.per_frame_loss_weight[i] * (idx == i)
+            for k, v in cur_loss_dict.items():
+                loss_dict[f"frame.{idx}.{k}.loss"] = v * cur_frame_loss_weight
+        return loss_dict
+
+    # ------------------------------------------------------------------ decode (:221-252)
+    def get_point_cloud_prediction(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range,
+                                   img_metas=None, batched_origin_points=None):
+        """The current head frame's prediction, decoded against its own frames' GT (src == tgt)."""
+        cur = dict(pred_dict)
+        cur["next_bev_preds"] = pred_dict["next_bev_preds"][:, :, self.pred_history_frame_num, ...].contiguous()
+        valid_frames = np.array(pred_dict["valid_frames"])
+        frames = valid_frames + self.history_queue_length
+        valid_gt_points, cur_origin_points = self._get_reference_gt_points(gt_points, frames, frames, img_metas)
+        return ViDARRayHead.get_point_cloud_prediction(self, cur, valid_gt_points, start_idx, tgt_bev_h, tgt_bev_w,
+                                                       tgt_pc_range, img_metas=img_metas,
+                                                       batched_origin_points=cur_origin_points)

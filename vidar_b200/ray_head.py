@@ -14,6 +14,10 @@ projects/mmdet3d_plugin/bevformer/dense_heads/vidar_head_base.py:
   dense_chamfer_loss(...)     == the Chamfer loop of the `use_dense_loss` branch of ViDARHeadBase.loss
                                  (:638-659) over every (sample, frame) pair in one batched op
                                  (csrc/dense_chamfer.cu), no host sync.
+  dense_chamfer_group_loss(...) == the same Chamfer term over a pair table, one loss per group
+                                 (ViDARHeadV1: a group per head frame);
+  align_gt(...)               == ViDARHeadV1._get_reference_gt_points (vidar_head_v1.py:94-148) for every
+                                 (head frame, target frame) job in one op.
 
 Low-level autograd ops: `ray_sample` (logits/lengths, differentiable w.r.t. sigma) and `ray_ce`.
 All tensors must be CUDA; there is no PyTorch fallback.
@@ -352,3 +356,132 @@ def dense_chamfer_loss(dist, points, origin, gt, gt_tindex, grid, frame_weights,
     loss, pairs = _DenseChamfer.apply(dist, points, origin, gt, gt_tindex, grid, frame_weights, weight_sum,
                                       eval_within_grid, pc_range if pc_range is not None else [0.0] * 6)
     return (loss, pairs) if return_pairs else loss
+
+
+def _pinned_upload(host, dtype, device):
+    """Host array -> device tensor by one pinned non-blocking copy (no host sync)."""
+    t = torch.from_numpy(np.ascontiguousarray(host, dtype=dtype)).pin_memory()
+    return t.to(device, non_blocking=True)
+
+
+class _DenseChamferGroups(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, dist, points, origin, gt, gt_tindex, tables, dims, grid, within_grid, pc_range):
+        slot_pair, pair_tab, pair_w, group_norm = tables
+        P, groups, R0, Sg, Fg, M = dims
+        dev = dist.device
+        W, H, Z = (int(v) for v in grid)
+        Pq = P * R0 + Sg * M
+        qbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
+        cbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
+        q_mask = torch.empty(Pq, dtype=torch.uint8, device=dev)
+        c_mask = torch.empty(Pq, dtype=torch.uint8, device=dev)
+        seg_off = torch.empty((2, 2 * P + 1), dtype=torch.int64, device=dev)
+        idx = torch.empty(Pq, dtype=torch.int64, device=dev)
+        pairs = torch.empty((P, 4), dtype=torch.float64, device=dev)
+        loss = torch.empty(groups, dtype=torch.float32, device=dev)
+        rng = (C.c_float * 6)(*[float(v) for v in pc_range])
+        Pt = _lib.ptr
+        _call(_lib.lib().vidar_dense_chamfer_groups_forward, dev, Pt(dist), Pt(points), Pt(origin), Pt(gt),
+              Pt(gt_tindex), Pt(slot_pair), Pt(pair_tab), Pt(pair_w), Pt(group_norm), C.cast(rng, C.c_void_p),
+              Pt(qbuf), Pt(cbuf), Pt(q_mask), Pt(c_mask), Pt(seg_off[0]), Pt(seg_off[1]), Pt(idx), Pt(pairs),
+              Pt(loss), P, groups, R0, Sg, Fg, M, W, H, Z, int(bool(within_grid)))
+        ctx.save_for_backward(points, origin, qbuf, cbuf, q_mask, seg_off, idx, pairs, pair_tab, pair_w, group_norm)
+        ctx.dims = dims
+        ctx.mark_non_differentiable(pairs)
+        return loss, pairs
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_loss, _gp):
+        points, origin, qbuf, cbuf, q_mask, seg_off, idx, pairs, pair_tab, pair_w, group_norm = ctx.saved_tensors
+        P, groups, R0, Sg, Fg, M = ctx.dims
+        g = grad_loss.float().contiguous()
+        grad_dist = torch.empty(P * R0, dtype=torch.float32, device=qbuf.device)
+        Pt = _lib.ptr
+        _call(_lib.lib().vidar_dense_chamfer_groups_backward, qbuf.device, Pt(points), Pt(origin), Pt(qbuf),
+              Pt(cbuf), Pt(q_mask), Pt(seg_off[0]), Pt(seg_off[1]), Pt(idx), Pt(pairs), Pt(pair_tab), Pt(pair_w),
+              Pt(group_norm), Pt(g), Pt(grad_dist), P, groups, R0, Sg, Fg, M)
+        return grad_dist, None, None, None, None, None, None, None, None, None
+
+
+def dense_chamfer_group_loss(dist, points, origin, gt, gt_tindex, grid, pairs, pair_weights, group_norms,
+                             eval_within_grid=False, pc_range=None, return_pairs=False):
+    """`dense_chamfer_loss` over a pair table, one loss per group, differentiable in `dist`.
+
+    dist [P*R0] decoded lengths, points [P*R0, 3] ray end points (rays of pair n at n*R0 ..), origin [No, 3],
+    gt [Sg, M, 3] and gt_tindex [Sg, M] (float frame in [0, Fg), -1 = padding, any order), voxel units on one CUDA
+    device; grid = (W, H, Z).  Host tables: pairs [P, 4] ints (gt sample, gt frame, origin row, group), in increasing
+    (gt sample, gt frame) order; pair_weights [P]; group_norms [groups].
+    loss[g] = sum over the pairs n of group g of w_n * (mean pred->gt + mean gt->pred) / 2 / group_norms[g].
+    Returns loss [groups] (and, with return_pairs, the [P, 4] float64 per-pair sums of dense_chamfer_loss)."""
+    tab = np.asarray(pairs, dtype=np.int64).reshape(-1, 4)
+    w = np.asarray(pair_weights, dtype=np.float32).reshape(-1)
+    norms = np.asarray(group_norms, dtype=np.float32).reshape(-1)
+    P, groups = tab.shape[0], norms.shape[0]
+    if P == 0 or w.shape[0] != P or groups == 0:
+        raise RuntimeError(f"need P > 0 pairs [P, 4] with P weights and > 0 group norms, got {tab.shape}, "
+                           f"{w.shape}, {norms.shape}")
+    if dist.dim() != 1 or dist.shape[0] % P:
+        raise RuntimeError(f"dist must be [P*R0] with P = {P} pairs, got {tuple(dist.shape)}")
+    R0 = dist.shape[0] // P
+    if gt.dim() != 3 or gt.shape[2] != 3 or tuple(gt_tindex.shape) != tuple(gt.shape[:2]):
+        raise RuntimeError("expected gt [Sg, M, 3] and gt_tindex [Sg, M]")
+    Sg, M = gt.shape[:2]
+    if tuple(points.shape) != (P * R0, 3) or origin.dim() != 2 or origin.shape[1] != 3:
+        raise RuntimeError("expected points [P*R0, 3] and origin [No, 3]")
+    for name, t in (("dist", dist), ("points", points), ("origin", origin), ("gt", gt), ("gt_tindex", gt_tindex)):
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must be float32")
+    Fg = int(tab[:, 1].max()) + 1
+    slot = tab[:, 0] * Fg + tab[:, 1]
+    if ((tab[:, 0] < 0) | (tab[:, 0] >= Sg) | (tab[:, 1] < 0)).any() or (np.diff(slot) <= 0).any():
+        raise RuntimeError("pairs must name distinct (gt sample, frame) slots in increasing order")
+    if ((tab[:, 2] < 0) | (tab[:, 2] >= origin.shape[0]) | (tab[:, 3] < 0) | (tab[:, 3] >= groups)).any():
+        raise RuntimeError("pair origin row or group out of range")
+    if eval_within_grid and pc_range is None:
+        raise RuntimeError("eval_within_grid needs pc_range")
+    _lib.require_cuda(dist=dist, points=points, origin=origin, gt=gt, gt_tindex=gt_tindex)
+    slot_pair = np.full(Sg * Fg, -1, dtype=np.int64)
+    slot_pair[slot] = np.arange(P)
+    ints = _pinned_upload(np.concatenate([slot_pair, np.stack([slot, tab[:, 2], tab[:, 3]], 1).ravel()]), np.int32,
+                          dist.device)
+    floats = _pinned_upload(np.concatenate([w, norms]), np.float32, dist.device)
+    tables = (ints[: Sg * Fg], ints[Sg * Fg:], floats[:P], floats[P:])
+    loss, pair_sums = _DenseChamferGroups.apply(dist, points, origin, gt, gt_tindex, tables,
+                                                (P, groups, R0, Sg, Fg, M), grid, eval_within_grid,
+                                                pc_range if pc_range is not None else [0.0] * 6)
+    return (loss, pair_sums) if return_pairs else loss
+
+
+def align_gt(gt, mats, jobs, voxel, with_points=False):
+    """GT alignment of ViDARHeadV1 for every head frame (vidar_head_v1.py:94-148), csrc/dense_chamfer.cu.
+
+    gt [bs, M, Cg] float32 GT rows in metres, NaN-padded, the frame in the last column; mats [H*V, bs, 4, 4]
+    float32 (device) src -> tgt transform per (head frame, slot) job; jobs: host ints [H, V], the source frame of
+    each job, -1 = none; voxel: host (offset[3], scale[3], cells[3]), ray = ((x' - offset) * scale) * cells.
+    Returns rays [H*bs, M, 3] voxel units, tindex [H*bs, M] (slot, -1 = padding) and, with_points, the aligned
+    points [H*bs, M, 3] in metres: per (head frame, sample) the slots in order, the rows of a slot in their order,
+    then padding."""
+    jobs = np.asarray(jobs, dtype=np.int64)
+    if jobs.ndim != 2:
+        raise RuntimeError(f"jobs must be [head frames, slots], got shape {jobs.shape}")
+    H, V = jobs.shape
+    if gt.dim() != 3 or gt.shape[2] < 4 or gt.dtype != torch.float32:
+        raise RuntimeError("gt must be float32 [bs, M, Cg >= 4]")
+    bs, M, Cg = gt.shape
+    if tuple(mats.shape) != (H * V, bs, 4, 4) or mats.dtype != torch.float32:
+        raise RuntimeError(f"mats must be float32 {(H * V, bs, 4, 4)}, got {tuple(mats.shape)}")
+    voxel = np.asarray(voxel, dtype=np.float32).reshape(-1)
+    if voxel.shape != (9,):
+        raise RuntimeError("voxel must hold 9 floats: offset[3], scale[3], cells[3]")
+    _lib.require_cuda(gt=gt, mats=mats)
+    dev = gt.device
+    rays = torch.empty((H * bs, M, 3), dtype=torch.float32, device=dev)
+    tindex = torch.empty((H * bs, M), dtype=torch.float32, device=dev)
+    points = torch.empty((H * bs, M, 3), dtype=torch.float32, device=dev) if with_points else None
+    j = (C.c_int32 * (H * V))(*[int(v) for v in jobs.ravel()])
+    vx = (C.c_float * 9)(*[float(v) for v in voxel])
+    _call(_lib.lib().vidar_head_align_gt, dev, _lib.ptr(gt), _lib.ptr(mats), C.cast(j, C.c_void_p),
+          C.cast(vx, C.c_void_p), _lib.ptr(rays), _lib.ptr(tindex), _lib.ptr(points), bs, M, Cg, H, V)
+    return rays, tindex, points
