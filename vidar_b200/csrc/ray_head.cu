@@ -138,6 +138,25 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// The order of torch's max / argmax: a NaN above every number, the smaller index on ties (and among NaNs).
+// A lane that holds no sample starts at (-inf, INT_MAX), so its first sample always replaces it.
+__device__ __forceinline__ bool argmax_takes(float v, int k, float best, int best_k) {
+  const bool vn = isnan(v), bn = isnan(best);
+  if (vn != bn) return vn;
+  return (vn || v == best) ? k < best_k : v > best;
+}
+
+// warp arg-max of (value, index) in that order, carrying the winner's length
+__device__ __forceinline__ void warp_argmax(float& best, int& best_k, float& best_len) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int ok = __shfl_xor_sync(0xffffffffu, best_k, o);
+    const float ol = __shfl_xor_sync(0xffffffffu, best_len, o);
+    if (argmax_takes(ov, ok, best, best_k)) { best = ov; best_k = ok; best_len = ol; }
+  }
+}
+
 // ---- materialising sampler (API parity with _get_grid_features) --------------------------
 __global__ void __launch_bounds__(kRaysPerBlock * 32)
 ray_sample_kernel(RayDims D, const float* __restrict__ sigma, const float* __restrict__ origin,
@@ -252,7 +271,10 @@ ray_ce_bwd_kernel(RayDims D, const float* __restrict__ sigma, const float* __res
 // ---- fused gumbel decode of the dense loss term --------------------------------------------
 // ViDARHeadBase._custom_gumbel_softmax_distance (vidar_head_base.py:754-773) on the sampler's
 // logits without the GT slot (`dense_feat_total[0][..., 1:]`, :631-636), per ray:
-//   idx   = argmax_k (logit_k + gumbel_k)                 F.gumbel_softmax(hard=True), forward value
+//   idx   = argmax_k (logit_k + gumbel_k)                 F.gumbel_softmax(hard=True), forward value; the
+//                                                         reference takes the arg-max of softmax(logit + gumbel),
+//                                                         which can round two distinct maxima to one value
+//                                                         (DESIGN.md 4.4): this is the exact arg-max in fp32
 //   pred  = length_idx                                    ((1 - s) + s == 1 exactly in fp32)
 //   p     = sum_{length_k > pred} e^{logit_k} / sum_k e^{logit_k}
 //   out   = (1 - p.detach() + p) * pred  = pred,          d out / d logit_j = pred * softmax_j * ([length_j > pred] - p)
@@ -279,17 +301,11 @@ ray_gumbel_fwd_kernel(RayDims D, const float* __restrict__ sigma, const float* _
     const Sample q = make_sample(D, s, k);
     const float v = q.masked ? -INFINITY : trilinear(vol, corners(D, q));
     const float y = v + __ldg(nz + k - 1);
-    if (best_k == 0x7fffffff || y > best) { best = y; best_k = k; best_len = q.length; }
+    if (argmax_takes(y, k, best, best_k)) { best = y; best_k = k; best_len = q.length; }
     if (v > m) { acc = acc * expf(m - v) + 1.f; m = v; }
     else if (v > -INFINITY) acc += expf(v - m);
   }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {   // warp arg-max, smallest index wins ties
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int ok = __shfl_xor_sync(0xffffffffu, best_k, o);
-    const float ol = __shfl_xor_sync(0xffffffffu, best_len, o);
-    if (ov > best || (ov == best && ok < best_k)) { best = ov; best_k = ok; best_len = ol; }
-  }
+  warp_argmax(best, best_k, best_len);
   const float M = warp_max(m);
   const float S = warp_sum((m == -INFINITY) ? 0.f : acc * expf(m - M));
   float nx = 0.f;
@@ -299,7 +315,9 @@ ray_gumbel_fwd_kernel(RayDims D, const float* __restrict__ sigma, const float* _
     nx += expf(trilinear(vol, corners(D, q)) - M);
   }
   nx = warp_sum(nx);
-  if (lane == 0) { dist[r] = best_len; lse_out[r] = M + logf(S); p_out[r] = nx / S; }
+  // every waypoint masked (the origin outside the volume): S = 0, the reference's softmax is NaN; here the
+  // first waypoint's length, lse = -inf, p_next = 0, and the backward scatters nothing (DESIGN.md 4.4)
+  if (lane == 0) { dist[r] = best_len; lse_out[r] = M + logf(S); p_out[r] = S > 0.f ? nx / S : 0.f; }
 }
 
 __global__ void __launch_bounds__(kRaysPerBlock * 32)
@@ -354,16 +372,9 @@ ray_argmax_kernel(RayDims D, const float* __restrict__ sigma, const float* __res
     const Sample q = make_sample(D, s, k);
     float v = trilinear(vol, corners(D, q));     // no mask here: outside samples are exactly 0
     if (v == 0.f) v = -INFINITY;                  // masked_fill(sigma == 0, -inf)  (:728)
-    if (best_k == 0x7fffffff || v > best) { best = v; best_k = k; best_len = q.length; }
+    if (argmax_takes(v, k, best, best_k)) { best = v; best_k = k; best_len = q.length; }
   }
-  // warp arg-max with smallest-index tie-break
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int ok = __shfl_xor_sync(0xffffffffu, best_k, o);
-    const float ol = __shfl_xor_sync(0xffffffffu, best_len, o);
-    if (ov > best || (ov == best && ok < best_k)) { best = ov; best_k = ok; best_len = ol; }
-  }
+  warp_argmax(best, best_k, best_len);
   if (lane == 0) {
     depth[r] = best_len;
     if (index) index[r] = (float)best_k;
