@@ -440,7 +440,8 @@ int vidar_eval_prologue(const float* pred, const float* gt, const float* origin,
 
 /* Ray errors and the deterministic per-cloud reduction over the NN results of the 3N segments
  * (vidar_nn_segments_forward on the prologue's layout; dists / idx [Pp + 2Pg]).
- *   partials: 3N * ceil(max_len / 256) * 4 doubles of scratch, max_len >= every cloud's size
+ *   partials: 3N * ceil(max_len / 256) * 4 doubles of scratch, max_len >= every cloud's size (a cloud whose points
+ *       are all masked, like the trailing segment of vidar_eval_decode_clouds, may be longer: it adds nothing)
  *   out [N, VIDAR_EVAL_FIELDS] fp64: sum l1, sum absrel, count (gt points kept), sum forward d, pred points
  *       inside, sum backward d, gt points inside, flags (VIDAR_EVAL_* bits)
  *   rays [Pg, 9] (NULL = skip): interpolated point, clamped gt, clamped interpolated point (NaN for masked gt) */
@@ -454,6 +455,26 @@ int vidar_eval_metrics(const float* pred, const float* gt, const float* origin, 
                        const int64_t* gt_off, const int64_t* q_off, const unsigned char* q_mask,
                        const float* dists, const int64_t* idx, double* partials, double* out, float* rays,
                        int N, int max_len, void* stream);
+
+/* The head's decoded rays -> the pred and gt clouds of every (sample, frame), in place of get_point_cloud_prediction's
+ * per-(sample, frame) boolean masks (dense_heads/vidar_head_base.py:698-745, get_rendered_pcds :363-389).
+ *   depth [bs, M]        arg-max depth of every row (voxel units; vidar_ray_argmax)
+ *   rays [bs, M, 3]      GT points in voxel units;  points [bs, M, 3] the same points in metres
+ *   tindex [bs, M]       float frame of each row; -1 or any value outside [0, F) = in no cloud
+ *   origin_vox, origin   [bs, F, 3] in voxel units / metres;  scale = (pc_range[3] - pc_range[0]) / bev_w
+ *   pc_range_host        6 floats (HOST), read when within_grid
+ * Row i of sample b joins cloud n = b * F + t when tindex == t, gt_dist = |rays - origin_vox| * scale > 0 and (within_grid)
+ * its metre point is inside pc_range.  Outputs:
+ *   pred, gt [bs * M, 3] metres: origin + unit(point - origin) * dist with dist = depth * scale / gt_dist, the rows of a
+ *            cloud in their original order
+ *   off [bs * F + 2] int64: cloud n at rows [off[n], off[n+1]); segment bs * F, rows [off[bs*F], bs * M), holds the
+ *            other rows as NaN, so vidar_eval_prologue masks all of them.  Pred and gt share the offsets.
+ * Feed the N + 1 = bs * F + 1 segments to vidar_eval_prologue / _metrics with Pp = Pg = bs * M, max_len = M, and drop
+ * the last row of the table.  3 launches (1 when M = 0), scratch from the library's memory pool, no host sync. */
+int vidar_eval_decode_clouds(const float* depth, const float* rays, const float* points, const float* tindex,
+                             const float* origin_vox, const float* origin, const float* pc_range_host, float scale,
+                             int within_grid, float* pred, float* gt, int64_t* off, int bs, int M, int F,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------
  * (v) The head's dense loss term 'loss.dense_voxel' (dense_heads/vidar_head_base.py:594-659, get_rendered_pcds

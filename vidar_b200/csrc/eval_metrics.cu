@@ -11,7 +11,15 @@
 //   queries    [pred xyz (Pp) | gt xyz (Pg) | gt spherical (Pg)]   segments 0..N-1 | N..2N-1 | 2N..3N-1
 //   candidates [gt xyz (Pg) | pred xyz (Pp) | pred spherical (Pp)]
 // so one segmented NN launch (knn.cu) serves both Chamfer directions and the spherical search.
+//
+// vidar_eval_decode_clouds builds those clouds on the device from the head's decoded rays
+// (dense_heads/vidar_head_base.py:698-745 get_point_cloud_prediction, :363-389 get_rendered_pcds): row r of sample b
+// joins cloud n = b * F + t when tindex == t, gt_dist > 0 and (within_grid) its metre point is inside pc_range.  A
+// stable counting sort keyed by (b, t) (counting_sort.cuh) keeps the rows of a cloud in their original order, which
+// decides NN ties as the boolean masks of the reference do.  Every other row goes, as NaN, into one trailing segment
+// N that every search and sum masks out; its row of the metric table is dropped by the caller.
 #include "common.cuh"
+#include "counting_sort.cuh"
 
 namespace vidar {
 namespace {
@@ -274,7 +282,8 @@ __global__ void eval_finish_kernel(const int64_t* __restrict__ q_off, const doub
   for (int r = 0; r < 3; ++r) {
     const int s = r * N + n;
     const long long Lq = q_off[s + 1] - q_off[s];
-    const int nb = (int)((Lq + kEvalThreads - 1) / kEvalThreads);
+    int nb = (int)((Lq + kEvalThreads - 1) / kEvalThreads);
+    if (nb > nbx) nb = nbx;      // only a fully masked segment (decode_clouds' trailing one) is longer than max_len
     for (int bx = 0; bx < nb; ++bx) {
       const double* p = partials + ((size_t)s * nbx + bx) * 4;
       acc[r][0] += p[0]; acc[r][1] += p[1]; acc[r][2] += p[2];
@@ -288,10 +297,140 @@ __global__ void eval_finish_kernel(const int64_t* __restrict__ q_off, const doub
   o[7] = (double)flags;
 }
 
+// ------------------------------------------------------------------ decoded rays -> per-(sample, frame) clouds
+struct DecodeDims {
+  int bs, M, F, nchunk, within;
+  float scale;      // (pc_range[3] - pc_range[0]) / bev_w, as torch rounds the Python float
+  float pc[6];
+};
+
+// Frame t of row i of sample b when the row joins cloud b * F + t, else -1; gt_dist (metres) of a joining row.
+// gt_dist = sqrt(sum (g_vox - o_vox)^2) * scale (ray_head.decode_ray_depth, then `gt_dist * scale`).
+__device__ __forceinline__ int decode_frame(const DecodeDims& D, const float* __restrict__ rays,
+                                            const float* __restrict__ points, const float* __restrict__ tindex,
+                                            const float* __restrict__ origin_vox, int b, int i, float& gt_dist) {
+  const size_t k = (size_t)b * D.M + i;
+  const float t = tindex[k];
+  if (!(t >= 0.f && t < (float)D.F && t == floorf(t))) return -1;
+  const int f = (int)t;
+  const float* o = origin_vox + ((size_t)b * D.F + f) * 3;
+  const float* g = rays + k * 3;
+  gt_dist = __fmul_rn(norm3(__fsub_rn(g[0], o[0]), __fsub_rn(g[1], o[1]), __fsub_rn(g[2], o[2])), D.scale);
+  if (!(gt_dist > 0.f)) return -1;
+  if (D.within) {     // get_inside_mask on the metre point, float32 bounds, inclusive
+    const float* p = points + k * 3;
+    if (!(D.pc[0] <= p[0] && p[0] <= D.pc[3] && D.pc[1] <= p[1] && p[1] <= D.pc[4] && D.pc[2] <= p[2] &&
+          p[2] <= D.pc[5]))
+      return -1;
+  }
+  return f;
+}
+
+// grid (nchunk, bs): per-(cloud, chunk) row counts
+__global__ void __launch_bounds__(kSortChunk)
+decode_count_kernel(DecodeDims D, const float* __restrict__ rays, const float* __restrict__ points,
+                    const float* __restrict__ tindex, const float* __restrict__ origin_vox, int* __restrict__ counts) {
+  extern __shared__ int hist[];       // [32][F]
+  const int b = blockIdx.y, c = blockIdx.x, i = c * kSortChunk + threadIdx.x;
+  float gd = 0.f;
+  const int f = i < D.M ? decode_frame(D, rays, points, tindex, origin_vox, b, i, gd) : -1;
+  sort_count(f, D.F, b, c, D.nchunk, hist, counts);
+}
+
+// One block: cloud offsets off[0..N] (cloud n = slot b * F + t), then off[N + 1] = bs * M closes the trailing segment.
+__global__ void decode_offsets_kernel(DecodeDims D, int* __restrict__ counts, int64_t* __restrict__ off) {
+  const int N = D.bs * D.F;
+  sort_offsets(N, D.nchunk, counts, off);
+  if (threadIdx.x == 0) off[N + 1] = (int64_t)D.bs * D.M;
+}
+
+// grid as the count kernel: every joining row to its place in its cloud, both points rendered from the metre
+// origin o and point p with get_rendered_pcds' statements, o + ((p - o) / sqrt(sum (p - o)^2)) * dist, for
+// dist = depth * scale (pred) and gt_dist (gt).  Rows [off[N], bs * M) of both clouds are NaN.
+__global__ void __launch_bounds__(kSortChunk)
+decode_scatter_kernel(DecodeDims D, const float* __restrict__ depth, const float* __restrict__ rays,
+                      const float* __restrict__ points, const float* __restrict__ tindex,
+                      const float* __restrict__ origin_vox, const float* __restrict__ origin,
+                      const int* __restrict__ counts, const int64_t* __restrict__ off, float* __restrict__ pred,
+                      float* __restrict__ gt) {
+  extern __shared__ int hist[];
+  const int b = blockIdx.y, c = blockIdx.x, i = c * kSortChunk + threadIdx.x;
+  float gd = 0.f;
+  const int f = i < D.M ? decode_frame(D, rays, points, tindex, origin_vox, b, i, gd) : -1;
+  const int pos = sort_rank(f, D.F, hist);
+  const int64_t r = (int64_t)b * D.M + i;
+  if (i < D.M && r >= off[D.bs * D.F]) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) pred[r * 3 + a] = gt[r * 3 + a] = NAN;
+  }
+  if (f < 0) return;
+  const int n = b * D.F + f;
+  const int64_t dst = off[n] + counts[(size_t)n * D.nchunk + c] + pos;
+  const float* o = origin + (size_t)n * 3;
+  const float* p = points + r * 3;
+  const float v[3] = {__fsub_rn(p[0], o[0]), __fsub_rn(p[1], o[1]), __fsub_rn(p[2], o[2])};
+  const float len = norm3(v[0], v[1], v[2]);
+  const float pd = __fmul_rn(depth[r], D.scale);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float u = __fdiv_rn(v[a], len);
+    pred[dst * 3 + a] = __fadd_rn(o[a], __fmul_rn(u, pd));
+    gt[dst * 3 + a] = __fadd_rn(o[a], __fmul_rn(u, gd));
+  }
+}
+
 }  // namespace
 }  // namespace vidar
 
 using namespace vidar;
+
+extern "C" int vidar_eval_decode_clouds(const float* depth, const float* rays, const float* points,
+                                        const float* tindex, const float* origin_vox, const float* origin,
+                                        const float* pc_range_host, float scale, int within_grid, float* pred,
+                                        float* gt, int64_t* off, int bs, int M, int F, void* stream) {
+  const char* who = "eval_decode_clouds";
+  VIDAR_REQUIRE(bs > 0 && M >= 0 && F > 0 && F <= 64, "%s: bad sizes bs=%d M=%d F=%d (F <= 64)", who, bs, M, F);
+  VIDAR_REQUIRE(bs <= 65535 && (long long)bs * F + 1 <= 65535 / 3, "%s: %lld clouds, at most %d", who,
+                (long long)bs * F, 65535 / 3 - 1);
+  VIDAR_REQUIRE((long long)bs * M < (1LL << 31), "%s: %lld rows, at most 2^31 - 1", who, (long long)bs * M);
+  VIDAR_REQUIRE(off && (M == 0 || (depth && rays && points && tindex && origin_vox && origin && pred && gt)),
+                "%s: null pointer argument", who);
+  VIDAR_REQUIRE(!within_grid || pc_range_host, "%s: within_grid needs pc_range", who);
+  DecodeDims D{};
+  D.bs = bs; D.M = M; D.F = F; D.within = within_grid ? 1 : 0; D.scale = scale;
+  D.nchunk = (M + kSortChunk - 1) / kSortChunk;
+  if (within_grid)
+    for (int k = 0; k < 6; ++k) D.pc[k] = pc_range_host[k];
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N = bs * F;
+  const size_t bytes = sizeof(int) * ((size_t)N * D.nchunk + 1);
+  cudaMemPool_t pool;
+  cudaError_t e = scratch_pool(&pool);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: scratch memory pool: %s", who, cudaGetErrorString(e));
+  int* counts = nullptr;
+  e = cudaMallocFromPoolAsync((void**)&counts, bytes, pool, st);
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cudaMallocFromPoolAsync: %s", who, cudaGetErrorString(e));
+  const dim3 grid(D.nchunk, bs);
+  const size_t smem = sizeof(int) * 32 * F;
+  int rc = VIDAR_OK;
+  if (M > 0) {
+    decode_count_kernel<<<grid, kSortChunk, smem, st>>>(D, rays, points, tindex, origin_vox, counts);
+    rc = check_launch("eval_decode_clouds(count)");
+  }
+  if (!rc) {
+    decode_offsets_kernel<<<1, 256, 0, st>>>(D, counts, off);
+    rc = check_launch("eval_decode_clouds(offsets)");
+  }
+  if (!rc && M > 0) {
+    decode_scatter_kernel<<<grid, kSortChunk, smem, st>>>(D, depth, rays, points, tindex, origin_vox, origin, counts,
+                                                          off, pred, gt);
+    rc = check_launch("eval_decode_clouds(scatter)");
+  }
+  e = cudaFreeAsync(counts, st);
+  if (rc) return rc;
+  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: cudaFreeAsync: %s", who, cudaGetErrorString(e));
+  return VIDAR_OK;
+}
 
 extern "C" int vidar_eval_prologue(const float* pred, const float* gt, const float* origin, const int64_t* pred_off,
                                    const int64_t* gt_off, const float* pc_range_host, float* qbuf, float* cbuf,

@@ -123,6 +123,7 @@ nn_segments_kernel(const float* __restrict__ q, const float* __restrict__ c, con
   if (j0 >= j1) return;
   float a[3];
   const bool live = i < Lq && (!q_mask || q_mask[q0 + i]);
+  if (!__syncthreads_or(live)) return;      // a block of masked queries only: no tile to scan
 #pragma unroll
   for (int d = 0; d < 3; ++d) a[d] = live ? q[(q0 + i) * 3 + d] : 0.f;
   float bd = INFINITY;

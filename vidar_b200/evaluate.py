@@ -10,7 +10,8 @@ frame_metrics scores every (sample, frame) pair of a batch in five kernel launch
 and frame count, and copies one [bs * F, 8] float64 tensor to the host at the end.  Failures the reference
 raises surface with the same exception types: a degenerate ray (RuntimeError), a clamped ray that never
 touches the volume (AssertionError); gt points kept with no pred point kept, where the reference fails with an
-IndexError, raise ValueError naming the (sample, frame).  CUDA tensors only.
+IndexError, raise ValueError naming the (sample, frame).  CUDA tensors only.  `metrics_flat` is the same pass over
+clouds already laid out flat with device offsets (the head's batched `evaluate` builds them on the device).
 """
 import ctypes as C
 
@@ -64,9 +65,19 @@ def metrics_device(preds, gts, origins, pc_range=DEFAULT_PC_RANGE, rays=False):
     psz = [int(p.shape[0]) for p in preds]
     gsz = [int(g.shape[0]) for g in gts]
     offs, _ = _device_offsets(psz + gsz, dev)          # one copy: [pred_off | gt_off shifted by Pp]
-    Pp, Pg = sum(psz), sum(gsz)
-    pred_off = offs[: N + 1]
-    gt_off = offs[N:] - Pp
+    Pp = sum(psz)
+    r = metrics_flat(pred, gt, origin, offs[: N + 1], offs[N:] - Pp, max(psz + gsz), pc_range, rays)
+    return dict(r, pred_sizes=psz, gt_sizes=gsz)
+
+
+def metrics_flat(pred, gt, origin, pred_off, gt_off, max_len, pc_range=DEFAULT_PC_RANGE, rays=False):
+    """metrics_device once the clouds are flat: pred [Pp, 3], gt [Pg, 3], origin [N, 3] (float32, contiguous, CUDA),
+    pred_off / gt_off [N + 1] int64 on the device (cloud n at rows [off[n], off[n+1]), the clouds tiling [0, Pp) and
+    [0, Pg)), max_len a host bound of every cloud's size (a cloud of masked points only may be longer).  Four library
+    calls, no host sync; returns the dict of metrics_device without the sizes."""
+    N = int(origin.shape[0])
+    dev = pred.device
+    Pp, Pg = int(pred.shape[0]), int(gt.shape[0])
     Pq = Pp + 2 * Pg
     qbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
     cbuf = torch.empty((Pg + 2 * Pp, 3), dtype=torch.float32, device=dev)
@@ -76,7 +87,6 @@ def metrics_device(preds, gts, origins, pc_range=DEFAULT_PC_RANGE, rays=False):
     dists = torch.empty(Pq, dtype=torch.float32, device=dev)
     idx = torch.empty(Pq, dtype=torch.int64, device=dev)
     scratch = torch.empty(Pq, dtype=torch.int64, device=dev)
-    max_len = max(psz + gsz)
     nbx = (max_len + 255) // 256
     partials = torch.empty(max(3 * N * nbx * 4, 1), dtype=torch.float64, device=dev)
     out = torch.empty((N, FIELDS), dtype=torch.float64, device=dev)
@@ -94,7 +104,7 @@ def metrics_device(preds, gts, origins, pc_range=DEFAULT_PC_RANGE, rays=False):
         _lib.check(L.vidar_eval_metrics(P(pred), P(gt), P(origin), P(pred_off), P(gt_off), P(seg_off[0]),
                                         P(q_mask), P(dists), P(idx), P(partials), P(out), P(ray_buf), N, max_len,
                                         st))
-    return dict(out=out, idx=idx, dists=dists, q_mask=q_mask, rays=ray_buf, pred_sizes=psz, gt_sizes=gsz)
+    return dict(out=out, idx=idx, dists=dists, q_mask=q_mask, rays=ray_buf)
 
 
 def raise_for_flags(flags, where):

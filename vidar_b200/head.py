@@ -11,6 +11,7 @@ arguments, returned keys and arithmetic
   get_point_cloud_prediction       :662-752   arg-max decode -> predicted / GT point clouds
   get_rendered_pcds                :344-389
   _custom_gumbel_softmax_distance  :754-773
+  evaluate / evaluate_device       detectors/vidar.py:439-497 (forward_test's decode + metric loop), batched
 
 What runs where: the CE term never materialises the [levels, rays, 513] logits
 (`ray_head.ce_regularization_loss`, one fused kernel per frame set); the dense term's gumbel decode
@@ -21,6 +22,8 @@ squared NN distance each way).  With CE + dense (use_dist_loss=False) `loss` run
 a host sync.  `ViDARRayHeadV1` is the same for ViDARHeadV1 (vidar_head_v1.py): every head frame's GT
 alignment and loss in one batched pass.  The distance term samples through `ray_head.get_grid_features` (CUDA
 sampler) and then follows the reference's torch statements; decoding is `ray_head.decode_ray_depth`.
+`evaluate` decodes, renders and scores every (sample, frame) in one pass without a host sync before its final
+copy (`ray_head.ray_argmax` over every row, `ray_head.decode_clouds`, `evaluate.metrics_flat`).
 CUDA only, like everything else in this package.
 """
 import numpy as np
@@ -28,6 +31,7 @@ import torch
 import torch.nn.functional as F
 
 from . import bev_geometry, chamfer, ray_head
+from . import evaluate as eval_metrics
 
 
 def get_inside_mask(points, point_cloud_range):
@@ -242,6 +246,59 @@ class ViDARRayHead:
         pred_pcds = self.get_rendered_pcds(batched_origin_points, batched_gt_points, gt_tindex, gt_dist, pred_dist, tgt_pc_range)
         gt_pcds = self.get_rendered_pcds(batched_origin_points, batched_gt_points, gt_tindex, gt_dist, gt_dist, tgt_pc_range)
         return dict(pred_pcds=pred_pcds, gt_pcds=gt_pcds, origin=batched_origin_points)
+
+    # ------------------------------------------------------------------ evaluation (vidar.py:439-497)
+    def evaluate(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas=None,
+                 batched_origin_points=None):
+        """forward_test's decode and metric loop (vidar.py:439-497) in one batched device pass: the same arguments as
+        get_point_cloud_prediction -> the per-sample ret_dict {f"frame.{t + start_idx}": {count, chamfer_distance,
+        l1_error, absrel_error}}, equal to evaluate.frame_metrics(get_point_cloud_prediction(...)), with its
+        exceptions.  One host copy at the end."""
+        out, bs, F = self._evaluate_table(pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range,
+                                          img_metas, batched_origin_points)
+        return eval_metrics.frame_metrics_host(out, bs, F, start_idx)
+
+    def evaluate_device(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas=None,
+                        batched_origin_points=None):
+        """Device part of `evaluate`: the [bs * F, 8] float64 table of evaluate.frame_metrics_device (row b * F + t),
+        no host sync."""
+        return self._evaluate_table(pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas,
+                                    batched_origin_points)[0]
+
+    def _evaluate_table(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas,
+                        batched_origin_points):
+        """get_point_cloud_prediction without its per-(sample, frame) loops: every row of the batch is decoded by one
+        arg-max launch over the [bs * Fp] volumes, the clouds are built in place (ray_head.decode_clouds) and scored
+        as bs * F clouds plus the trailing segment of the rows in no cloud, whose table row is dropped."""
+        bev_preds = pred_dict["next_bev_preds"].float()
+        valid_frames = pred_dict["valid_frames"]
+        Fp, inter_num, bs, token_num, Z = bev_preds.shape
+        (origin_grids, origin, gt_grids, points, gt_tindex) = self._process_gt_points(
+            bev_preds, gt_points, batched_origin_points, valid_frames, start_idx, Fp, tgt_bev_h, tgt_bev_w, tgt_pc_range)
+        F = origin.shape[1]
+        if F < Fp:
+            raise RuntimeError("origin must hold one row per frame of sigma")
+        dev = bev_preds.device
+        M = gt_grids.shape[1]
+        sigma = self._sigma_volume(bev_preds[:, -1], bs, Fp, Z, tgt_bev_h, tgt_bev_w).view(bs * Fp, Z, tgt_bev_h,
+                                                                                            tgt_bev_w)
+        t = gt_tindex.float()
+        keep = (t >= 0) & (t < Fp) & (t == t.floor())       # the rows decode_ray_depth decodes
+        base = torch.arange(bs, dtype=torch.int32, device=dev)[:, None] * Fp
+        frame = torch.where(keep, t.clamp(0, Fp - 1).to(torch.int32) + base, -1).view(-1).contiguous()
+        rays = gt_grids.float().contiguous()
+        origin_vox = origin_grids.float().contiguous()
+        depth, _ = ray_head.ray_argmax(sigma, origin_vox[:, :Fp].reshape(bs * Fp, 3), rays.view(bs * M, 3), frame,
+                                       self.ray_grid_num, self.ray_grid_step)
+        scale = (tgt_pc_range[3] - tgt_pc_range[0]) / tgt_bev_w
+        origin = origin.float().contiguous()
+        pred, gt, off = ray_head.decode_clouds(depth.view(bs, M), rays, points.float().contiguous(),
+                                               torch.where(keep, t, -1.0).contiguous(), origin_vox, origin, scale,
+                                               self.eval_within_grid, tgt_pc_range)
+        N = bs * F
+        origins = torch.cat([origin.view(N, 3), origin.new_zeros(1, 3)])
+        out = eval_metrics.metrics_flat(pred, gt, origins, off, off, M, tgt_pc_range)["out"]
+        return out[:N], bs, F
 
 
 class ViDARRayHeadV1(ViDARRayHead):
@@ -499,3 +556,36 @@ class ViDARRayHeadV1(ViDARRayHead):
         return ViDARRayHead.get_point_cloud_prediction(self, cur, valid_gt_points, start_idx, tgt_bev_h, tgt_bev_w,
                                                        tgt_pc_range, img_metas=img_metas,
                                                        batched_origin_points=cur_origin_points)
+
+    # ------------------------------------------------------------------ evaluation
+    def evaluate(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas=None,
+                 batched_origin_points=None):
+        """ViDARRayHead.evaluate of the current head frame (`pred_history_frame_num`), equal to
+        evaluate.frame_metrics(get_point_cloud_prediction(...)); the GT alignment is one align_gt op."""
+        out, bs, F = self._evaluate_table(pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range,
+                                          img_metas, batched_origin_points)
+        return eval_metrics.frame_metrics_host(out, bs, F, start_idx)
+
+    def evaluate_device(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas=None,
+                        batched_origin_points=None):
+        """Device part of `evaluate`: [bs * F, 8] float64 (row b * F + t), no host sync."""
+        return self._evaluate_table(pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas,
+                                    batched_origin_points)[0]
+
+    def _evaluate_table(self, pred_dict, gt_points, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas,
+                        batched_origin_points):
+        """get_point_cloud_prediction's alignment (src == tgt frames) without the host row counts of
+        _get_reference_gt_points: every sample keeps its M aligned rows, padding rows with frame -1, which
+        _process_gt_points treats as rows of no frame."""
+        cur = dict(pred_dict)
+        cur["next_bev_preds"] = pred_dict["next_bev_preds"][:, :, self.pred_history_frame_num, ...].contiguous()
+        frames = np.array(pred_dict["valid_frames"]) + self.history_queue_length
+        dev = gt_points[0].device
+        mats = self._transforms(img_metas, frames, frames)
+        mats_d = ray_head._pinned_upload(mats.numpy(), np.float32, dev)
+        _, tindex, pts = ray_head.align_gt(self._pack_gt(gt_points, dev), mats_d, [list(frames)],
+                                           [0.0] * 3 + [1.0] * 3 + [0.0] * 3, with_points=True)
+        rows = [torch.cat([pts[b], tindex[b, :, None]], 1) for b in range(len(gt_points))]
+        origin = mats_d[:, :, 3, :3].permute(1, 0, 2).contiguous()
+        return ViDARRayHead._evaluate_table(self, cur, rows, start_idx, tgt_bev_h, tgt_bev_w, tgt_pc_range, img_metas,
+                                            origin)

@@ -424,11 +424,11 @@ class SyntheticViDAR(nn.Module):
             preds.append(p.permute(0, 4, 1, 2, 3).contiguous())
         return torch.stack(preds, 1)
 
-    # ---- one training forward (vidar.py:239-387) -> dict of losses ----
-    def forward_train(self, img, lidar2img, gt_points, can_bus=None):
-        """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
-        (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
-        frame index 0 = current .. future_frames)."""
+    # ---- history BEV, current BEV, future roll-outs, head (vidar.py:239-387 and :392-437) ----
+    def _next_bev_preds(self, img, lidar2img, can_bus, future_frames):
+        """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + future_frames, inter, pred_frame, bs, Q, 16]: the history
+        BEV of the first T - 1 frames (no grad), the current frame's BEV as ref_bev, `future_frames` roll-outs with a
+        queue of length 1, then the head."""
         bs, T = img.shape[:2]
         dev = img.device
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
@@ -447,13 +447,20 @@ class SyntheticViDAR(nn.Module):
         inter_num = len(self.bev_pred_head)
         next_bev_feats = [ref_bev.unsqueeze(0).repeat(inter_num, 1, 1, 1)]
         prev_bev_input = ref_bev.unsqueeze(1)
-        for _ in range(self.future_frames):
+        for _ in range(future_frames):
             pred_feat, last = self.decode_future(prev_bev_input, can_bus)
             next_bev_feats.append(pred_feat)
             prev_bev_input = last.unsqueeze(1)                                         # queue length 1 (vidar.py:359-360)
         self._mark("future_decoder")
         next_bev_feats = torch.stack(next_bev_feats, 0)
-        next_bev_preds = self.forward_head(next_bev_feats)                              # [F, inter, pred_frame, bs, Q, 16]
+        return self.forward_head(next_bev_feats)                                        # [F, inter, pred_frame, bs, Q, 16]
+
+    # ---- one training forward (vidar.py:239-387) -> dict of losses ----
+    def forward_train(self, img, lidar2img, gt_points, can_bus=None):
+        """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
+        (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
+        frame index 0 = current .. future_frames)."""
+        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames)
         valid_frames = list(range(1 + self.future_frames))
         losses = {}
         for i in range(self.pred_frame_num):                                            # vidar_head_v1.py:179-218
@@ -465,6 +472,27 @@ class SyntheticViDAR(nn.Module):
                 losses[f"frame.{i}.{k}"] = v
         self._mark("head+loss")
         return losses
+
+    # ---- inference (vidar.py:389-502) ----
+    @torch.no_grad()
+    def predict_future(self, img, lidar2img, future_frames, can_bus=None):
+        """forward_test's prediction (vidar.py:392-437): the same inputs as forward_train, `future_frames` roll-outs
+        (the reference's test_future_frame_num) -> pred_dict {next_bev_preds [1 + future_frames, inter, pred_frame,
+        bs, Q, 16], valid_frames [0 .. future_frames]}."""
+        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames)
+        return dict(next_bev_preds=next_bev_preds, valid_frames=list(range(1 + future_frames)))
+
+    def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None):
+        """vidar.py:389-502 without submission writing and visualisation -> [ret_dict], ret_dict =
+        {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}} for the current frame (t = 0) and every
+        future frame, scored on the current head frame (`history_frames`) by ray_head.evaluate (one batched device
+        pass).  gt_points as forward_train's, frames 0 .. future_frames; the origin is zero in every frame.  Under a
+        process group every rank computes the same result."""
+        pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus)
+        cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.history_frames])
+        with torch.no_grad():
+            ret = self.ray_head.evaluate(cur, gt_points, 0, self.bev_h, self.bev_w, PC_RANGE)
+        return [ret]
 
 
 # ------------------------------------------------------------------------------------------------

@@ -17,7 +17,10 @@ projects/mmdet3d_plugin/bevformer/dense_heads/vidar_head_base.py:
   dense_chamfer_group_loss(...) == the same Chamfer term over a pair table, one loss per group
                                  (ViDARHeadV1: a group per head frame);
   align_gt(...)               == ViDARHeadV1._get_reference_gt_points (vidar_head_v1.py:94-148) for every
-                                 (head frame, target frame) job in one op.
+                                 (head frame, target frame) job in one op;
+  decode_clouds(...)          == get_point_cloud_prediction's rendering of the decoded rays (:698-745,
+                                 get_rendered_pcds :363-389) for every (sample, frame) at once, as flat
+                                 clouds with device offsets (csrc/eval_metrics.cu), no host sync.
 
 Low-level autograd ops: `ray_sample` (logits/lengths, differentiable w.r.t. sigma) and `ray_ce`.
 All tensors must be CUDA; there is no PyTorch fallback.
@@ -485,3 +488,36 @@ def align_gt(gt, mats, jobs, voxel, with_points=False):
     _call(_lib.lib().vidar_head_align_gt, dev, _lib.ptr(gt), _lib.ptr(mats), C.cast(j, C.c_void_p),
           C.cast(vx, C.c_void_p), _lib.ptr(rays), _lib.ptr(tindex), _lib.ptr(points), bs, M, Cg, H, V)
     return rays, tindex, points
+
+
+def decode_clouds(depth, rays, points, tindex, origin_vox, origin, scale, within_grid=False, pc_range=None):
+    """The pred and gt clouds of every (sample, frame) from the decoded rays, csrc/eval_metrics.cu.
+
+    depth [bs, M] arg-max depth (voxel units), rays [bs, M, 3] GT points in voxel units and points [bs, M, 3] in metres,
+    tindex [bs, M] float frame (-1 or outside [0, F) = in no cloud), origin_vox / origin [bs, F, 3] voxel units /
+    metres, all float32 on one CUDA device; scale = (pc_range[3] - pc_range[0]) / bev_w; pc_range: metres, used by
+    within_grid like get_rendered_pcds.  Returns pred, gt [bs * M, 3] and off [bs * F + 2] int64: cloud n = b * F + t
+    at rows [off[n], off[n+1]), then one segment of every other row (NaN points, masked by the metrics)."""
+    if rays.dim() != 3 or rays.shape[2] != 3:
+        raise RuntimeError(f"rays must be [bs, M, 3], got {tuple(rays.shape)}")
+    bs, M = rays.shape[:2]
+    F = origin.shape[1] if origin.dim() == 3 else -1
+    if (tuple(depth.shape) != (bs, M) or tuple(points.shape) != (bs, M, 3) or tuple(tindex.shape) != (bs, M)
+            or tuple(origin.shape) != (bs, F, 3) or tuple(origin_vox.shape) != (bs, F, 3)):
+        raise RuntimeError("expected depth [bs, M], points [bs, M, 3], tindex [bs, M], origin / origin_vox [bs, F, 3]")
+    for name, t in (("depth", depth), ("rays", rays), ("points", points), ("tindex", tindex),
+                    ("origin_vox", origin_vox), ("origin", origin)):
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must be float32")
+    if within_grid and pc_range is None:
+        raise RuntimeError("eval_within_grid needs pc_range")
+    _lib.require_cuda(depth=depth, rays=rays, points=points, tindex=tindex, origin_vox=origin_vox, origin=origin)
+    dev = rays.device
+    pred = torch.empty((bs * M, 3), dtype=torch.float32, device=dev)
+    gt = torch.empty((bs * M, 3), dtype=torch.float32, device=dev)
+    off = torch.empty(bs * F + 2, dtype=torch.int64, device=dev)
+    rng = (C.c_float * 6)(*[float(v) for v in (pc_range if pc_range is not None else [0.0] * 6)])
+    P = _lib.ptr
+    _call(_lib.lib().vidar_eval_decode_clouds, dev, P(depth), P(rays), P(points), P(tindex), P(origin_vox), P(origin),
+          C.cast(rng, C.c_void_p), float(scale), int(bool(within_grid)), P(pred), P(gt), P(off), bs, M, F)
+    return pred, gt, off
