@@ -543,6 +543,31 @@ int vidar_head_align_gt(const float* gt, const float* mats, const int32_t* jobs_
                         float* rays, float* tindex, float* points, int bs, int M, int Cg, int H, int V,
                         void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (vii) Modulated deformable convolution (DCNv2): mmcv's modulated_deform_conv2d, the deformable 3x3 convs of the
+ *   image backbone (ResNet-101 dcn=dict(type='DCNv2', ...), stage_with_dcn=(False, False, True, True)), groups = 1,
+ *   deform_groups = 1.  The host runs the contraction as a GEMM over an explicit column matrix.
+ *   x       [N, H, W, C]        input, channel-last
+ *   offset  [N, 2*kh*kw, Ho, Wo] (dy, dx) of kernel point k = i*kw + j at channels 2k, 2k+1
+ *   mask    [N, kh*kw, Ho, Wo]  modulation (after the sigmoid)
+ *   Ho, Wo must equal the convolution's output size for the stride (sh, sw), padding (ph, pw), dilation (dh, dw).
+ *   A call covers the images [n0, n0 + nb); column row m = (n - n0) * Ho * Wo + ho * Wo + wo.
+ * Sample of (n, ho, wo, k): h = ho*sh - ph + i*dh + dy, w = wo*sw - pw + j*dw + dx; v_c = bilinear value of x[n, :, :, c]
+ * on the floor cell, 0 when h <= -1, h >= H, w <= -1 or w >= W, corners outside the image add 0.
+ *   cols [nb*Ho*Wo, kh*kw*C]  fully overwritten: mask * v_c at k*C + c (so y = cols @ weight.permute(0,2,3,1)^T) */
+int vidar_dcn_im2col(const float* x, const float* offset, const float* mask, float* cols, int N, int C, int H, int W,
+                     int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int n0, int nb,
+                     void* stream);
+/* Backward of the sampling, from grad_cols [nb*Ho*Wo, kh*kw*C] (the gradient of cols):
+ *   grad_x      [N, H, W, C]         caller-zeroed, accumulated (mask * corner weight * grad_col)
+ *   grad_offset [N, 2*kh*kw, Ho, Wo] written for images [n0, n0 + nb): mask * sum_c grad_col * d v_c / d(h, w)
+ *   grad_mask   [N, kh*kw, Ho, Wo]   written for images [n0, n0 + nb): sum_c grad_col * v_c
+ * d v / d(h, w) is the derivative of the bilinear form on the floor cell (one-sided on integer lines, 0 outside the
+ * open range).  Both calls take 16-byte vector paths when C % 4 == 0 and the buffers are 16-byte aligned. */
+int vidar_dcn_col2im(const float* x, const float* offset, const float* mask, const float* grad_cols, float* grad_x,
+                     float* grad_offset, float* grad_mask, int N, int C, int H, int W, int Ho, int Wo, int kh, int kw,
+                     int sh, int sw, int ph, int pw, int dh, int dw, int n0, int nb, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

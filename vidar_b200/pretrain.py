@@ -3,9 +3,10 @@ hot-path modules of this package, with the intra-sample sharding of SURVEY.md 8e
 
 This is a HARNESS, not a port of the detector: it composes the reference's step
 (projects/mmdet3d_plugin/bevformer/detectors/vidar.py:239-387) from
-  * a random-init torchvision ResNet-101 (strides 8/16/32; stage 1 frozen, BN in eval mode as in
-    vidar_1_8_nusc_3future.py:88-95 -- the reference's DCN in stages 3-4 is out of scope, plain convs) and
-    a 4-level FPN (cfg :96-106);
+  * a random-init ResNet-101 (strides 8/16/32; stage 1 frozen, BN in eval mode as in
+    vidar_1_8_nusc_3future.py:88-95).  `dcn=True` (`build(device, dcn=True)`) is the reference's caffe-style backbone
+    with a DCNv2 (vidar_b200/dcn.py) as conv2 of every block in stages 3-4; the default dcn=False runs torchvision's
+    plain convolutions there.  Then a 4-level FPN (cfg :96-106);
   * the BEV encoder: 6 x [TemporalSelfAttention, LN, SpatialCrossAttention, LN, (LatentRendering in
     layer 2), FFN 256-512-256, LN]  (modules/encoder.py:159-253, encoder_v2.py:52-209, cfg :141-190);
   * the future decoder: 3 x [PredictionMSDeformableAttention (self), LN, PredictionMSDeformableAttention
@@ -49,12 +50,27 @@ EMBED, BEV_H, BEV_W, HEIGHTS = 256, 200, 200, 16
 # image side
 # ------------------------------------------------------------------------------------------------
 class ImageBackbone(nn.Module):
-    """ResNet-101 C3..C5 (strides 8, 16, 32).  frozen_stages=1 and norm_eval=True (cfg :92-94)."""
+    """ResNet-101 C3..C5 (strides 8, 16, 32).  frozen_stages=1 and norm_eval=True (cfg :92-94).
 
-    def __init__(self):
+    dcn=True is the reference's backbone (cfg :88-95): style='caffe' -- the stride of the first block of layer2..4 sits
+    on its 1x1 conv1, not on the 3x3 conv2 -- and conv2 of every block of layer3 and layer4 (23 + 3 = 26 layers) is a
+    DCNv2, `vidar_b200.dcn.ModulatedDeformConv2dPack(planes, planes, 3, padding=1, bias=False)` (stage_with_dcn=(False,
+    False, True, True), fallback_on_stride=False).  dcn=False keeps torchvision's pytorch-style plain convolutions."""
+
+    def __init__(self, dcn=False):
         super().__init__()
         import torchvision
         r = torchvision.models.resnet101(weights=None)
+        if dcn:
+            from .dcn import ModulatedDeformConv2dPack
+            for li, layer in enumerate((r.layer2, r.layer3, r.layer4)):
+                first = layer[0]
+                first.conv1.stride, first.conv2.stride = (2, 2), (1, 1)
+                if li > 0:
+                    for blk in layer:
+                        width = blk.conv2.in_channels
+                        blk.conv2 = ModulatedDeformConv2dPack(width, width, 3, stride=1, padding=1, bias=False)
+        self.dcn = dcn
         self.stem = nn.Sequential(r.conv1, r.bn1, r.relu, r.maxpool)
         self.layer1, self.layer2, self.layer3, self.layer4 = r.layer1, r.layer2, r.layer3, r.layer4
         for m in (self.stem, self.layer1):
@@ -257,12 +273,12 @@ class SyntheticViDAR(nn.Module):
     """The pre-training graph of ViDAR-RN101 (3 history frames, 3 future frames, 5 predicted head frames)."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
-                 latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512):
+                 latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False):
         super().__init__()
         self.num_cams, self.future_frames, self.history_frames = num_cams, future_frames, history_frames
         self.bev_h, self.bev_w = bev_hw
         BEV_H, BEV_W = bev_hw          # noqa: N806  (shadows the module defaults below)
-        self.backbone, self.neck = ImageBackbone(), FPN()
+        self.backbone, self.neck = ImageBackbone(dcn=dcn), FPN()
         self.bev_embedding = nn.Embedding(BEV_H * BEV_W, EMBED)
         self.positional_encoding = LearnedPositionalEncoding(BEV_H, BEV_W)
         self.cams_embeds = nn.Parameter(torch.randn(num_cams, EMBED) * 0.02)

@@ -71,9 +71,29 @@ TRANSFORMER_LAYER = Registry("transformerLayer")
 TRANSFORMER_LAYER_SEQUENCE = Registry("transformer-layers sequence")
 
 
+CONV_LAYERS = Registry("conv layer")
+CONV_LAYERS.register_module("Conv2d", module=nn.Conv2d)
+CONV_LAYERS.register_module("Conv", module=nn.Conv2d)
+
+
 def build_attention(cfg, default_args=None):
     """mmcv.cnn.bricks.transformer.build_attention."""
     return build_from_cfg(cfg, ATTENTION, default_args)
+
+
+def build_conv_layer(cfg, *args, **kwargs):
+    """mmcv.cnn.build_conv_layer: `cfg` None means Conv2d; otherwise CONV_LAYERS[cfg['type']](*args, **kwargs, **rest of
+    cfg), e.g. mmdet's ResNet `build_conv_layer(dict(type='DCNv2', deform_groups=1), planes, planes, kernel_size=3,
+    stride=1, padding=1, dilation=1, bias=False)`."""
+    from . import dcn  # noqa: F401  (registers DCNv2)
+    cfg_ = dict(type="Conv2d") if cfg is None else copy.deepcopy(cfg)
+    if not isinstance(cfg_, dict) or "type" not in cfg_:
+        raise TypeError(f"cfg must be a dict with the key \"type\", but got {cfg}")
+    layer_type = cfg_.pop("type")
+    cls = CONV_LAYERS.get(layer_type)
+    if cls is None:
+        raise KeyError(f"Unrecognized conv type {layer_type}")
+    return cls(*args, **kwargs, **cfg_)
 
 
 class BaseModule(nn.Module):
@@ -108,11 +128,18 @@ def xavier_init(module, gain=1, bias=0, distribution="normal"):
 
 def register_into_mmcv():
     """If mmcv is installed, expose this package's modules under the reference's names in
-    mmcv's own ATTENTION registry (force=True replaces the plugin's classes)."""
+    mmcv's own ATTENTION registry (force=True replaces the plugin's classes), and its
+    deformable convolution as `DCNv2` in mmcv's CONV_LAYERS (what mmdet's ResNet builds for
+    `dcn=dict(type='DCNv2', ...)`)."""
     try:
         from mmcv.cnn.bricks.registry import ATTENTION as MMCV_ATTENTION
+        from mmcv.cnn.bricks.registry import CONV_LAYERS as MMCV_CONV_LAYERS
     except Exception:
         return False
+    from . import dcn  # noqa: F401  (registers DCNv2)
     for name, cls in ATTENTION.module_dict.items():
         MMCV_ATTENTION.register_module(name=name, force=True, module=cls)
+    for name, cls in CONV_LAYERS.module_dict.items():
+        if cls.__module__.startswith(__package__ + "."):           # this package's ops only, not torch's Conv2d
+            MMCV_CONV_LAYERS.register_module(name=name, force=True, module=cls)
     return True
