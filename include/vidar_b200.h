@@ -478,44 +478,28 @@ int vidar_eval_decode_clouds(const float* depth, const float* rays, const float*
 
 /* ------------------------------------------------------------------------------------
  * (v) The head's dense loss term 'loss.dense_voxel' (dense_heads/vidar_head_base.py:594-659, get_rendered_pcds
- *   :344-389): Chamfer distance between the decoded dense rays and the GT cloud of every (sample, frame) pair,
- *   S = bs * F pairs, n = b * F + f, in a fixed number of launches and without a host sync.
- *   dist      [bs, F*R0]     decoded ray lengths, frame-major: rays f*R0 .. (f+1)*R0-1 belong to frame f
- *   points    [bs, F*R0, 3]  ray end points (voxel units);  origin [bs, To, 3], To >= F (voxel units)
- *   gt        [bs, M, 3], gt_tindex [bs, M] (float frame, -1 = padding, any order; NULL when M = 0)
- *   weights_host [F] per-frame loss weights, weight_sum = sum of all loss weights (HOST); loss divides by
- *   weight_sum * bs.  pc_range_host: 6 floats (HOST), used when within_grid (the reference's
- *   get_inside_mask on the voxel-unit end points).  W, H, Z: the grid size (gt box 0 < x < W-1, ...).
- *   Pred cloud of n: rays with dist > 0, point (o + unit(p - o) * dist - o) * 0.1; gt cloud of n: rows with
- *   gt_tindex == f strictly inside the box, (g - o) * 0.1, in row order (it decides NN ties).
- * Forward outputs (Pq = bs*F*R0 + bs*M; all but loss are also inputs of the backward):
- *   qbuf, cbuf [Pq, 3]; q_mask, c_mask [Pq]; q_off, c_off [2S+1] int64; idx [Pq] int64: the search layout
- *   (segments 0..S-1 pred -> gt, S..2S-1 gt -> pred) and each query's nearest neighbour
- *   pairs [S, 4] fp64: sum pred->gt squared distances, pred points, sum gt->pred, gt points
- *   loss [1]: sum_n w_f * (mean pred->gt + mean gt->pred) / 2 / (weight_sum * bs) over pairs with gt points;
- *   NaN when a pair has gt points but no pred point.  Fixed-order fp64 sums: the same bits on every call.
- * Scratch from the library's memory pool.  Backward: grad_dist [bs, F*R0] fully overwritten (0 for rays
- * outside the pred cloud), grad_loss [1] the upstream gradient (device). */
-int vidar_dense_chamfer_forward(const float* dist, const float* points, const float* origin, const float* gt,
-                                const float* gt_tindex, const float* weights_host, const float* pc_range_host,
-                                float weight_sum, float* qbuf, float* cbuf, unsigned char* q_mask,
-                                unsigned char* c_mask, int64_t* q_off, int64_t* c_off, int64_t* idx, double* pairs,
-                                float* loss, int bs, int F, int R0, int To, int M, int W, int H, int Z,
-                                int within_grid, void* stream);
-int vidar_dense_chamfer_backward(const float* points, const float* origin, const float* qbuf, const float* cbuf,
-                                 const unsigned char* q_mask, const int64_t* q_off, const int64_t* c_off,
-                                 const int64_t* idx, const double* pairs, const float* weights_host,
-                                 float weight_sum, const float* grad_loss, float* grad_dist, int bs, int F, int R0,
-                                 int To, int M, void* stream);
-
-/* The same Chamfer term over a pair table, one loss per group (ViDARHeadV1: a group per head frame):
- *   dist [P*R0], points [P*R0, 3]  rays of pair n at n*R0 .. (n+1)*R0-1;  origin [No, 3]
- *   gt [Sg, M, 3], gt_tindex [Sg, M]  Sg gt samples, frames 0..Fg-1 (float, -1 = padding, any order)
+ *   :344-389): Chamfer distance between the decoded dense rays and the GT cloud of P (gt sample, frame) pairs
+ *   named by a pair table, one loss per group, in a fixed number of launches and without a host sync.
+ *   ViDARRayHead: P = bs*F pairs n = b*F + f, Sg = bs, Fg = F, one group; ViDARHeadV1: a group per head frame.
+ *   dist [P*R0], points [P*R0, 3]  decoded ray lengths and ray end points (voxel units), rays of pair n at
+ *                                  n*R0 .. (n+1)*R0-1;  origin [No, 3] (voxel units)
+ *   gt [Sg, M, 3], gt_tindex [Sg, M]  Sg gt samples, float frame 0..Fg-1, -1 = padding, any order; NULL when M = 0
  *   slot_pair [Sg*Fg] int32 (device): the pair of each (gt sample, frame) slot, -1 = none
  *   pair_table [P, 3] int32 (device): slot, origin row, group; pairs in increasing slot order
- *   pair_weight [P], group_norm [groups] (device): loss[g] = sum_{n in g} w_n * (...) / group_norm[g]
- *   q_off, c_off [2P+1]; pairs [P, 4]; loss [groups]; grad_loss [groups] (device).
- * vidar_dense_chamfer_forward / _backward are the case P = bs*F, Sg = bs, Fg = F, one group. */
+ *   pair_weight [P], group_norm [groups] (device)
+ *   pc_range_host: 6 floats (HOST), used when within_grid (the reference's get_inside_mask on the voxel-unit end
+ *   points).  W, H, Z: the grid size (gt box 0 < x < W-1, ...).
+ *   Pred cloud of n: rays with dist > 0, point (o + unit(p - o) * dist - o) * 0.1 with o its origin row; gt cloud
+ *   of n: rows of its slot's frame strictly inside the box, (g - o) * 0.1, in row order (it decides NN ties).
+ * Forward outputs (Pq = P*R0 + Sg*M; all but loss are also inputs of the backward):
+ *   qbuf, cbuf [Pq, 3]; q_mask, c_mask [Pq]; q_off, c_off [2P+1] int64; idx [Pq] int64: the search layout
+ *   (segments 0..P-1 pred -> gt, P..2P-1 gt -> pred) and each query's nearest neighbour
+ *   pairs [P, 4] fp64: sum pred->gt squared distances, pred points, sum gt->pred, gt points
+ *   loss [groups]: loss[g] = sum_{n in g} w_n * (mean pred->gt + mean gt->pred) / 2 / group_norm[g] over pairs
+ *   with gt points; NaN when a pair has gt points but no pred point.  Fixed-order fp64 sums: the same bits on
+ *   every call.
+ * Scratch from the library's memory pool.  Backward: grad_dist [P*R0] fully overwritten (0 for rays outside the
+ * pred cloud), grad_loss [groups] the upstream gradient (device). */
 int vidar_dense_chamfer_groups_forward(const float* dist, const float* points, const float* origin, const float* gt,
                                        const float* gt_tindex, const int32_t* slot_pair, const int32_t* pair_table,
                                        const float* pair_weight, const float* group_norm, const float* pc_range_host,

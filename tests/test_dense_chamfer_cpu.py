@@ -1,6 +1,5 @@
 """The head's dense Chamfer term without a GPU: the fp64 oracle against goldens made by the reference's own
-ViDARHeadBase.loss (tools/make_golden_dense_chamfer.py), and argument validation of the C entry points."""
-import ctypes
+ViDARHeadBase.loss (tools/make_golden_dense_chamfer.py), and argument validation of ray_head.dense_chamfer_loss."""
 import os
 
 import numpy as np
@@ -54,33 +53,28 @@ def test_cases_cover_what_they_are_named_for():
     assert len(np.unique(u.round(12), axis=0)) < live.sum()
 
 
-def test_entry_points_reject_bad_arguments():
-    """Sizes and pointers are checked before anything touches the device (a GPU-less host can run this)."""
-    from vidar_b200 import _lib
-    L = _lib.lib()
-    N, X = None, ctypes.c_void_p(0x1000)
-    w = ctypes.cast((ctypes.c_float * 4)(1, 1, 1, 1), ctypes.c_void_p)
-    rng = ctypes.cast((ctypes.c_float * 6)(0, 0, 0, 1, 1, 1), ctypes.c_void_p)
+def test_dense_chamfer_loss_rejects_bad_arguments():
+    """dense_chamfer_loss's own checks fire before anything touches the device (a GPU-less host can run this)."""
+    import torch
 
-    def fwd(bs=1, F=2, R0=40, To=2, M=100, W=16, H=16, Z=8, ptr=X, gt=X, weights=w, pc=rng):
-        return L.vidar_dense_chamfer_forward(ptr, X, X, gt, gt, weights, pc, 2.0, X, X, X, X, X, X, X, X, X, bs, F,
-                                             R0, To, M, W, H, Z, 0, N)
-
-    def bwd(bs=1, F=2, R0=40, To=2, M=100, ptr=X, weights=w):
-        return L.vidar_dense_chamfer_backward(X, X, X, X, X, X, X, X, X, weights, 2.0, X, ptr, bs, F, R0, To, M, N)
-
+    from vidar_b200 import ray_head
+    bs, F, R0, M = 2, 3, 4, 6
+    base = dict(dist=torch.zeros(bs, F * R0), points=torch.zeros(bs, F * R0, 3), origin=torch.zeros(bs, F, 3),
+                gt=torch.zeros(bs, M, 3), gt_tindex=torch.zeros(bs, M), grid=(8, 8, 4), frame_weights=[1.0] * F,
+                weight_sum=float(F))
     cases = [
-        (fwd, dict(bs=0), b"bad sizes"), (fwd, dict(F=0), b"bad sizes"), (fwd, dict(F=65), b"bad sizes"),
-        (fwd, dict(R0=0), b"bad sizes"), (fwd, dict(To=1), b"bad sizes"), (fwd, dict(M=-1), b"bad sizes"),
-        (fwd, dict(W=0), b"bad grid"), (fwd, dict(bs=20000), b"pairs"), (fwd, dict(R0=1 << 30), b"rows"),
-        (fwd, dict(ptr=N), b"null pointer"), (fwd, dict(gt=N), b"null gt"), (fwd, dict(weights=N), b"null loss weights"),
-        (fwd, dict(pc=N), b"null pc_range"),
-        (bwd, dict(F=0), b"bad sizes"), (bwd, dict(To=1), b"bad sizes"), (bwd, dict(ptr=N), b"null pointer"),
-        (bwd, dict(weights=N), b"null loss weights"),
+        (dict(dist=torch.zeros(bs, F * R0 + 1)), "dist must be"),
+        (dict(dist=torch.zeros(bs * F * R0)), "dist must be"),
+        (dict(frame_weights=[]), "dist must be"),
+        (dict(origin=torch.zeros(bs, F - 1, 3)), "origin"),
+        (dict(points=torch.zeros(bs, F * R0, 2)), "points"),
+        (dict(gt_tindex=torch.zeros(bs, M + 1)), "gt_tindex"),
+        (dict(gt=torch.zeros(bs, M, 3).double(), gt_tindex=torch.zeros(bs, M).double()), "gt must be float32"),
+        (dict(eval_within_grid=True), "pc_range"),
+        ({}, "CUDA"),
     ]
-    for fn, kw, needle in cases:
-        rc = fn(**kw)
-        assert rc == 1, (kw, rc, L.vidar_last_error())
-        assert needle in L.vidar_last_error(), (kw, L.vidar_last_error())
-    # no gt rows is a valid size (every pair is then skipped); it fails only on the null output pointer here
-    assert fwd(M=0, gt=N, ptr=N) == 1 and b"null pointer" in L.vidar_last_error()
+    for kw, needle in cases:
+        args = dict(base)
+        args.update(kw)
+        with pytest.raises(RuntimeError, match=needle):
+            ray_head.dense_chamfer_loss(**args)

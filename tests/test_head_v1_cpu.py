@@ -73,8 +73,8 @@ def test_c_entry_points_reject_bad_arguments():
     def align(bs=1, M=100, Cg=5, H=2, V=4, ptr=X, jobs=jobs, vox=vox):
         return L.vidar_head_align_gt(X, X, jobs, vox, ptr, X, N, bs, M, Cg, H, V, N)
 
-    def fwd(P=4, groups=2, R0=40, Sg=2, Fg=2, M=100, W=16, ptr=X, pc=rng):
-        return L.vidar_dense_chamfer_groups_forward(ptr, X, X, X, X, X, X, X, X, pc, X, X, X, X, X, X, X, X, X, P,
+    def fwd(P=4, groups=2, R0=40, Sg=2, Fg=2, M=100, W=16, ptr=X, gt=X, pc=rng):
+        return L.vidar_dense_chamfer_groups_forward(ptr, X, X, gt, gt, X, X, X, X, pc, X, X, X, X, X, X, X, X, X, P,
                                                     groups, R0, Sg, Fg, M, W, 16, 8, 0, N)
 
     def bwd(P=4, groups=2, R0=40, Sg=2, Fg=2, M=100, ptr=X):
@@ -88,10 +88,13 @@ def test_c_entry_points_reject_bad_arguments():
         (align, dict(vox=N), b"null host table"), (align, dict(ptr=N), b"null pointer"),
         (fwd, dict(P=0), b"bad sizes"), (fwd, dict(groups=0), b"bad sizes"), (fwd, dict(Fg=65), b"bad sizes"),
         (fwd, dict(P=40000), b"pairs"), (fwd, dict(R0=1 << 30), b"rows"), (fwd, dict(W=0), b"bad grid"),
-        (fwd, dict(pc=N), b"null pc_range"), (fwd, dict(ptr=N), b"null pointer"),
+        (fwd, dict(R0=0), b"bad sizes"), (fwd, dict(M=-1), b"bad sizes"), (fwd, dict(pc=N), b"null pc_range"),
+        (fwd, dict(ptr=N), b"null pointer"), (fwd, dict(gt=N), b"null gt buffer"),
         (bwd, dict(Sg=0), b"bad sizes"), (bwd, dict(ptr=N), b"null pointer"),
     ]
     for fn, kw, needle in cases:
         rc = fn(**kw)
         assert rc == 1, (kw, rc, L.vidar_last_error())
         assert needle in L.vidar_last_error(), (kw, L.vidar_last_error())
+    # no gt rows is a valid size (every pair is then skipped); it fails only on the null output pointer here
+    assert fwd(M=0, gt=N, ptr=N) == 1 and b"null pointer" in L.vidar_last_error()

@@ -10,9 +10,8 @@
 //   gt   = {(g - o) * 0.1 : rows of the pair's (gt sample, frame) slot, 0 < x < W-1, 0 < y < H-1, 0 < z < Z-1}
 //   loss[group] = sum_{n in group} w_n * (mean_pred min_gt |.|^2 + mean_gt min_pred |.|^2) / 2 / norm[group],
 //          pairs without gt skipped; gt but no pred gives NaN like the per-pair path.
-// vidar_dense_chamfer_*: the single-group case, pair n = b * F + f, origin [bs, To] row (b, f), w_n = w_f,
-// norm = sum(loss_weight) * bs.  vidar_dense_chamfer_groups_*: a device pair table (ViDARHeadV1: one group per head
-// frame, pairs of zero weight left out).
+// Pairs come from a device pair table.  ViDARRayHead: pair n = b * F + f, one group, norm = sum(loss_weight) * bs;
+// ViDARHeadV1: one group per head frame, pairs of zero weight left out.
 // fp32 statements in the reference's order with explicit _rn intrinsics (no FMA contraction).
 //
 // Layout (P pairs; Pp = P * R0 dense rays; G = gt points kept; Pq = Pp + Sg * M buffer rows):
@@ -46,21 +45,8 @@ struct DenseDims {
   float pc[6];
 };
 
-// pair n = b * F + f of a [bs, F] batch, one group
-struct FramePairs {
-  int F, To;
-  float w[kMaxFrames];                // per-frame loss weight
-  float norm;                         // sum(loss_weight) * bs
-  __device__ int slot_pair(int slot) const { return slot; }
-  __device__ int slot(int n) const { return n; }
-  __device__ int origin_row(int n) const { return (n / F) * To + n % F; }
-  __device__ float weight(int n) const { return w[n % F]; }
-  __device__ int group(int) const { return 0; }
-  __device__ float norm_of(int) const { return norm; }
-};
-
-// a device pair table, pairs in increasing slot order
-struct TablePairs {
+// the device pair table, pairs in increasing slot order
+struct PairTable {
   const int32_t* slots;               // [Sg * Fg] pair of each (gt sample, frame) slot, -1 = none
   const int32_t* tab;                 // [P, 3] slot, origin row, group
   const float* w;                     // [P]
@@ -74,8 +60,7 @@ struct TablePairs {
 };
 
 // frame of gt row i of gt sample s, or -1 when the row belongs to no pair (padding, other frames, outside the box)
-template <class Pairs>
-__device__ __forceinline__ int gt_frame(const DenseDims& D, const Pairs& Pr, const float* __restrict__ gt,
+__device__ __forceinline__ int gt_frame(const DenseDims& D, const PairTable& Pr, const float* __restrict__ gt,
                                         const float* __restrict__ tindex, int s, int i) {
   const size_t k = (size_t)s * D.M + i;
   const float t = tindex[k];
@@ -96,9 +81,8 @@ __device__ __forceinline__ void ray_unit(const float* p, const float* o, float u
 
 // grid (Sg * nchunk + pred blocks).  gt chunks: per-(slot, chunk) counts of kept rows.  Pred blocks: the pred
 // points of every ray into qbuf (row k = ray k) and their query mask.
-template <class Pairs>
 __global__ void __launch_bounds__(kChunk)
-dense_count_kernel(DenseDims D, Pairs Pr, const float* __restrict__ dist, const float* __restrict__ points,
+dense_count_kernel(DenseDims D, PairTable Pr, const float* __restrict__ dist, const float* __restrict__ points,
                    const float* __restrict__ origin, const float* __restrict__ gt, const float* __restrict__ tindex,
                    int* __restrict__ counts, float* __restrict__ qbuf, unsigned char* __restrict__ q_mask) {
   extern __shared__ int hist[];       // [32][Fg]
@@ -127,8 +111,7 @@ dense_count_kernel(DenseDims D, Pairs Pr, const float* __restrict__ dist, const 
 
 // One block: chunk counts -> slot offsets soff[0..Sg*Fg] of the compacted gt rows, then the segment offsets of
 // both searches.  c_off[0..P] = gt pair offsets; c_off[P] = G.
-template <class Pairs>
-__global__ void dense_offsets_kernel(DenseDims D, Pairs Pr, int* __restrict__ counts, int64_t* __restrict__ soff,
+__global__ void dense_offsets_kernel(DenseDims D, PairTable Pr, int* __restrict__ counts, int64_t* __restrict__ soff,
                                      int64_t* __restrict__ q_off, int64_t* __restrict__ c_off) {
   const int S = D.Sg * D.Fg;
   sort_offsets(S, D.nchunk, counts, soff);
@@ -144,9 +127,8 @@ __global__ void dense_offsets_kernel(DenseDims D, Pairs Pr, int* __restrict__ co
 
 // grid as the count kernel.  gt chunks: stable scatter of the kept rows, scaled, into both buffers; rows of
 // qbuf past Pp + G are masked.  Pred blocks: the pred points into cbuf behind the gt rows.
-template <class Pairs>
 __global__ void __launch_bounds__(kChunk)
-dense_scatter_kernel(DenseDims D, Pairs Pr, const float* __restrict__ origin, const float* __restrict__ gt,
+dense_scatter_kernel(DenseDims D, PairTable Pr, const float* __restrict__ origin, const float* __restrict__ gt,
                      const float* __restrict__ tindex, const int* __restrict__ counts,
                      const int64_t* __restrict__ soff, float* __restrict__ qbuf, float* __restrict__ cbuf,
                      unsigned char* __restrict__ q_mask, unsigned char* __restrict__ c_mask) {
@@ -207,8 +189,7 @@ dense_partials_kernel(const int64_t* __restrict__ q_off, const unsigned char* __
 
 // One block: pairs [P, 4] = (sum pred->gt, pred count, sum gt->pred, gt count), then each group's loss, pairs in
 // order.
-template <class Pairs>
-__global__ void dense_finish_kernel(DenseDims D, Pairs Pr, const int64_t* __restrict__ q_off,
+__global__ void dense_finish_kernel(DenseDims D, PairTable Pr, const int64_t* __restrict__ q_off,
                                     const double* __restrict__ partials, double* __restrict__ pairs,
                                     float* __restrict__ loss, int nbx) {
   const int S = D.P;
@@ -241,9 +222,8 @@ __global__ void dense_finish_kernel(DenseDims D, Pairs Pr, const int64_t* __rest
 // pred = ((o + u * d) - o) * 0.1:  d/dd = 0.1 * u . d/dpred.
 //   pred query i (ray k):  c_n * 2 (p_i - g_nn)      c_n = grad_loss[group] * w_n / (2 norm) / (pred count)
 //   gt query j:            -c_n * 2 (g_j - p_nn)     c_n = grad_loss[group] * w_n / (2 norm) / (gt count), onto p_nn's ray
-template <class Pairs>
 __global__ void __launch_bounds__(kSumThreads)
-dense_backward_kernel(DenseDims D, Pairs Pr, const float* __restrict__ points, const float* __restrict__ origin,
+dense_backward_kernel(DenseDims D, PairTable Pr, const float* __restrict__ points, const float* __restrict__ origin,
                       const float* __restrict__ qbuf, const float* __restrict__ cbuf,
                       const unsigned char* __restrict__ q_mask, const int64_t* __restrict__ q_off,
                       const int64_t* __restrict__ c_off, const int64_t* __restrict__ idx,
@@ -291,18 +271,7 @@ int dense_dims(DenseDims& D, int P, int groups, int Sg, int Fg, int R0, int M, c
   return VIDAR_OK;
 }
 
-int frame_pairs(FramePairs& Pr, const float* weights_host, float weight_sum, int bs, int F, int To, const char* who) {
-  VIDAR_REQUIRE(To >= F, "%s: bad sizes To=%d F=%d", who, To, F);
-  VIDAR_REQUIRE(weights_host, "%s: null loss weights", who);
-  Pr = FramePairs{};
-  Pr.F = F; Pr.To = To;
-  for (int f = 0; f < F; ++f) Pr.w[f] = weights_host[f];
-  Pr.norm = weight_sum * (float)bs;
-  return VIDAR_OK;
-}
-
-template <class Pairs>
-int dense_forward(const DenseDims& D, const Pairs& Pr, const float* dist, const float* points, const float* origin,
+int dense_forward(const DenseDims& D, const PairTable& Pr, const float* dist, const float* points, const float* origin,
                   const float* gt, const float* gt_tindex, float* qbuf, float* cbuf, unsigned char* q_mask,
                   unsigned char* c_mask, int64_t* q_off, int64_t* c_off, int64_t* idx, double* pairs, float* loss,
                   void* stream, const char* who) {
@@ -358,8 +327,7 @@ int dense_forward(const DenseDims& D, const Pairs& Pr, const float* dist, const 
   return VIDAR_OK;
 }
 
-template <class Pairs>
-int dense_backward(const DenseDims& D, const Pairs& Pr, const float* points, const float* origin, const float* qbuf,
+int dense_backward(const DenseDims& D, const PairTable& Pr, const float* points, const float* origin, const float* qbuf,
                    const float* cbuf, const unsigned char* q_mask, const int64_t* q_off, const int64_t* c_off,
                    const int64_t* idx, const double* pairs, const float* grad_loss, float* grad_dist, void* stream,
                    const char* who) {
@@ -440,53 +408,6 @@ align_scatter_kernel(AlignDims A, const float* __restrict__ gt, const float* __r
 
 using namespace vidar;
 
-extern "C" int vidar_dense_chamfer_forward(const float* dist, const float* points, const float* origin,
-                                           const float* gt, const float* gt_tindex, const float* weights_host,
-                                           const float* pc_range_host, float weight_sum, float* qbuf, float* cbuf,
-                                           unsigned char* q_mask, unsigned char* c_mask, int64_t* q_off,
-                                           int64_t* c_off, int64_t* idx, double* pairs, float* loss, int bs, int F,
-                                           int R0, int To, int M, int W, int H, int Z, int within_grid,
-                                           void* stream) {
-  const char* who = "dense_chamfer_forward";
-  VIDAR_REQUIRE(bs > 0 && F > 0 && F <= kMaxFrames && R0 > 0 && To >= F && M >= 0,
-                "%s: bad sizes bs=%d F=%d R0=%d To=%d M=%d (F <= %d)", who, bs, F, R0, To, M, kMaxFrames);
-  DenseDims D;
-  int rc = dense_dims(D, bs * F, 1, bs, F, R0, M, who);
-  if (rc) return rc;
-  FramePairs Pr;
-  rc = frame_pairs(Pr, weights_host, weight_sum, bs, F, To, who);
-  if (rc) return rc;
-  VIDAR_REQUIRE(W > 0 && H > 0 && Z > 0, "dense_chamfer_forward: bad grid %dx%dx%d", W, H, Z);
-  VIDAR_REQUIRE(pc_range_host, "dense_chamfer_forward: null pc_range");
-  D.W = W; D.H = H; D.Z = Z; D.within = within_grid ? 1 : 0;
-  for (int k = 0; k < 6; ++k) D.pc[k] = pc_range_host[k];
-  VIDAR_REQUIRE(dist && points && origin && qbuf && cbuf && q_mask && c_mask && q_off && c_off && idx && pairs && loss,
-                "dense_chamfer_forward: null pointer argument");
-  VIDAR_REQUIRE(M == 0 || (gt && gt_tindex), "dense_chamfer_forward: null gt buffer");
-  return dense_forward(D, Pr, dist, points, origin, gt, gt_tindex, qbuf, cbuf, q_mask, c_mask, q_off, c_off, idx,
-                       pairs, loss, stream, who);
-}
-
-extern "C" int vidar_dense_chamfer_backward(const float* points, const float* origin, const float* qbuf,
-                                            const float* cbuf, const unsigned char* q_mask, const int64_t* q_off,
-                                            const int64_t* c_off, const int64_t* idx, const double* pairs,
-                                            const float* weights_host, float weight_sum, const float* grad_loss,
-                                            float* grad_dist, int bs, int F, int R0, int To, int M, void* stream) {
-  const char* who = "dense_chamfer_backward";
-  VIDAR_REQUIRE(bs > 0 && F > 0 && F <= kMaxFrames && R0 > 0 && To >= F && M >= 0,
-                "%s: bad sizes bs=%d F=%d R0=%d To=%d M=%d (F <= %d)", who, bs, F, R0, To, M, kMaxFrames);
-  DenseDims D;
-  int rc = dense_dims(D, bs * F, 1, bs, F, R0, M, who);
-  if (rc) return rc;
-  FramePairs Pr;
-  rc = frame_pairs(Pr, weights_host, weight_sum, bs, F, To, who);
-  if (rc) return rc;
-  VIDAR_REQUIRE(points && origin && qbuf && cbuf && q_mask && q_off && c_off && idx && pairs && grad_loss && grad_dist,
-                "dense_chamfer_backward: null pointer argument");
-  return dense_backward(D, Pr, points, origin, qbuf, cbuf, q_mask, q_off, c_off, idx, pairs, grad_loss, grad_dist,
-                        stream, who);
-}
-
 extern "C" int vidar_dense_chamfer_groups_forward(const float* dist, const float* points, const float* origin,
                                                   const float* gt, const float* gt_tindex, const int32_t* slot_pair,
                                                   const int32_t* pair_table, const float* pair_weight,
@@ -506,7 +427,7 @@ extern "C" int vidar_dense_chamfer_groups_forward(const float* dist, const float
   VIDAR_REQUIRE(dist && points && origin && slot_pair && pair_table && pair_weight && group_norm && qbuf && cbuf &&
                 q_mask && c_mask && q_off && c_off && idx && pairs && loss, "%s: null pointer argument", who);
   VIDAR_REQUIRE(M == 0 || (gt && gt_tindex), "%s: null gt buffer", who);
-  const TablePairs Pr{slot_pair, pair_table, pair_weight, group_norm};
+  const PairTable Pr{slot_pair, pair_table, pair_weight, group_norm};
   return dense_forward(D, Pr, dist, points, origin, gt, gt_tindex, qbuf, cbuf, q_mask, c_mask, q_off, c_off, idx,
                        pairs, loss, stream, who);
 }
@@ -524,7 +445,7 @@ extern "C" int vidar_dense_chamfer_groups_backward(const float* points, const fl
   if (rc) return rc;
   VIDAR_REQUIRE(points && origin && qbuf && cbuf && q_mask && q_off && c_off && idx && pairs && pair_table &&
                 pair_weight && group_norm && grad_loss && grad_dist, "%s: null pointer argument", who);
-  const TablePairs Pr{nullptr, pair_table, pair_weight, group_norm};
+  const PairTable Pr{nullptr, pair_table, pair_weight, group_norm};
   return dense_backward(D, Pr, points, origin, qbuf, cbuf, q_mask, q_off, c_off, idx, pairs, grad_loss, grad_dist,
                         stream, who);
 }

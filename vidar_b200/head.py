@@ -136,6 +136,16 @@ class ViDARRayHead:
         return (1 - beyond.detach() + beyond) * sampled
 
     @staticmethod
+    def _dense_grid(bev_h, bev_w, Z, device):
+        """The dense term's ray end points of one sample (vidar_head_base.py:611-619), [R0, 3] voxel units."""
+        interval = 4
+        g = bev_geometry.get_bev_grids_3d(bev_h // interval, bev_w // interval, Z // interval, bs=1, device=device)
+        g[..., 0] = g[..., 0] * bev_w
+        g[..., 1] = g[..., 1] * bev_h
+        g[..., 2] = g[..., 2] * Z
+        return g.view(-1, 3).contiguous()
+
+    @staticmethod
     def _sigma_volume(level, bs, frames, heights, bev_h, bev_w):
         """[frames, bs, bev_h*bev_w, heights] -> [bs, frames, heights, bev_h, bev_w] (:557-563)."""
         return level.permute(1, 0, 3, 2).contiguous().view(bs, frames, heights, bev_h, bev_w)
@@ -168,29 +178,25 @@ class ViDARRayHead:
                 origin_grids, gt_grids, gt_tindex, inter_sigma, loss_weight, step, self.ray_grid_num)
         if self.use_dense_loss:
             tgt = inter_sigma[-1]
-            interval = 4
-            voxel_grids = bev_geometry.get_bev_grids_3d(tgt_bev_h // interval, tgt_bev_w // interval,
-                                                        num_height_pred // interval, bs=bs, device=sigma.device)
-            voxel_grids[..., 0] = voxel_grids[..., 0] * tgt_bev_w
-            voxel_grids[..., 1] = voxel_grids[..., 1] * tgt_bev_h
-            voxel_grids[..., 2] = voxel_grids[..., 2] * num_height_pred
-            voxel_grids = voxel_grids.view(bs, -1, 3)
-            ones = voxel_grids.new_ones(*voxel_grids.shape[:2]).to(gt_tindex.dtype)
-            voxel_grids = torch.cat([voxel_grids for _ in range(valid_frame_num)], 1)
-            voxel_tindex = torch.cat([ones * i for i in range(valid_frame_num)], 1)
+            grid = self._dense_grid(tgt_bev_h, tgt_bev_w, num_height_pred, sigma.device)
+            R0 = grid.shape[0]
+            voxel_grids = grid.repeat(bs * valid_frame_num, 1).view(bs, -1, 3)
+            voxel_tindex = (torch.arange(valid_frame_num, dtype=gt_tindex.dtype, device=sigma.device)
+                            .repeat_interleave(R0).repeat(bs, 1))
             if self.fuse_dense_decode:
-                # sampler + gumbel decode in one kernel per batch element: the [bs, rays, ray_grid_num]
-                # logits / softmax / one-hot tensors are never written.  The noise is drawn with the
-                # statement F.gumbel_softmax uses, on the shape its logits would have.
+                # sampler + gumbel decode in one kernel over the bs * F volumes (ray volume b * F + f): the
+                # [bs, rays, ray_grid_num] logits / softmax / one-hot tensors are never written.  The noise is drawn
+                # with the statement F.gumbel_softmax uses, on the shape its logits would have.
                 noise = gumbels.get("dense")
                 if noise is None:
                     noise = -torch.empty((bs, voxel_grids.shape[1], self.ray_grid_num), dtype=torch.float32,
                                          device=sigma.device).exponential_().log()
-                frame = voxel_tindex[0].to(torch.int32).contiguous()
-                dense_dist = torch.stack([
-                    ray_head.gumbel_distance(tgt[b], origin_grids[b, :valid_frame_num].contiguous().float(),
-                                             voxel_grids[b].contiguous(), frame, self.ray_grid_num, step, noise[b])
-                    for b in range(bs)])
+                frame = torch.arange(bs * valid_frame_num, dtype=torch.int32, device=sigma.device).repeat_interleave(R0)
+                dense_dist = ray_head.gumbel_distance(
+                    tgt.view(bs * valid_frame_num, num_height_pred, tgt_bev_h, tgt_bev_w),
+                    origin_grids[:, :valid_frame_num].reshape(bs * valid_frame_num, 3).float(),
+                    voxel_grids.view(-1, 3), frame, self.ray_grid_num, step,
+                    noise.reshape(-1, self.ray_grid_num)).view(bs, -1)
             else:
                 _, d_feat, _, d_len = ray_head.get_grid_features(
                     origin_grids, voxel_grids, voxel_tindex, [tgt], np.array([[1]] * valid_frame_num), step,
@@ -500,16 +506,6 @@ class ViDARRayHeadV1(ViDARRayHead):
             for k, v in terms.items():
                 loss_dict[f"frame.{idx}.{k}.loss"] = v[i] * (self.per_frame_loss_weight[i] * (idx == i))
         return loss_dict
-
-    @staticmethod
-    def _dense_grid(bev_h, bev_w, Z, device):
-        """The dense term's ray end points of one sample (vidar_head_base.py:611-619), [R0, 3] voxel units."""
-        interval = 4
-        g = bev_geometry.get_bev_grids_3d(bev_h // interval, bev_w // interval, Z // interval, bs=1, device=device)
-        g[..., 0] = g[..., 0] * bev_w
-        g[..., 1] = g[..., 1] * bev_h
-        g[..., 2] = g[..., 2] * Z
-        return g.view(-1, 3).contiguous()
 
     def _pair_noise(self, gumbels, frame_idx_for_loss, tab, bs, R0, device):
         """Gumbel noise [P*R0, K] of the weighted pairs: slices of the per-head-frame noise when given, else drawn

@@ -12,10 +12,10 @@ projects/mmdet3d_plugin/bevformer/dense_heads/vidar_head_base.py:
   decode_ray_depth(...)       == the per-(batch, frame) body of get_point_cloud_prediction
                                  (:706-738): arg-max waypoint -> distance;
   dense_chamfer_loss(...)     == the Chamfer loop of the `use_dense_loss` branch of ViDARHeadBase.loss
-                                 (:638-659) over every (sample, frame) pair in one batched op
-                                 (csrc/dense_chamfer.cu), no host sync.
-  dense_chamfer_group_loss(...) == the same Chamfer term over a pair table, one loss per group
-                                 (ViDARHeadV1: a group per head frame);
+                                 (:638-659) over every (sample, frame) pair in one batched op, no host
+                                 sync: dense_chamfer_group_loss with pair n = b*F + f and one group;
+  dense_chamfer_group_loss(...) == the same Chamfer term over a pair table (csrc/dense_chamfer.cu), one
+                                 loss per group (ViDARHeadV1: a group per head frame);
   align_gt(...)               == ViDARHeadV1._get_reference_gt_points (vidar_head_v1.py:94-148) for every
                                  (head frame, target frame) job in one op;
   decode_clouds(...)          == get_point_cloud_prediction's rendering of the decoded rays (:698-745,
@@ -26,6 +26,7 @@ Low-level autograd ops: `ray_sample` (logits/lengths, differentiable w.r.t. sigm
 All tensors must be CUDA; there is no PyTorch fallback.
 """
 import ctypes as C
+import functools
 
 import numpy as np
 import torch
@@ -284,52 +285,6 @@ def decode_ray_depth(sigma, origin_grids, gt_grids, gt_tindex, ray_grid_step, ra
     return pred, gt
 
 
-class _DenseChamfer(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, dist, points, origin, gt, gt_tindex, grid, weights, weight_sum, within_grid, pc_range):
-        dev = dist.device
-        bs, FR = dist.shape
-        F = len(weights)
-        R0 = FR // F
-        To, M = origin.shape[1], gt.shape[1]
-        W, H, Z = (int(v) for v in grid)
-        Pq = bs * FR + bs * M
-        S = bs * F
-        qbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
-        cbuf = torch.empty((Pq, 3), dtype=torch.float32, device=dev)
-        q_mask = torch.empty(Pq, dtype=torch.uint8, device=dev)
-        c_mask = torch.empty(Pq, dtype=torch.uint8, device=dev)
-        seg_off = torch.empty((2, 2 * S + 1), dtype=torch.int64, device=dev)
-        idx = torch.empty(Pq, dtype=torch.int64, device=dev)
-        pairs = torch.empty((S, 4), dtype=torch.float64, device=dev)
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        w = (C.c_float * F)(*weights)
-        rng = (C.c_float * 6)(*[float(v) for v in pc_range])
-        P = _lib.ptr
-        _call(_lib.lib().vidar_dense_chamfer_forward, dev, P(dist), P(points), P(origin), P(gt), P(gt_tindex),
-              C.cast(w, C.c_void_p), C.cast(rng, C.c_void_p), float(weight_sum), P(qbuf), P(cbuf), P(q_mask),
-              P(c_mask), P(seg_off[0]), P(seg_off[1]), P(idx), P(pairs), P(loss), bs, F, R0, To, M, W, H, Z,
-              int(bool(within_grid)))
-        ctx.save_for_backward(points, origin, qbuf, cbuf, q_mask, seg_off, idx, pairs)
-        ctx.meta = (tuple(weights), float(weight_sum), bs, F, R0, To, M)
-        ctx.mark_non_differentiable(pairs)
-        return loss, pairs
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_loss, _gp):
-        points, origin, qbuf, cbuf, q_mask, seg_off, idx, pairs = ctx.saved_tensors
-        weights, weight_sum, bs, F, R0, To, M = ctx.meta
-        g = grad_loss.float().contiguous()
-        grad_dist = torch.empty((bs, F * R0), dtype=torch.float32, device=qbuf.device)
-        w = (C.c_float * F)(*weights)
-        P = _lib.ptr
-        _call(_lib.lib().vidar_dense_chamfer_backward, qbuf.device, P(points), P(origin), P(qbuf), P(cbuf),
-              P(q_mask), P(seg_off[0]), P(seg_off[1]), P(idx), P(pairs), C.cast(w, C.c_void_p), weight_sum, P(g),
-              P(grad_dist), bs, F, R0, To, M)
-        return grad_dist, None, None, None, None, None, None, None, None, None
-
-
 def dense_chamfer_loss(dist, points, origin, gt, gt_tindex, grid, frame_weights, weight_sum, eval_within_grid=False,
                        pc_range=None, return_pairs=False):
     """`loss.dense_voxel` before its `dense_loss_weight` (vidar_head_base.py:594-659), every (sample, frame) pair
@@ -339,9 +294,8 @@ def dense_chamfer_loss(dist, points, origin, gt, gt_tindex, grid, frame_weights,
     [bs, >=F, 3], gt [bs, M, 3] and gt_tindex [bs, M] (float, -1 = padding, any order), all voxel units on one CUDA
     device; grid = (W, H, Z); frame_weights: F host floats (loss_weight[f, 0]); weight_sum: loss_weight.sum(), the
     loss divides by weight_sum * bs; pc_range: metres, used by eval_within_grid like get_rendered_pcds.
-    Returns the 0-dim loss (and, with return_pairs, [bs*F, 4] float64 per pair: sum pred->gt squared distances,
-    pred points, sum gt->pred, gt points)."""
-    _lib.require_cuda(dist=dist, points=points, origin=origin, gt=gt, gt_tindex=gt_tindex)
+    Returns the 0-dim loss (and, with return_pairs, [bs*F, 4] float64 per pair n = b*F + f: sum pred->gt squared
+    distances, pred points, sum gt->pred, gt points)."""
     frame_weights = [float(v) for v in frame_weights]
     F = len(frame_weights)
     if dist.dim() != 2 or F == 0 or dist.shape[1] % F:
@@ -356,9 +310,43 @@ def dense_chamfer_loss(dist, points, origin, gt, gt_tindex, grid, frame_weights,
             raise RuntimeError(f"{name} must be float32")
     if eval_within_grid and pc_range is None:
         raise RuntimeError("eval_within_grid needs pc_range")
-    loss, pairs = _DenseChamfer.apply(dist, points, origin, gt, gt_tindex, grid, frame_weights, weight_sum,
-                                      eval_within_grid, pc_range if pc_range is not None else [0.0] * 6)
-    return (loss, pairs) if return_pairs else loss
+    _lib.require_cuda(dist=dist, points=points, origin=origin, gt=gt, gt_tindex=gt_tindex)
+    norm = float(np.float32(weight_sum) * np.float32(bs))        # the fp32 product weight_sum * bs
+    loss, pairs = _chamfer_groups(dist.view(-1), points.view(-1, 3), origin.view(-1, 3), gt, gt_tindex, grid,
+                                  _frame_tables(bs, F, origin.shape[1], tuple(frame_weights), norm), bs * F, 1, F,
+                                  eval_within_grid, pc_range)
+    return (loss.view(()), pairs) if return_pairs else loss.view(())
+
+
+@functools.lru_cache(maxsize=64)
+def _frame_tables(bs, F, To, frame_weights, norm):
+    """dense_chamfer_loss's host tables, built once per shape and weights (the loss is host-bound at small bs):
+    pair n = b*F + f of sample b's frame f, origin row b*To + f, weight frame_weights[f], one group."""
+    b, f = np.divmod(np.arange(bs * F), F)
+    return _host_tables(np.stack([b, f, b * To + f, np.zeros_like(b)], 1), np.tile(np.float32(frame_weights), bs),
+                        np.float32([norm]), bs, F)
+
+
+def _host_tables(tab, w, norms, Sg, Fg):
+    """The pair tables as one int32 host array: pair of each (gt sample, frame) slot [Sg*Fg] (-1 = none), (slot,
+    origin row, group) of each pair [P, 3], then the float32 bits of the pair weights [P] and group norms."""
+    slot = tab[:, 0] * Fg + tab[:, 1]
+    slot_pair = np.full(Sg * Fg, -1, dtype=np.int64)
+    slot_pair[slot] = np.arange(tab.shape[0])
+    ints = np.concatenate([slot_pair, np.stack([slot, tab[:, 2], tab[:, 3]], 1).ravel()]).astype(np.int32)
+    return np.concatenate([ints, np.concatenate([w, norms]).astype(np.float32).view(np.int32)])
+
+
+def _chamfer_groups(dist, points, origin, gt, gt_tindex, grid, host, P, groups, Fg, eval_within_grid, pc_range):
+    """Checked arguments of dense_chamfer_group_loss -> (loss [groups], pairs [P, 4]); the host tables reach the
+    device in one pinned non-blocking copy."""
+    Sg, M = gt.shape[:2]
+    table = _pinned_upload(host, np.int32, dist.device)
+    n = Sg * Fg + 3 * P
+    tables = (table[: Sg * Fg], table[Sg * Fg:n], table[n:n + P].view(torch.float32), table[n + P:].view(torch.float32))
+    return _DenseChamferGroups.apply(dist, points, origin, gt, gt_tindex, tables,
+                                     (P, groups, dist.shape[0] // P, Sg, Fg, M), grid, eval_within_grid,
+                                     pc_range if pc_range is not None else [0.0] * 6)
 
 
 def _pinned_upload(host, dtype, device):
@@ -445,15 +433,8 @@ def dense_chamfer_group_loss(dist, points, origin, gt, gt_tindex, grid, pairs, p
     if eval_within_grid and pc_range is None:
         raise RuntimeError("eval_within_grid needs pc_range")
     _lib.require_cuda(dist=dist, points=points, origin=origin, gt=gt, gt_tindex=gt_tindex)
-    slot_pair = np.full(Sg * Fg, -1, dtype=np.int64)
-    slot_pair[slot] = np.arange(P)
-    ints = _pinned_upload(np.concatenate([slot_pair, np.stack([slot, tab[:, 2], tab[:, 3]], 1).ravel()]), np.int32,
-                          dist.device)
-    floats = _pinned_upload(np.concatenate([w, norms]), np.float32, dist.device)
-    tables = (ints[: Sg * Fg], ints[Sg * Fg:], floats[:P], floats[P:])
-    loss, pair_sums = _DenseChamferGroups.apply(dist, points, origin, gt, gt_tindex, tables,
-                                                (P, groups, R0, Sg, Fg, M), grid, eval_within_grid,
-                                                pc_range if pc_range is not None else [0.0] * 6)
+    loss, pair_sums = _chamfer_groups(dist, points, origin, gt, gt_tindex, grid, _host_tables(tab, w, norms, Sg, Fg),
+                                      P, groups, Fg, eval_within_grid, pc_range)
     return (loss, pair_sums) if return_pairs else loss
 
 
