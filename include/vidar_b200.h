@@ -552,6 +552,22 @@ int vidar_dcn_col2im(const float* x, const float* offset, const float* mask, con
                      float* grad_offset, float* grad_mask, int N, int C, int H, int W, int Ho, int Wo, int kh, int kw,
                      int sh, int sw, int ph, int pw, int dh, int dw, int n0, int nb, void* stream);
 
+/* The same two calls with x, offset, mask and cols / grad_cols in 16 bits: `dtype` is VIDAR_DTYPE_F16 (IEEE half)
+ * or VIDAR_DTYPE_BF16 (bfloat16); any other value returns VIDAR_E_INVALID ("unsupported dtype").  Every value is
+ * converted to fp32 on load, so a sample lands where the fp32 op puts it for the same (rounded) offsets; bilinear
+ * weights, products and sums are fp32.  im2col rounds each column element once, to `dtype`.  col2im accumulates
+ * grad_x and writes grad_offset / grad_mask in fp32 (same layouts as above).  The vector paths (8 channels per
+ * 16-byte load) run when C % 8 == 0 and the buffers are 16-byte aligned. */
+#define VIDAR_DTYPE_F16 1
+#define VIDAR_DTYPE_BF16 2
+int vidar_dcn_im2col_half(const void* x, const void* offset, const void* mask, void* cols, int dtype, int N, int C,
+                          int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
+                          int n0, int nb, void* stream);
+int vidar_dcn_col2im_half(const void* x, const void* offset, const void* mask, const void* grad_cols, float* grad_x,
+                          float* grad_offset, float* grad_mask, int dtype, int N, int C, int H, int W, int Ho, int Wo,
+                          int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int n0, int nb,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,9 +6,17 @@
 // outside the image adds 0).  Column row m = (n, ho, wo) holds mask[n, k, ho, wo] * v_c at k * C + c, so the
 // convolution is cols [M, kh*kw*C] times the weight permuted to [Cout, kh, kw, C] -- a GEMM the host runs.
 //
-// x is channel-last (NHWC): every bilinear corner is one contiguous C-float line, and a column row is written as
-// kh*kw full lines.  One warp per (row, kernel point); its lanes stride over the channels, four at a time when
-// C % 4 == 0 (16-byte loads, stores and red.global.add.v4), one at a time otherwise.
+// x is channel-last (NHWC): every bilinear corner is one contiguous C-element line, and a column row is written as
+// kh*kw full lines.  One warp per (row, kernel point); its lanes stride over the channels, one 16-byte vector at a
+// time when C is a multiple of its width (4 floats, or 8 fp16 / bf16 values) and the buffers are 16-byte aligned,
+// one channel at a time otherwise.
+//
+// Storage type T is float, __half or __nv_bfloat16 for x, offset, mask and the columns.  Every value is converted to
+// fp32 on load; the bilinear weights, products and sums are fp32.  A 16-bit im2col rounds each column element once on
+// its store.  col2im accumulates grad_x and writes grad_offset / grad_mask in fp32 whatever T is.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace vidar {
@@ -31,8 +39,16 @@ struct Sample {
   bool v00, v01, v10, v11;
 };
 
-__device__ __forceinline__ Sample locate(const float* __restrict__ offset, const float* __restrict__ mask,
-                                         const DcnGeom& g, long long m, int k) {
+__device__ __forceinline__ float to_f(float v) { return v; }
+__device__ __forceinline__ float to_f(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ void store1(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store1(__half* p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void store1(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+template <typename T>
+__device__ __forceinline__ Sample locate(const T* __restrict__ offset, const T* __restrict__ mask, const DcnGeom& g,
+                                         long long m, int k) {
   const int K = g.kh * g.kw;
   const long long HW = (long long)g.Ho * g.Wo;
   Sample s;
@@ -41,10 +57,10 @@ __device__ __forceinline__ Sample locate(const float* __restrict__ offset, const
   const int ho = (int)(p / g.Wo), wo = (int)(p - (long long)ho * g.Wo);
   const int i = k / g.kw, j = k - i * g.kw;
   s.n = g.n0 + nl;
-  const float* op = offset + (s.n * 2 * K + 2 * k) * HW + p;
-  const float h = (float)(ho * g.sh - g.ph + i * g.dh) + __ldg(op);
-  const float w = (float)(wo * g.sw - g.pw + j * g.dw) + __ldg(op + HW);
-  s.m = __ldg(mask + (s.n * K + k) * HW + p);
+  const T* op = offset + (s.n * 2 * K + 2 * k) * HW + p;
+  const float h = (float)(ho * g.sh - g.ph + i * g.dh) + to_f(__ldg(op));
+  const float w = (float)(wo * g.sw - g.pw + j * g.dw) + to_f(__ldg(op + HW));
+  s.m = to_f(__ldg(mask + (s.n * K + k) * HW + p));
   s.inside = !(h <= -1.f || h >= (float)g.H || w <= -1.f || w >= (float)g.W);
   const float hf = floorf(h), wf = floorf(w);
   s.y0 = (int)hf;
@@ -58,8 +74,9 @@ __device__ __forceinline__ Sample locate(const float* __restrict__ offset, const
   return s;
 }
 
-template <int V> struct Vec;
-template <> struct Vec<4> {
+// V channels of storage type T as fp32 values: load / store convert, red adds into an fp32 buffer.
+template <typename T, int V> struct Vec;
+template <> struct Vec<float, 4> {
   using T = float4;
   static __device__ __forceinline__ T load(const float* p) { return ldg4(p); }
   static __device__ __forceinline__ void store(float* p, T v) { *reinterpret_cast<float4*>(p) = v; }
@@ -72,10 +89,10 @@ template <> struct Vec<4> {
   static __device__ __forceinline__ float dot(T a, T b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
   static __device__ __forceinline__ void red(float* p, T v) { red_add_v4(p, v); }
 };
-template <> struct Vec<1> {
+template <typename S> struct Vec<S, 1> {
   using T = float;
-  static __device__ __forceinline__ T load(const float* p) { return __ldg(p); }
-  static __device__ __forceinline__ void store(float* p, T v) { *p = v; }
+  static __device__ __forceinline__ T load(const S* p) { return to_f(__ldg(p)); }
+  static __device__ __forceinline__ void store(S* p, T v) { store1(p, v); }
   static __device__ __forceinline__ T zero() { return 0.f; }
   static __device__ __forceinline__ T fma(float a, T x, T y) { return fmaf(a, x, y); }
   static __device__ __forceinline__ T scale(float a, T x) { return a * x; }
@@ -84,12 +101,60 @@ template <> struct Vec<1> {
   static __device__ __forceinline__ void red(float* p, T v) { red_add_f32(p, v); }
 };
 
+// Eight 16-bit channels: one 16-byte load / store (a uint4 holding four half2 / bfloat162 pairs), two fp32 float4s
+// in registers, two red.global.add.v4.f32 into the fp32 gradient.
+struct F8 {
+  float4 a, b;
+};
+template <typename S> struct Pair;
+template <> struct Pair<__half> {
+  static __device__ __forceinline__ float2 unpack(unsigned u) { return __half22float2(*reinterpret_cast<__half2*>(&u)); }
+  static __device__ __forceinline__ unsigned pack(float lo, float hi) {
+    __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<unsigned*>(&h);
+  }
+};
+template <> struct Pair<__nv_bfloat16> {
+  static __device__ __forceinline__ float2 unpack(unsigned u) {
+    return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u));
+  }
+  static __device__ __forceinline__ unsigned pack(float lo, float hi) {
+    __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<unsigned*>(&h);
+  }
+};
+template <typename S> struct Vec<S, 8> {
+  using T = F8;
+  using V4 = Vec<float, 4>;
+  static __device__ __forceinline__ T load(const S* p) {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+    const float2 q0 = Pair<S>::unpack(u.x), q1 = Pair<S>::unpack(u.y), q2 = Pair<S>::unpack(u.z), q3 = Pair<S>::unpack(u.w);
+    return {make_float4(q0.x, q0.y, q1.x, q1.y), make_float4(q2.x, q2.y, q3.x, q3.y)};
+  }
+  static __device__ __forceinline__ void store(S* p, T v) {
+    *reinterpret_cast<uint4*>(p) = make_uint4(Pair<S>::pack(v.a.x, v.a.y), Pair<S>::pack(v.a.z, v.a.w),
+                                              Pair<S>::pack(v.b.x, v.b.y), Pair<S>::pack(v.b.z, v.b.w));
+  }
+  static __device__ __forceinline__ T zero() { return {V4::zero(), V4::zero()}; }
+  static __device__ __forceinline__ T fma(float a, T x, T y) { return {V4::fma(a, x.a, y.a), V4::fma(a, x.b, y.b)}; }
+  static __device__ __forceinline__ T scale(float a, T x) { return {V4::scale(a, x.a), V4::scale(a, x.b)}; }
+  static __device__ __forceinline__ T sub(T a, T b) { return {V4::sub(a.a, b.a), V4::sub(a.b, b.b)}; }
+  static __device__ __forceinline__ float dot(T a, T b) { return V4::dot(a.a, b.a) + V4::dot(a.b, b.b); }
+  static __device__ __forceinline__ void red(float* p, T v) {
+    red_add_v4(p, v.a);
+    red_add_v4(p + 4, v.b);
+  }
+};
+
+// The vector width of storage type T: 16 bytes.
+template <typename T> constexpr int kVec = 16 / sizeof(T);
+
 // cols [rows, K * C]: row m, kernel point k, channel c at (m * K + k) * C + c.
-template <int V>
-__global__ void __launch_bounds__(kThreads) dcn_im2col_kernel(const float* __restrict__ x, const float* __restrict__ offset,
-                                                              const float* __restrict__ mask, float* __restrict__ cols,
+template <typename T, int V>
+__global__ void __launch_bounds__(kThreads) dcn_im2col_kernel(const T* __restrict__ x, const T* __restrict__ offset,
+                                                              const T* __restrict__ mask, T* __restrict__ cols,
                                                               DcnGeom g, long long items) {
-  using Op = Vec<V>;
+  using Op = Vec<T, V>;
   const int lane = threadIdx.x & 31;
   const int K = g.kh * g.kw;
   const long long stride = (long long)gridDim.x * kWarps;
@@ -97,13 +162,13 @@ __global__ void __launch_bounds__(kThreads) dcn_im2col_kernel(const float* __res
     const long long m = it / K;
     const int k = (int)(it - m * K);
     const Sample s = locate(offset, mask, g, m, k);
-    float* out = cols + it * g.C;
+    T* out = cols + it * g.C;
     const float w00 = (1.f - s.lh) * (1.f - s.lw), w01 = (1.f - s.lh) * s.lw, w10 = s.lh * (1.f - s.lw), w11 = s.lh * s.lw;
-    const float* img = x + s.n * g.H * g.W * g.C;
-    const float* p00 = img + ((long long)s.y0 * g.W + s.x0) * g.C;
-    const float* p01 = p00 + g.C;
-    const float* p10 = p00 + (long long)g.W * g.C;
-    const float* p11 = p10 + g.C;
+    const T* img = x + s.n * g.H * g.W * g.C;
+    const T* p00 = img + ((long long)s.y0 * g.W + s.x0) * g.C;
+    const T* p01 = p00 + g.C;
+    const T* p10 = p00 + (long long)g.W * g.C;
+    const T* p11 = p10 + g.C;
     for (int c = lane * V; c < g.C; c += 32 * V) {
       typename Op::T v = Op::zero();
       if (s.v00) v = Op::fma(w00, Op::load(p00 + c), v);
@@ -120,13 +185,13 @@ __global__ void __launch_bounds__(kThreads) dcn_im2col_kernel(const float* __res
 //   grad_offset [N, 2K, Ho, Wo]           = mask * sum_c grad_col * d v_c / d(h, w)
 //   grad_mask [N, K, Ho, Wo]              = sum_c grad_col * v_c
 // The derivative is that of the bilinear form on the floor cell (one-sided on integer lines, 0 outside the open range).
-template <int V>
-__global__ void __launch_bounds__(kThreads) dcn_col2im_kernel(const float* __restrict__ x, const float* __restrict__ offset,
-                                                              const float* __restrict__ mask,
-                                                              const float* __restrict__ grad_cols, float* __restrict__ grad_x,
+template <typename T, int V>
+__global__ void __launch_bounds__(kThreads) dcn_col2im_kernel(const T* __restrict__ x, const T* __restrict__ offset,
+                                                              const T* __restrict__ mask,
+                                                              const T* __restrict__ grad_cols, float* __restrict__ grad_x,
                                                               float* __restrict__ grad_offset, float* __restrict__ grad_mask,
                                                               DcnGeom g, long long items) {
-  using Op = Vec<V>;
+  using Op = Vec<T, V>;
   const int lane = threadIdx.x & 31;
   const int K = g.kh * g.kw;
   const long long HW = (long long)g.Ho * g.Wo;
@@ -135,7 +200,7 @@ __global__ void __launch_bounds__(kThreads) dcn_col2im_kernel(const float* __res
     const long long m = it / K;
     const int k = (int)(it - m * K);
     const Sample s = locate(offset, mask, g, m, k);
-    const float* gc = grad_cols + it * g.C;
+    const T* gc = grad_cols + it * g.C;
     const float hh = 1.f - s.lh, hw = 1.f - s.lw;
     const float w00 = hh * hw, w01 = hh * s.lw, w10 = s.lh * hw, w11 = s.lh * s.lw;
     const long long img = s.n * g.H * g.W * g.C;
@@ -201,6 +266,36 @@ int grid_for(long long items) {
   return (int)(want < cap ? want : cap);
 }
 
+// The vector kernel when C fills whole 16-byte vectors and the buffers are 16-byte aligned, else the scalar one.
+template <typename T>
+int im2col(const char* who, const void* x, const void* offset, const void* mask, void* cols, const DcnGeom& g,
+           long long items, cudaStream_t st) {
+  const T *xt = (const T*)x, *ot = (const T*)offset, *mt = (const T*)mask;
+  if (g.C % kVec<T> == 0 && aligned16(x) && aligned16(cols))
+    dcn_im2col_kernel<T, kVec<T>><<<grid_for(items), kThreads, 0, st>>>(xt, ot, mt, (T*)cols, g, items);
+  else
+    dcn_im2col_kernel<T, 1><<<grid_for(items), kThreads, 0, st>>>(xt, ot, mt, (T*)cols, g, items);
+  return check_launch(who);
+}
+
+template <typename T>
+int col2im(const char* who, const void* x, const void* offset, const void* mask, const void* grad_cols, float* grad_x,
+           float* grad_offset, float* grad_mask, const DcnGeom& g, long long items, cudaStream_t st) {
+  const T *xt = (const T*)x, *ot = (const T*)offset, *mt = (const T*)mask, *gt = (const T*)grad_cols;
+  if (g.C % kVec<T> == 0 && aligned16(x) && aligned16(grad_cols) && aligned16(grad_x))
+    dcn_col2im_kernel<T, kVec<T>><<<grid_for(items), kThreads, 0, st>>>(xt, ot, mt, gt, grad_x, grad_offset, grad_mask,
+                                                                        g, items);
+  else
+    dcn_col2im_kernel<T, 1><<<grid_for(items), kThreads, 0, st>>>(xt, ot, mt, gt, grad_x, grad_offset, grad_mask, g,
+                                                                  items);
+  return check_launch(who);
+}
+
+int check_dtype(const char* who, int dtype) {
+  VIDAR_REQUIRE(dtype == VIDAR_DTYPE_F16 || dtype == VIDAR_DTYPE_BF16, "%s: unsupported dtype %d", who, dtype);
+  return VIDAR_OK;
+}
+
 }  // namespace
 }  // namespace vidar
 
@@ -215,13 +310,24 @@ extern "C" int vidar_dcn_im2col(const float* x, const float* offset, const float
   if (rc) return rc;
   if (nb == 0) return VIDAR_OK;
   const DcnGeom g{C, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, n0};
+  return im2col<float>(who, x, offset, mask, cols, g, (long long)nb * Ho * Wo * kh * kw, (cudaStream_t)stream);
+}
+
+extern "C" int vidar_dcn_im2col_half(const void* x, const void* offset, const void* mask, void* cols, int dtype, int N,
+                                     int C, int H, int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw,
+                                     int dh, int dw, int n0, int nb, void* stream) {
+  const char* who = "dcn_im2col_half";
+  VIDAR_REQUIRE(x && offset && mask && cols, "%s: null pointer argument", who);
+  int rc = check_dtype(who, dtype);
+  if (rc) return rc;
+  rc = validate(who, N, C, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, n0, nb);
+  if (rc) return rc;
+  if (nb == 0) return VIDAR_OK;
+  const DcnGeom g{C, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, n0};
   const long long items = (long long)nb * Ho * Wo * kh * kw;
   cudaStream_t st = (cudaStream_t)stream;
-  if (C % 4 == 0 && aligned16(x) && aligned16(cols))
-    dcn_im2col_kernel<4><<<grid_for(items), kThreads, 0, st>>>(x, offset, mask, cols, g, items);
-  else
-    dcn_im2col_kernel<1><<<grid_for(items), kThreads, 0, st>>>(x, offset, mask, cols, g, items);
-  return check_launch(who);
+  return dtype == VIDAR_DTYPE_F16 ? im2col<__half>(who, x, offset, mask, cols, g, items, st)
+                                  : im2col<__nv_bfloat16>(who, x, offset, mask, cols, g, items, st);
 }
 
 extern "C" int vidar_dcn_col2im(const float* x, const float* offset, const float* mask, const float* grad_cols,
@@ -234,13 +340,25 @@ extern "C" int vidar_dcn_col2im(const float* x, const float* offset, const float
   if (rc) return rc;
   if (nb == 0) return VIDAR_OK;
   const DcnGeom g{C, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, n0};
+  return col2im<float>(who, x, offset, mask, grad_cols, grad_x, grad_offset, grad_mask, g,
+                       (long long)nb * Ho * Wo * kh * kw, (cudaStream_t)stream);
+}
+
+extern "C" int vidar_dcn_col2im_half(const void* x, const void* offset, const void* mask, const void* grad_cols,
+                                     float* grad_x, float* grad_offset, float* grad_mask, int dtype, int N, int C, int H,
+                                     int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw, int dh,
+                                     int dw, int n0, int nb, void* stream) {
+  const char* who = "dcn_col2im_half";
+  VIDAR_REQUIRE(x && offset && mask && grad_cols && grad_x && grad_offset && grad_mask, "%s: null pointer argument", who);
+  int rc = check_dtype(who, dtype);
+  if (rc) return rc;
+  rc = validate(who, N, C, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, n0, nb);
+  if (rc) return rc;
+  if (nb == 0) return VIDAR_OK;
+  const DcnGeom g{C, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, dh, dw, n0};
   const long long items = (long long)nb * Ho * Wo * kh * kw;
   cudaStream_t st = (cudaStream_t)stream;
-  if (C % 4 == 0 && aligned16(x) && aligned16(grad_cols) && aligned16(grad_x))
-    dcn_col2im_kernel<4><<<grid_for(items), kThreads, 0, st>>>(x, offset, mask, grad_cols, grad_x, grad_offset, grad_mask,
-                                                                g, items);
-  else
-    dcn_col2im_kernel<1><<<grid_for(items), kThreads, 0, st>>>(x, offset, mask, grad_cols, grad_x, grad_offset, grad_mask,
-                                                                g, items);
-  return check_launch(who);
+  return dtype == VIDAR_DTYPE_F16
+             ? col2im<__half>(who, x, offset, mask, grad_cols, grad_x, grad_offset, grad_mask, g, items, st)
+             : col2im<__nv_bfloat16>(who, x, offset, mask, grad_cols, grad_x, grad_offset, grad_mask, g, items, st);
 }

@@ -16,13 +16,18 @@ Columns are computed for chunks of whole images of at most MAX_COLS_BYTES (512 M
 columns are larger), so the scratch does not grow with the batch.  At the reference's 6 x 928 x 1600 input a stage-3
 layer's columns are 6 x 5800 x 2304 floats (321 MB) and a stage-4 layer's 160 MB: one chunk each.
 
-Only groups == 1 and deform_groups == 1 (every reference config) and fp32 CUDA tensors are supported; anything else
-raises, there is no CPU fallback.
+Mixed precision (mmcv 1.4.0's amp rule, see ModulatedDeformConv2dFunction): the op computes in the dtype of `offset`,
+float32, float16 or bfloat16.  In 16 bits x, offset, mask and the columns are stored in that dtype, the sampling
+arithmetic is fp32, and the GEMMs run on cuBLAS in that dtype with fp32 accumulation; the 3xTF32 GEMM is fp32 only.
+
+Only groups == 1 and deform_groups == 1 (every reference config) and CUDA tensors of those three dtypes are supported;
+anything else raises, there is no CPU fallback.
 """
 import math
 
 import torch
 import torch.nn as nn
+from torch.amp import custom_bwd, custom_fwd
 from torch.autograd.function import Function, once_differentiable
 from torch.nn.modules.utils import _pair
 
@@ -43,9 +48,24 @@ def _check_groups(groups, deform_groups):
                          f"(got groups={groups}, deform_groups={deform_groups})")
 
 
-def chunk_images(N, per_image_floats):
-    """Images per column chunk: as many as fit in MAX_COLS_BYTES, at least one."""
-    return max(1, min(N, MAX_COLS_BYTES // max(1, 4 * per_image_floats)))
+def chunk_images(N, per_image_elems, elem_size=4):
+    """Images per column chunk: as many as fit in MAX_COLS_BYTES, at least one (`elem_size` bytes per element)."""
+    return max(1, min(N, MAX_COLS_BYTES // max(1, elem_size * per_image_elems)))
+
+
+# dtype codes of vidar_dcn_im2col_half / vidar_dcn_col2im_half (VIDAR_DTYPE_F16 / _BF16 of include/vidar_b200.h)
+HALF_DTYPE_CODES = {torch.float16: 1, torch.bfloat16: 2}
+_COMPUTE_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def compute_dtype(input, offset, mask, weight, bias=None):
+    """The dtype the op computes in, from the dtypes of its five tensors (None for no bias): mmcv's amp rule, the
+    dtype of `offset`.  Every tensor must be float32, float16 or bfloat16 (the others are cast to the result);
+    anything else raises TypeError."""
+    for name, dt in (("input", input), ("offset", offset), ("mask", mask), ("weight", weight), ("bias", bias)):
+        if dt is not None and dt not in _COMPUTE_DTYPES:
+            raise TypeError(f"modulated_deform_conv2d: {name} must be float32, float16 or bfloat16 (got {dt})")
+    return offset
 
 
 def _gemm(a, w, bias, out, scratch):
@@ -71,16 +91,33 @@ def _geometry(x, weight, stride, padding, dilation):
 
 class ModulatedDeformConv2dFunction(Function):
     """mmcv.ops.ModulatedDeformConv2dFunction: forward(input, offset, mask, weight, bias=None, stride=1, padding=0,
-    dilation=1, groups=1, deform_groups=1)."""
+    dilation=1, groups=1, deform_groups=1).
+
+    Dtypes, restated from mmcv 1.4.0's published `ModulatedDeformConv2dFunction.forward` (its source is not part of
+    this project, and this rule has not been run against it): the op computes in cd = offset.dtype, and input, mask,
+    weight and bias are cast to cd.  Under autocast the offset conv emits the autocast dtype, so the op runs in it;
+    mmcv's fp16 mode (`Fp16OptimizerHook` + `auto_fp16`) is autocast on torch >= 1.6.
+      cd = float32             the fp32 path (3xTF32 / fp32 cuBLAS GEMMs), unchanged by this rule.
+      cd = float16, bfloat16   x, offset, mask and the columns in cd, sampling arithmetic in fp32 (csrc/dcn.cu, each
+                               column element rounded once); y = cols @ W'^T (+ bias) and grad_cols = g @ W' on cuBLAS
+                               in cd with fp32 accumulation (the user's allow_fp16/bf16_reduced_precision_reduction
+                               settings apply); grad_W' per chunk by `torch.mm(..., out_dtype=torch.float32)`, summed
+                               over chunks in fp32; grad_x, grad_offset and grad_mask from col2im in fp32.
+      anything else            TypeError (`compute_dtype`).
+    The output has dtype cd; each gradient is cast once to its leaf's dtype (an fp32 weight gets an fp32 grad_weight).
+    The GEMMs run with autocast disabled, so their dtypes do not depend on the autocast state around the call."""
 
     @staticmethod
+    @custom_fwd(device_type="cuda")
     def forward(ctx, input, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1, deform_groups=1):
         _check_groups(groups, deform_groups)
         for name, t in (("input", input), ("offset", offset), ("mask", mask), ("weight", weight), ("bias", bias)):
             if t is not None and not t.is_cuda:
                 raise RuntimeError(f"{name} must be a CUDA tensor")
-            if t is not None and t.dtype != torch.float32:
-                raise TypeError(f"modulated_deform_conv2d: {name} must be float32 (got {t.dtype})")
+        cd = compute_dtype(input.dtype, offset.dtype, mask.dtype, weight.dtype, bias.dtype if bias is not None else None)
+        ctx.leaf_dtypes = tuple(t.dtype if t is not None else None for t in (input, offset, mask, weight, bias))
+        input, mask, weight = input.to(cd), mask.to(cd), weight.to(cd)
+        bias = bias.to(cd) if bias is not None else None
         geom = _geometry(input, weight, stride, padding, dilation)
         N, C, H, W, Ho, Wo, kh, kw = geom[:8]
         Cout = weight.shape[0]
@@ -99,53 +136,71 @@ class ModulatedDeformConv2dFunction(Function):
         b = bias.detach().contiguous() if bias is not None else None
         ctx.geom, ctx.with_bias = geom, bias is not None
         ctx.save_for_backward(x, off, msk, w2)
-        y = torch.empty((N * Ho * Wo, Cout), dtype=torch.float32, device=input.device)
+        y = torch.empty((N * Ho * Wo, Cout), dtype=cd, device=input.device)
         if N:
             scratch = _split_scratch(w2)
-            _columns_pass(x, off, msk, geom, lambda cols, rows, n0, nb: _gemm(cols, w2, b, y[rows], scratch))
+            with torch.autocast("cuda", enabled=False):
+                _columns_pass(x, off, msk, geom, lambda cols, rows, n0, nb: _gemm(cols, w2, b, y[rows], scratch))
         return y.view(N, Ho, Wo, Cout).permute(0, 3, 1, 2)                       # channels_last strides
 
     @staticmethod
+    @custom_bwd(device_type="cuda")
     @once_differentiable
     def backward(ctx, grad_output):
-        x, off, msk, w2 = ctx.saved_tensors
-        N, C, H, W, Ho, Wo, kh, kw = ctx.geom[:8]
-        Cout, Kc = w2.shape
-        need_x, need_off, need_mask, need_w = ctx.needs_input_grad[:4]
-        g = _lib.aligned(grad_output.permute(0, 2, 3, 1).contiguous().view(N * Ho * Wo, Cout))
-        gb = g.sum(0) if ctx.with_bias and ctx.needs_input_grad[4] else None
-        gw = torch.zeros_like(w2) if need_w else None
-        gx = go = gm = None
-        if need_x or need_off or need_mask:
-            gx = torch.zeros_like(x)
-            go = torch.empty_like(off)
-            gm = torch.empty_like(msk)
-        if N and (need_w or gx is not None):
-            wt = w2.t().contiguous()                                                  # [Kc, Cout]: grad_cols = g @ W'
-            scratch = _split_scratch(wt)
-            stream = _lib.stream_ptr(x.device)
+        with torch.autocast("cuda", enabled=False):
+            grads = _backward(ctx, grad_output)
+        return tuple(g.to(dt) if g is not None else None for g, dt in zip(grads, ctx.leaf_dtypes)) + (None,) * 5
 
-            def chunk(cols, rows, n0, nb):
-                gc = g[rows]
-                if gw is not None:
+
+def _backward(ctx, grad_output):
+    """(grad_input, grad_offset, grad_mask, grad_weight, grad_bias), each None where not needed: in fp32 for
+    cd = float32; for 16 bits grad_bias and grad_weight are fp32 sums and the sampling gradients come from col2im in
+    fp32."""
+    x, off, msk, w2 = ctx.saved_tensors
+    N, C, H, W, Ho, Wo, kh, kw = ctx.geom[:8]
+    Cout, Kc = w2.shape
+    half = w2.dtype != torch.float32
+    need_x, need_off, need_mask, need_w = ctx.needs_input_grad[:4]
+    g = _lib.aligned(grad_output.to(w2.dtype).permute(0, 2, 3, 1).contiguous().view(N * Ho * Wo, Cout))
+    gb = None
+    if ctx.with_bias and ctx.needs_input_grad[4]:
+        gb = g.sum(0, dtype=torch.float32) if half else g.sum(0)
+    gw = torch.zeros_like(w2, dtype=torch.float32) if need_w else None
+    gx = go = gm = None
+    if need_x or need_off or need_mask:
+        gx = torch.zeros_like(x, dtype=torch.float32)
+        go = torch.empty_like(off, dtype=torch.float32)
+        gm = torch.empty_like(msk, dtype=torch.float32)
+    if N and (need_w or gx is not None):
+        wt = w2 if half else w2.t().contiguous()                                  # fp32: [Kc, Cout], grad_cols = g @ W'
+        scratch = None if half else _split_scratch(wt)
+        stream = _lib.stream_ptr(x.device)
+
+        def chunk(cols, rows, n0, nb):
+            gc = g[rows]
+            if gw is not None:
+                if half:
+                    gw.add_(torch.mm(gc.t(), cols, out_dtype=torch.float32))          # cuBLAS, fp32 out
+                else:
                     gw.addmm_(gc.t(), cols)                                           # fp32 cuBLAS
-                if gx is not None:
-                    _gemm(gc, wt, None, cols, scratch)                                # grad_cols, in place of cols
-                    _lib.check(_lib.lib().vidar_dcn_col2im(
-                        _lib.ptr(x), _lib.ptr(off), _lib.ptr(msk), _lib.ptr(cols), _lib.ptr(gx), _lib.ptr(go),
-                        _lib.ptr(gm), *ctx.geom, n0, nb, stream))
+            if gx is not None:
+                if half:
+                    torch.mm(gc, wt, out=cols)                                        # grad_cols, in place of cols
+                else:
+                    _gemm(gc, wt, None, cols, scratch)
+                _col2im(x, off, msk, cols, gx, go, gm, ctx.geom, n0, nb, stream)
 
-            _columns_pass(x, off, msk, ctx.geom, chunk, recompute=need_w)
-        gw = gw.view(Cout, kh, kw, C).permute(0, 3, 1, 2).contiguous() if gw is not None else None
-        gx = gx.permute(0, 3, 1, 2) if need_x else None
-        return gx, go if need_off else None, gm if need_mask else None, gw, gb, None, None, None, None, None
+        _columns_pass(x, off, msk, ctx.geom, chunk, recompute=need_w)
+    gw = gw.view(Cout, kh, kw, C).permute(0, 3, 1, 2).contiguous() if gw is not None else None
+    gx = gx.permute(0, 3, 1, 2) if need_x else None
+    return gx, go if need_off else None, gm if need_mask else None, gw, gb
 
 
 def _split_scratch(w):
-    """Split-weight scratch of the 3xTF32 GEMM for weight `w` [Nout, K], or None when the GEMM runs on cuBLAS: shapes
-    the kernel does not take, and contractions longer than TC_MAX_K."""
+    """Split-weight scratch of the 3xTF32 GEMM for weight `w` [Nout, K], or None when the GEMM runs on cuBLAS: 16-bit
+    weights, shapes the kernel does not take, and contractions longer than TC_MAX_K."""
     Nout, K = w.shape
-    if not _tc.supported(K, Nout) or K > TC_MAX_K or torch.is_autocast_enabled():
+    if w.dtype != torch.float32 or not _tc.supported(K, Nout) or K > TC_MAX_K or torch.is_autocast_enabled():
         return None
     return torch.empty(2 * Nout * K, dtype=torch.float32, device=w.device)
 
@@ -155,18 +210,37 @@ def _columns_pass(x, off, msk, geom, fn, recompute=True):
     chunk written by vidar_dcn_im2col when `recompute` (else the buffer holds garbage for fn to overwrite)."""
     N, C, H, W, Ho, Wo, kh, kw = geom[:8]
     per_image = Ho * Wo * kh * kw * C
-    nb = chunk_images(N, per_image)
-    buf = torch.empty(nb * per_image, dtype=torch.float32, device=x.device)
+    nb = chunk_images(N, per_image, x.element_size())
+    buf = torch.empty(nb * per_image, dtype=x.dtype, device=x.device)
     stream = _lib.stream_ptr(x.device)
     with torch.cuda.device(x.device):
         for n0 in range(0, N, nb):
             b = min(nb, N - n0)
             cols = buf[: b * per_image].view(b * Ho * Wo, kh * kw * C)
             if recompute:
-                _lib.check(_lib.lib().vidar_dcn_im2col(_lib.ptr(x), _lib.ptr(off), _lib.ptr(msk), _lib.ptr(cols), *geom,
-                                                       n0, b, stream))
+                _im2col(x, off, msk, cols, geom, n0, b, stream)
             rows = slice(n0 * Ho * Wo, (n0 + b) * Ho * Wo)
             fn(cols, rows, n0, b)
+
+
+def _im2col(x, off, msk, cols, geom, n0, nb, stream):
+    L = _lib.lib()
+    if x.dtype == torch.float32:
+        rc = L.vidar_dcn_im2col(_lib.ptr(x), _lib.ptr(off), _lib.ptr(msk), _lib.ptr(cols), *geom, n0, nb, stream)
+    else:
+        rc = L.vidar_dcn_im2col_half(_lib.ptr(x), _lib.ptr(off), _lib.ptr(msk), _lib.ptr(cols),
+                                     HALF_DTYPE_CODES[x.dtype], *geom, n0, nb, stream)
+    _lib.check(rc)
+
+
+def _col2im(x, off, msk, grad_cols, gx, go, gm, geom, n0, nb, stream):
+    L = _lib.lib()
+    ptrs = [_lib.ptr(t) for t in (x, off, msk, grad_cols, gx, go, gm)]
+    if x.dtype == torch.float32:
+        rc = L.vidar_dcn_col2im(*ptrs, *geom, n0, nb, stream)
+    else:
+        rc = L.vidar_dcn_col2im_half(*ptrs, HALF_DTYPE_CODES[x.dtype], *geom, n0, nb, stream)
+    _lib.check(rc)
 
 
 def modulated_deform_conv2d(input, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1,

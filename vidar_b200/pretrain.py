@@ -270,11 +270,19 @@ def run_decoder(layers, query, prev, bev_pos, ref, bev_shapes, bev_lsi, group=No
 
 
 class SyntheticViDAR(nn.Module):
-    """The pre-training graph of ViDAR-RN101 (3 history frames, 3 future frames, 5 predicted head frames)."""
+    """The pre-training graph of ViDAR-RN101 (3 history frames, 3 future frames, 5 predicted head frames).
+
+    `backbone_autocast` = torch.float16 or torch.bfloat16 runs the backbone and FPN of `extract_feat` under
+    torch.autocast("cuda", dtype) and casts the FPN outputs to fp32 before the camera and level embeddings: what the
+    reference's `auto_fp16` on `extract_feat` and the `force_fp32` ops after it amount to in its fp16 mode.  The
+    default None runs everything in fp32.  The setting holds no state (the state_dict does not change)."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
-                 latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False):
+                 latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None):
         super().__init__()
+        if backbone_autocast not in (None, torch.float16, torch.bfloat16):
+            raise ValueError(f"backbone_autocast must be None, torch.float16 or torch.bfloat16 (got {backbone_autocast})")
+        self.backbone_autocast = backbone_autocast
         self.num_cams, self.future_frames, self.history_frames = num_cams, future_frames, history_frames
         self.bev_h, self.bev_w = bev_hw
         BEV_H, BEV_W = bev_hw          # noqa: N806  (shadows the module defaults below)
@@ -352,7 +360,12 @@ class SyntheticViDAR(nn.Module):
         per_cam = {}
         if mine:
             x = img[:, mine].reshape(bs * len(mine), *img.shape[2:])
-            outs = self.neck(self.backbone(x))
+            if self.backbone_autocast is None:
+                outs = self.neck(self.backbone(x))
+            else:
+                with torch.autocast("cuda", dtype=self.backbone_autocast):
+                    outs = self.neck(self.backbone(x))
+                outs = [f.float() for f in outs]
             for i, c in enumerate(mine):
                 lv = []
                 for lvl, f in enumerate(outs):
@@ -532,22 +545,30 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=synthetic.IMG_HW, rays_per
     return dict(img=img, lidar2img=lidar2img, gt_points=pts)
 
 
-def train_step(model, optimizer, sample, group=None, record=False):
+def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
     """forward_train + backward + gradient sync of the sharded parameters + clip(35) + AdamW step
-    (config :379-388).  -> (loss value tensor, [(stage, ms)] when `record`)."""
+    (config :379-388).  With a `torch.amp.GradScaler` (for a float16 `backbone_autocast`) the loss is scaled before
+    the backward and the gradients unscaled before the clip; the scaler skips a step whose gradients are not finite.
+    -> (loss value tensor, [(stage, ms)] when `record`)."""
     model.timings = [] if record else None
     if record:
         model._mark("start")
     optimizer.zero_grad(set_to_none=True)
     losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"])
     loss = sum(losses.values())
-    loss.backward()
+    (loss if scaler is None else scaler.scale(loss)).backward()
     model._mark("backward")
     if group is not None:
         sharding.allreduce_partial_grads(model, group)
         model._mark("grad_sync")
+    if scaler is not None:
+        scaler.unscale_(optimizer)
     torch.nn.utils.clip_grad_norm_([p for p in model.parameters() if p.requires_grad], 35.0)
-    optimizer.step()
+    if scaler is None:
+        optimizer.step()
+    else:
+        scaler.step(optimizer)
+        scaler.update()
     model._mark("optimizer")
     stages = None
     if record:
