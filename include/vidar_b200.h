@@ -568,6 +568,38 @@ int vidar_dcn_col2im_half(const void* x, const void* offset, const void* mask, c
                           int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int n0, int nb,
                           void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (viii) Deformable convolution v3 (InternImage's DCNv3 core op, ops_dcnv3 `dcnv3_forward` / `dcnv3_backward`).
+ *   `dtype` VIDAR_DTYPE_F32, _F16 or _BF16 is the storage type of every buffer but grad_input; anything else returns
+ *   VIDAR_E_INVALID ("unsupported dtype").  All arithmetic is fp32, each stored value is rounded once.
+ *   input   [N, H, W, group*group_channels]      channel-last
+ *   offset  [N, Ho, Wo, group*K*2]              (dx, dy) of kernel point p = i*kernel_h + j (i < kernel_w along x)
+ *   mask    [N, Ho, Wo, group*K]                weights (softmaxed by the caller), K = kernel_h*kernel_w
+ *   output  [N, Ho, Wo, group*group_channels]   fully overwritten
+ *   Ho = (H + 2*pad_h - (dilation_h*(kernel_h-1)+1)) / stride_h + 1, Wo likewise; both must be positive.
+ * Sample of (n, ho, wo, g, p), s = offset_scale, cw = (dilation_w*(kernel_w-1)) >> 1, ch likewise:
+ *   x = wo*stride_w - pad_w + cw + (i*dilation_w - cw + dx)*s,  y = ho*stride_h - pad_h + ch + (j*dilation_h - ch + dy)*s;
+ *   it adds mask * bilinear value (floor cell, corners outside the image read 0) when -1 < y < H and -1 < x < W.
+ * im2col_step > 0 and N % min(N, im2col_step) == 0 (the reference's rule); it does not change the computation.
+ * One launch each, on `stream`, no host sync.  Vector paths when group_channels is a multiple of 4 (fp32) / 8 (16-bit)
+ * and input, output / grad_output, grad_input are 16-byte aligned. */
+enum { VIDAR_DTYPE_F32 = 0 };  /* next to VIDAR_DTYPE_F16 = 1 and VIDAR_DTYPE_BF16 = 2 of the DCNv2 calls */
+int vidar_dcnv3_forward(const void* input, const void* offset, const void* mask, void* output, int dtype, int N, int H,
+                        int W, int group, int group_channels, int kernel_h, int kernel_w, int stride_h, int stride_w,
+                        int pad_h, int pad_w, int dilation_h, int dilation_w, float offset_scale, int im2col_step,
+                        void* stream);
+/* Backward from grad_output [N, Ho, Wo, group*group_channels] (dtype):
+ *   grad_input  [N, H, W, group*group_channels] fp32, caller-zeroed, accumulated (mask * corner weight * grad_out)
+ *   grad_offset [N, Ho, Wo, group*K*2] (dtype)  written: offset_scale * mask * sum_c grad_out * d v_c / d(x, y)
+ *   grad_mask   [N, Ho, Wo, group*K] (dtype)    written: sum_c grad_out * v_c
+ * d v / d(x, y) is the derivative of the bilinear form on the floor cell (one-sided on integer lines); a point
+ * outside the open range, one exactly on -1 included, gets 0 for every gradient. */
+int vidar_dcnv3_backward(const void* input, const void* offset, const void* mask, const void* grad_output,
+                         float* grad_input, void* grad_offset, void* grad_mask, int dtype, int N, int H, int W,
+                         int group, int group_channels, int kernel_h, int kernel_w, int stride_h, int stride_w,
+                         int pad_h, int pad_w, int dilation_h, int dilation_w, float offset_scale, int im2col_step,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif
