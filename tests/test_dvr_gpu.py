@@ -1,5 +1,6 @@
 """Parity of the CUDA ray-casters (through the C ABI) with the CPU oracle, BASELINE
-configs[0] (50x50x8, 1k rays) and a LiDAR-like 3-frame case.  pred/gt: 1e-5 relative (fp64
+configs[0] (50x50x8, 1k rays), a LiDAR-like 3-frame case and long 4x4xX grids on either side
+of the warp kernels' shared-memory budget.  pred/gt: 1e-5 relative (fp64
 internally on both sides, fp32 outputs); gradients: 1e-4 relative + fp32-atomic noise."""
 import numpy as np
 import pytest
@@ -25,10 +26,27 @@ def _close(a, b, what, rtol=1e-4, atol_scale=1e-5):
     assert (err <= tol).all(), f"{what}: max err {err.max():.3e} scale {scale:.3e}, {(err > tol).sum()} bad"
 
 
+def _long_x_grid(X, seed=21, M=320):
+    """A 4 x 4 x X grid (T = 1) on either side of the warp kernels' shared-memory budget.  They keep
+    cap = X + Y + Z + 8 records rounded up to 32, 20 B each, for 4 rays per block, and run only while
+    that is at most 200 KiB (csrc/dvr.cu, warp_ray_config).  X = 2544: cap 2560, 204 800 B, the last
+    size on the warp kernels.  X = 2545: cap 2592, 207 360 B, so every entry point runs one ray per
+    thread.  Integer, half-integer and outside-the-grid (x < 0) origins; end points spread along x,
+    so many rays close more than MAX_D = 1026 segments, which caps the lists and the fused backward."""
+    rng = np.random.default_rng(seed)
+    sigma = rng.uniform(0, 0.004, (1, 1, 4, 4, X)).astype(np.float32)
+    origin = np.array([[[3.0, 2.0, 1.0], [40.5, 1.5, 2.5], [-6.3, 1.7, 2.2]]], np.float32)
+    points = (rng.uniform(0, 1, (1, M, 3)) * np.array([X + 40, 6, 6]) - np.array([20, 1, 1])).astype(np.float32)
+    tindex = rng.integers(0, 3, (1, M)).astype(np.float32)
+    return sigma, origin, points, tindex
+
+
 CFG = [("cfg1-int", lambda: dvr_inputs_cfg1(seed=0, integer_origin=True)),
        ("cfg1-frac", lambda: dvr_inputs_cfg1(seed=0, integer_origin=False)),
        ("lidar-3f", lambda: dvr_inputs_lidar(M=3000, T=3, grid=(16, 200, 200), seed=1, pad=24)),
-       ("static-T1", lambda: (lambda s, o, p, t: (s[:, :1], o, p, t))(*dvr_inputs_lidar(M=900, T=3, grid=(8, 60, 50), seed=2)))]
+       ("static-T1", lambda: (lambda s, o, p, t: (s[:, :1], o, p, t))(*dvr_inputs_lidar(M=900, T=3, grid=(8, 60, 50), seed=2))),
+       ("long-x2544-warp", lambda: _long_x_grid(2544)),
+       ("long-x2545-thread", lambda: _long_x_grid(2545))]
 
 
 @pytest.mark.parametrize("name,make", CFG)

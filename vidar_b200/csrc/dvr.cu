@@ -8,9 +8,8 @@
 // operation order (float->int truncation of the origin, the -1:+1 / 0:+1 first-boundary
 // rule, strict-< tie order X<Y, X<Z, Y<Z else Z, the rounded "path" voxel of
 // render_forward/dvxlr, the consecutive-duplicate merge of dvxlr, termination rules),
-// so every branch decision of the thread-per-ray kernels (dvxlr family, and every ray that
-// starts outside the grid) equals the reference's.  The warp-per-ray kernels used by
-// dvr.render_forward / dvr.render compute crossing times as fma(i, tDelta, tMax0) instead of by
+// so every branch decision of the one-thread walk (serial_ray) equals the reference's.  The
+// warp-per-ray kernel computes crossing times as fma(i, tDelta, tMax0) instead of by
 // repeated addition and the rounded path voxel as round(fma(last, d, v0)): a decision can
 // differ from the reference's only when two crossing times (or a path coordinate and a .5
 // tie) agree to ~1e-13 relative.  Every step is therefore checked for such a near-tie (1e-9
@@ -29,8 +28,10 @@
 // S_0 before the first emission, so gradient kernels walk the ray twice (pass 1: pred,
 // S_0; pass 2: emit) instead of storing the path.  Gradients are accumulated with
 // red.global.add.f32 (the reference's `+=` at dvr.cu:622 is a data race).
-// Launch: 64-thread blocks (30k rays -> 469 blocks over 132 SMs; the reference's
-// 1024-thread blocks give 30 blocks), one ray per thread, neighbouring rays in a warp.
+// Launch (launch_rays): one ray per warp (render_warp_kernel, 4 rays per block) when a ray's
+// crossing records fit its shared-memory budget (warp_ray_config); otherwise, and always for
+// the lists of dvxlr.render / render_v2, one ray per thread (render_thread_kernel) in 64-thread
+// blocks (30k rays -> 469 blocks over 132 SMs; the reference's 1024-thread blocks give 30).
 #include <float.h>
 #include <math.h>
 
@@ -45,6 +46,25 @@ template <int V> struct Traits;
 template <> struct Traits<V_DVR_FWD>    { static constexpr bool kRounded = true;  static constexpr bool kMerge = false; static constexpr int kNegBoundary = -1; };
 template <> struct Traits<V_DVR_RENDER> { static constexpr bool kRounded = false; static constexpr bool kMerge = false; static constexpr int kNegBoundary = 0; };
 template <> struct Traits<V_DVXLR>      { static constexpr bool kRounded = true;  static constexpr bool kMerge = true;  static constexpr int kNegBoundary = -1; };
+
+// What a ray-caster call computes per ray; `mode` is the call's run-time option.
+//   M_FWD: pred, gt (`mode` = train phase)          M_LOSS_GRAD: dvr.render (`mode` = loss type)
+//   M_FUSED_BWD: fused backward of DifferentiableVoxelRendering[V2] (external grad_pred / grad_ray_pred)
+//   M_LISTS: pred, gt and the per-ray lists of dvxlr.render / render_v2
+enum Mode { M_FWD = 0, M_LOSS_GRAD = 1, M_FUSED_BWD = 2, M_LISTS = 3 };
+
+// The buffers of a call besides sigma / pred / gt / grad_sigma; what a mode does not use is nullptr.
+struct RayExtra {
+  int max_d;                   // M_FUSED_BWD, M_LISTS: list length (the MAX_D cap)
+  const float* grad_pred;      // M_FUSED_BWD: [N, M]
+  const float* grad_ray_pred;  // M_FUSED_BWD, v2: [N, M, max_d]
+  float* grad_sigma_regul;     // M_FUSED_BWD, v2: like sigma
+  float* dd_dsigma;            // M_LISTS: [N, M, max_d] or nullptr
+  float* indices;              // M_LISTS: [N, M, max_d, 3] or nullptr
+  float* ray_pred;             // M_LISTS, v2: [N, M, max_d]
+  float* indicator;            // M_LISTS, v2: [N, M, max_d]
+  const float* sigma_regul;    // M_LISTS, v2: like sigma
+};
 
 struct Grid {
   int N, M, T, To, Z, Y, X;
@@ -177,77 +197,73 @@ struct Segmenter {
   }
 };
 
-// Pass 1: expected distance, in the reference's summation order, plus S_0.
-struct Composite {
+// The transmittance recursion over a ray's segments, shared by both passes: step() hands
+// segment i (exit distance d) to `emit` as (i, R_i), R_i = sum_{k<i} T_k Delta_k, then
+// advances T_prev to T_i = exp(-csd_i).  After the last segment R = S_0.
+struct Transmittance {
   int count = 0;
-  double csd = 0.0, T_prev = 1.0, exp_d = 0.0, d_last = 0.0, S0 = 0.0;
-  __device__ __forceinline__ void commit(int, int, int, double sigma, double dt, double d) {
+  double csd = 0.0, T_prev = 1.0, d_last = 0.0, R = 0.0;
+  template <typename Emit>
+  __device__ __forceinline__ void step(double sigma, double dt, double d, Emit&& emit) {
+    if (count > 0) R += T_prev * (d - d_last);
+    emit(count, R);
     const double sd = sigma * dt;
-    const double csd_new = (count == 0) ? sd : csd + sd;
-    const double T_new = exp(-csd_new);
-    const double p = (count == 0) ? 1.0 - T_new : T_prev - T_new;
-    exp_d += p * d;
-    if (count > 0) S0 += T_prev * (d - d_last);
-    csd = csd_new;
-    T_prev = T_new;
+    csd = (count == 0) ? sd : csd + sd;
+    T_prev = exp(-csd);
     d_last = d;
     ++count;
+  }
+};
+
+// Pass 1: expected distance, in the reference's summation order, plus S_0.
+struct Composite : Transmittance {
+  double exp_d = 0.0;
+  __device__ __forceinline__ void commit(int, int, int, double sigma, double dt, double d) {
+    const double T_before = (count == 0) ? 1.0 : T_prev;   // p_0 = 1 - T_0
+    step(sigma, dt, d, [](int, double) {});
+    exp_d += (T_before - T_prev) * d;
   }
   // pred = sum p_i d_i + p_out * max_d   (dvr.cu:286-298)
   __device__ __forceinline__ double pred() const { return exp_d + T_prev * d_last; }
 };
 
-// Pass 2 sinks.  All see segment i with R_i = sum_{k<i} T_k Delta_k and emit
-// dd_i = -dt_i (S0 - R_i).
-struct ScatterSink {  // atomically add coef * dd_i into grad_sigma
+// Pass 2 sinks.  Each emits, for segment i, something of dd_i = -dt_i (S0 - R_i).
+struct ScatterSink : Transmittance {  // atomically add coef * dd_i into grad_sigma
   float* __restrict__ gsig;   // grad_sigma + frame offset
   const float* __restrict__ grp;  // grad_ray_pred row for this ray (v2) or nullptr
   float* __restrict__ gsreg;  // grad_sigma_regul + frame offset (v2) or nullptr
   int Y, X, max_d;
   double S0, coef;
   bool nan_to_zero;
-  int count = 0;
-  double csd = 0.0, T_prev = 1.0, d_last = 0.0, R = 0.0;
   __device__ __forceinline__ void commit(int x, int y, int z, double sigma, double dt, double d) {
-    if (count > 0) R += T_prev * (d - d_last);
-    const size_t vo = ((size_t)z * Y + y) * X + x;
-    if (count < max_d) {
+    step(sigma, dt, d, [&](int i, double R) {
+      if (i >= max_d) return;
+      const size_t vo = ((size_t)z * Y + y) * X + x;
       // float(dd) * float(coef) like `gradpred[..., None] * dd_dsigma` on fp32 tensors
       float g = (float)(-dt * (S0 - R)) * (float)coef;
       if (nan_to_zero && isnan(g)) g = 0.f;
       if (g != 0.f) red_add_f32(gsig + vo, g);
       if (grp) {
-        const float gr = grp[count];
+        const float gr = grp[i];
         if (gr != 0.f) red_add_f32(gsreg + vo, gr);
       }
-    }
-    const double sd = sigma * dt;
-    csd = (count == 0) ? sd : csd + sd;
-    T_prev = exp(-csd);
-    d_last = d;
-    ++count;
+    });
   }
 };
 
-struct RenderGradSink {  // dvr.render: grad_sigma += dl_dd * dd_i in fp64 then fp32 atomics
+struct RenderGradSink : Transmittance {  // dvr.render: grad_sigma += dl_dd * dd_i in fp64 then fp32 atomics
   float* __restrict__ gsig;
   int Y, X;
   double S0, dl_dd;
-  int count = 0;
-  double csd = 0.0, T_prev = 1.0, d_last = 0.0, R = 0.0;
   __device__ __forceinline__ void commit(int x, int y, int z, double sigma, double dt, double d) {
-    if (count > 0) R += T_prev * (d - d_last);
-    const float g = (float)(dl_dd * (-dt * (S0 - R)));
-    if (g != 0.f) red_add_f32(gsig + ((size_t)z * Y + y) * X + x, g);
-    const double sd = sigma * dt;
-    csd = (count == 0) ? sd : csd + sd;
-    T_prev = exp(-csd);
-    d_last = d;
-    ++count;
+    step(sigma, dt, d, [&](int, double R) {
+      const float g = (float)(dl_dd * (-dt * (S0 - R)));
+      if (g != 0.f) red_add_f32(gsig + ((size_t)z * Y + y) * X + x, g);
+    });
   }
 };
 
-struct ListSink {  // dvxlr.render: write the per-ray lists
+struct ListSink : Transmittance {  // dvxlr.render: write the per-ray lists
   float* __restrict__ dd;       // [max_d]
   float* __restrict__ idx;      // [max_d,3]
   float* __restrict__ ray_pred; // [max_d] or nullptr
@@ -256,29 +272,22 @@ struct ListSink {  // dvxlr.render: write the per-ray lists
   int Y, X, max_d;
   double S0, gt_raw;
   bool reached = false;
-  int count = 0;
-  double csd = 0.0, T_prev = 1.0, d_last = 0.0, R = 0.0;
   __device__ __forceinline__ void commit(int x, int y, int z, double sigma, double dt, double d) {
-    if (count > 0) R += T_prev * (d - d_last);
-    if (count < max_d) {
+    step(sigma, dt, d, [&](int i, double R) {
+      if (i >= max_d) return;
       if (dd) {
-        dd[count] = (float)(-dt * (S0 - R));
-        idx[count * 3 + 0] = (float)z;
-        idx[count * 3 + 1] = (float)y;
-        idx[count * 3 + 2] = (float)x;
+        dd[i] = (float)(-dt * (S0 - R));
+        idx[i * 3 + 0] = (float)z;
+        idx[i * 3 + 1] = (float)y;
+        idx[i * 3 + 2] = (float)x;
       }
       if (ray_pred) {
         float ind = 0.f;
         if (!reached && d >= gt_raw) { ind = 1.f; reached = true; }
-        indicator[count] = ind;
-        ray_pred[count] = __ldg(sreg + ((size_t)z * Y + y) * X + x);
+        indicator[i] = ind;
+        ray_pred[i] = __ldg(sreg + ((size_t)z * Y + y) * X + x);
       }
-    }
-    const double sd = sigma * dt;
-    csd = (count == 0) ? sd : csd + sd;
-    T_prev = exp(-csd);
-    d_last = d;
-    ++count;
+    });
   }
 };
 
@@ -300,60 +309,69 @@ __global__ void init_kernel(Grid G, const float* __restrict__ points,
     occ[((((size_t)n * G.T + ts) * G.Z + vz) * G.Y + vy) * G.X + vx] = 1.f;
 }
 
-// Forward only (dvr.render_forward; also the forward half of the fused autograd op).
-template <int V>
-__global__ void __launch_bounds__(kRayBlock)
-forward_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
-               const float* __restrict__ points, const float* __restrict__ tindex,
-               float* __restrict__ pred_dist, float* __restrict__ gt_dist, int clamp_gt) {
-  const int n = blockIdx.y;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= G.M) return;
-  const Ray r = load_ray(G, origin, points, tindex, n, c);
-  if (!r.ok) return;
-  const size_t vol = (size_t)G.Z * G.Y * G.X;
-  Composite comp;
-  Segmenter<Traits<V>::kMerge, Composite> seg(sigma + ((size_t)n * G.T + r.ts) * vol, G.Y, G.X, comp);
+// Walks the ray and hands its segments (merged for dvxlr) to `sink`.
+template <int V, typename Sink>
+__device__ __forceinline__ void walk_segments(const Grid& G, const Ray& r, const float* sig, Sink& sink) {
+  Segmenter<Traits<V>::kMerge, Sink> seg(sig, G.Y, G.X, sink);
   walk<V>(G, r, seg);
   seg.finish();
-  if (comp.count > 0) {
+}
+
+// One ray by one thread, bit-faithful: the body of render_thread_kernel and the fallback of
+// render_warp_kernel.  Pass 1 gives pred and S_0; the gradient and list modes walk the ray again.
+template <int V, int MODE>
+__device__ void serial_ray(const Grid& G, const Ray& r, const float* __restrict__ sigma,
+                           float* __restrict__ pred_dist, float* __restrict__ gt_dist,
+                           float* __restrict__ grad_sigma, int n, int c, int mode, const RayExtra& ex) {
+  const size_t vol = (size_t)G.Z * G.Y * G.X;
+  const size_t foff = ((size_t)n * G.T + r.ts) * vol;
+  const float* sg = sigma + foff;
+  Composite comp;
+  walk_segments<V>(G, r, sg, comp);
+  if (comp.count == 0) return;
+  const double exp_d = comp.pred();
+  const size_t ray = (size_t)n * G.M + c;
+  if constexpr (MODE == M_FUSED_BWD) {
+    const bool v2 = ex.grad_ray_pred != nullptr;
+    ScatterSink sink{{}, grad_sigma + foff, v2 ? ex.grad_ray_pred + ray * ex.max_d : nullptr,
+                     v2 ? ex.grad_sigma_regul + foff : nullptr, G.Y, G.X, ex.max_d, comp.R,
+                     (double)ex.grad_pred[ray], !v2};
+    walk_segments<V>(G, r, sg, sink);
+  } else {
     double gt = r.gt_d;
-    if (clamp_gt) gt = fmin(gt, comp.d_last);
-    pred_dist[(size_t)n * G.M + c] = (float)comp.pred();
-    gt_dist[(size_t)n * G.M + c] = (float)gt;
+    if (MODE == M_LOSS_GRAD || Traits<V>::kMerge || mode == 1) gt = fmin(gt, comp.d_last);
+    pred_dist[ray] = (float)exp_d;
+    gt_dist[ray] = (float)gt;
+    if constexpr (MODE == M_LOSS_GRAD) {   // dvr.cu:576-625
+      double dl_dd = 1.0;
+      if (mode == 0) dl_dd = (exp_d >= gt) ? 1 : -1;
+      else if (mode == 1) dl_dd = (exp_d - gt);
+      else if (mode == 2) dl_dd = (exp_d >= gt) ? (1.0 / gt) : -(1.0 / gt);
+      RenderGradSink sink{{}, grad_sigma + foff, G.Y, G.X, comp.R, dl_dd};
+      walk_segments<V>(G, r, sg, sink);
+    } else if constexpr (MODE == M_LISTS) {
+      const size_t row = ray * ex.max_d;
+      ListSink sink{{}, ex.dd_dsigma ? ex.dd_dsigma + row : nullptr, ex.indices ? ex.indices + row * 3 : nullptr,
+                    ex.ray_pred ? ex.ray_pred + row : nullptr, ex.indicator ? ex.indicator + row : nullptr,
+                    ex.sigma_regul ? ex.sigma_regul + foff : nullptr, G.Y, G.X, ex.max_d, comp.R, r.gt_d};
+      walk_segments<V>(G, r, sg, sink);
+    }
   }
 }
 
-// dvr.render: forward + loss gradient (L1 / L2 / AbsRel), dvr.cu:576-625.
+// One ray per thread: the lists (M_LISTS) always, every other mode when the warp kernel's
+// records do not fit in shared memory (launch_rays).
+template <int V, int MODE>
 __global__ void __launch_bounds__(kRayBlock)
-render_grad_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
-                   const float* __restrict__ points, const float* __restrict__ tindex,
-                   float* __restrict__ pred_dist, float* __restrict__ gt_dist,
-                   float* __restrict__ grad_sigma, int loss_type) {
+render_thread_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
+                     const float* __restrict__ points, const float* __restrict__ tindex,
+                     float* __restrict__ pred_dist, float* __restrict__ gt_dist,
+                     float* __restrict__ grad_sigma, int mode, RayExtra ex) {
   const int n = blockIdx.y;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= G.M) return;
   const Ray r = load_ray(G, origin, points, tindex, n, c);
-  if (!r.ok) return;
-  const size_t vol = (size_t)G.Z * G.Y * G.X;
-  const size_t foff = ((size_t)n * G.T + r.ts) * vol;
-  Composite comp;
-  {
-    Segmenter<false, Composite> seg(sigma + foff, G.Y, G.X, comp);
-    walk<V_DVR_RENDER>(G, r, seg);
-  }
-  if (comp.count == 0) return;
-  const double exp_d = comp.pred();
-  const double gt = fmin(r.gt_d, comp.d_last);
-  pred_dist[(size_t)n * G.M + c] = (float)exp_d;
-  gt_dist[(size_t)n * G.M + c] = (float)gt;
-  double dl_dd = 1.0;
-  if (loss_type == 0) dl_dd = (exp_d >= gt) ? 1 : -1;
-  else if (loss_type == 1) dl_dd = (exp_d - gt);
-  else if (loss_type == 2) dl_dd = (exp_d >= gt) ? (1.0 / gt) : -(1.0 / gt);
-  RenderGradSink sink{grad_sigma + foff, G.Y, G.X, comp.S0, dl_dd};
-  Segmenter<false, RenderGradSink> seg(sigma + foff, G.Y, G.X, sink);
-  walk<V_DVR_RENDER>(G, r, seg);
+  if (r.ok) serial_ray<V, MODE>(G, r, sigma, pred_dist, gt_dist, grad_sigma, n, c, mode, ex);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -377,10 +395,15 @@ render_grad_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
 // shared-memory budget take the serial code on lane 0.
 constexpr int kWarpRaysPerBlock = 4;
 
-__device__ __forceinline__ double warp_incl_scan(double v, int lane) {
+// relative distance below which two crossing times / a path coordinate and a .5 tie count as a near-tie
+// (render_warp_kernel): such rays take the serial traversal, whose decisions are the reference's
+constexpr double kTieEps = 1e-9;
+
+template <typename T>
+__device__ __forceinline__ T warp_incl_scan(T v, int lane) {
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
-    const double u = __shfl_up_sync(0xffffffffu, v, o);
+    const T u = __shfl_up_sync(0xffffffffu, v, o);
     if (lane >= o) v += u;
   }
   return v;
@@ -394,69 +417,35 @@ __device__ __forceinline__ int crossings_before(double T, double tMax0, double t
   return q >= (double)hi ? hi : (int)q;
 }
 
-// One ray by one thread, bit-faithful: the fallback of the warp-per-ray kernels.
-//   MODE 0: forward (pred, gt; `mode` = train phase)      MODE 1: dvr.render (loss gradient; `mode` = loss type)
-//   MODE 2: fused backward of DifferentiableVoxelRendering[V2] (external grad_pred / grad_ray_pred)
-template <int V, int MODE>
-__device__ void serial_ray(const Grid& G, const Ray& r, const float* __restrict__ sigma,
-                           float* __restrict__ pred_dist, float* __restrict__ gt_dist,
-                           float* __restrict__ grad_sigma, int n, int c, int mode,
-                           const float* __restrict__ grad_pred, const float* __restrict__ grad_ray_pred,
-                           float* __restrict__ grad_sigma_regul, int max_d) {
-  constexpr bool MERGE = Traits<V>::kMerge;
-  const size_t vol = (size_t)G.Z * G.Y * G.X;
-  const size_t foff = ((size_t)n * G.T + r.ts) * vol;
-  Composite comp;
-  {
-    Segmenter<MERGE, Composite> seg(sigma + foff, G.Y, G.X, comp);
-    walk<V>(G, r, seg);
-    seg.finish();
+// Merge variants (dvxlr): a run of consecutive records with the same (rounded) voxel is ONE segment --
+// length from the crossing before the run to the run's last crossing (dvxlr.cu:366-373) -- closed by
+// the run's last record.  run_head returns the head record of the run that lane's record belongs to
+// (a warp max-scan of the head flags) and carries it across chunks in `carry_head`.  It touches no
+// shared memory: with the record loads moved in here as well, the compiler lays out the whole warp
+// kernel differently (one more stack slot in render_warp_kernel<V_DVXLR, M_FWD>).
+__device__ __forceinline__ int run_head(bool head, int k, int lane, int& carry_head) {
+  int hs = head ? k : -1;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, hs, o);
+    if (lane >= o) hs = max(hs, u);
   }
-  if (comp.count == 0) return;
-  const double exp_d = comp.pred();
-  const size_t ray = (size_t)n * G.M + c;
-  if (MODE != 2) {
-    double gt = r.gt_d;
-    if (MODE == 1 || MERGE || mode == 1) gt = fmin(gt, comp.d_last);
-    pred_dist[ray] = (float)exp_d;
-    gt_dist[ray] = (float)gt;
-    if (MODE == 0) return;
-    double dl_dd = 1.0;
-    if (mode == 0) dl_dd = (exp_d >= gt) ? 1 : -1;
-    else if (mode == 1) dl_dd = (exp_d - gt);
-    else if (mode == 2) dl_dd = (exp_d >= gt) ? (1.0 / gt) : -(1.0 / gt);
-    RenderGradSink sink{grad_sigma + foff, G.Y, G.X, comp.S0, dl_dd};
-    Segmenter<MERGE, RenderGradSink> seg(sigma + foff, G.Y, G.X, sink);
-    walk<V>(G, r, seg);
-    seg.finish();
-  } else {
-    const bool v2 = grad_ray_pred != nullptr;
-    ScatterSink sink{grad_sigma + foff, v2 ? grad_ray_pred + ray * max_d : nullptr, v2 ? grad_sigma_regul + foff : nullptr,
-                     G.Y, G.X, max_d, comp.S0, (double)grad_pred[ray], !v2};
-    Segmenter<MERGE, ScatterSink> seg(sigma + foff, G.Y, G.X, sink);
-    walk<V>(G, r, seg);
-    seg.finish();
-  }
+  hs = max(hs, carry_head);
+  carry_head = __shfl_sync(0xffffffffu, hs, 31);
+  return hs;
 }
 
-// MODE as in serial_ray.  mode: MODE 1 ? loss_type : train_phase.  Merge variants (dvxlr): a run of
-// consecutive records with the same (rounded) voxel is ONE segment -- length from the crossing before the
-// run to the run's last crossing (dvxlr.cu:366-373) -- carried by the run's last record; run heads are
-// found with a warp max-scan, list ordinals (the MAX_D cap, grad_ray_pred slots) with an add-scan.
-struct WarpRayExtra {
-  const float* grad_pred;       // MODE 2: [N, M]
-  const float* grad_ray_pred;   // MODE 2, v2: [N, M, max_d] or nullptr
-  float* grad_sigma_regul;      // MODE 2, v2
-  int max_d;
-};
+// Every mode but M_LISTS; mode: M_LOSS_GRAD ? loss_type : train_phase.  Merge variants: a run's segment is
+// carried by its last record (run_head); list ordinals (the MAX_D cap, grad_ray_pred slots) come from an
+// add-scan of the tail flags.
 template <int V, int MODE>
 __global__ void __launch_bounds__(kWarpRaysPerBlock * 32)
 render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
                    const float* __restrict__ points, const float* __restrict__ tindex,
                    float* __restrict__ pred_dist, float* __restrict__ gt_dist,
-                   float* __restrict__ grad_sigma, int mode, int cap, double tie_eps, WarpRayExtra ex) {
+                   float* __restrict__ grad_sigma, int mode, int cap, RayExtra ex) {
   using TR = Traits<V>;
-  constexpr bool GRAD = MODE != 0;
+  constexpr bool GRAD = MODE != M_FWD;
   constexpr bool MERGE = TR::kMerge;
   extern __shared__ double smem_d[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -492,7 +481,7 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
   }
   eligible = eligible && bound > 0 && bound <= cap && isfinite(r.gt_d) && r.gt_d > 0;
   if (!eligible) {
-    if (lane == 0) serial_ray<V, MODE>(G, r, sigma, pred_dist, gt_dist, grad_sigma, n, c, mode, ex.grad_pred, ex.grad_ray_pred, ex.grad_sigma_regul, ex.max_d);
+    if (lane == 0) serial_ray<V, MODE>(G, r, sigma, pred_dist, gt_dist, grad_sigma, n, c, mode, ex);
     return;
   }
   // ---- phase 1: slices of the parameter range
@@ -513,14 +502,9 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
     nsteps += rem[a];
   }
   // exclusive scan of the per-lane step counts -> where this lane writes
-  int off = nsteps;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, off, o);
-    if (lane >= o) off += u;
-  }
-  const int N = __shfl_sync(0xffffffffu, off, 31);
-  off -= nsteps;
+  const int incl = warp_incl_scan(nsteps, lane);
+  const int N = __shfl_sync(0xffffffffu, incl, 31);
+  const int off = incl - nsteps;
   // Near-tie detection.  Crossing times here are fma(i, tDelta, tMax0); the reference adds tDelta i
   // times, so the two agree to ~1e-13 relative but not bit for bit.  That only matters where a branch
   // decision hangs on the last bits: two axes crossing at (almost) the same parameter, or -- rounded-path
@@ -549,7 +533,7 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
         if (a != ax && moves[a] && gi[a] < hi[a] && (gi[a] > 0 || gi[ax] > 0) &&
-            fabs(tm[a] - tcur) <= tie_eps * fabs(tcur))
+            fabs(tm[a] - tcur) <= kTieEps * fabs(tcur))
           tie = true;
       }
       const bool inside = v[0] >= 0 && v[0] < G.X && v[1] >= 0 && v[1] < G.Y && v[2] >= 0 && v[2] < G.Z;
@@ -560,9 +544,9 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
           const double cx = fma(last, r.dx, (double)r.vx0), cy = fma(last, r.dy, (double)r.vy0),
                        cz = fma(last, r.dz, (double)r.vz0);
           if (last > 0.0) {
-            tie = tie || fabs(fabs(cx - floor(cx)) - 0.5) <= tie_eps * fmax(1.0, fabs(cx)) ||
-                  fabs(fabs(cy - floor(cy)) - 0.5) <= tie_eps * fmax(1.0, fabs(cy)) ||
-                  fabs(fabs(cz - floor(cz)) - 0.5) <= tie_eps * fmax(1.0, fabs(cz));
+            tie = tie || fabs(fabs(cx - floor(cx)) - 0.5) <= kTieEps * fmax(1.0, fabs(cx)) ||
+                  fabs(fabs(cy - floor(cy)) - 0.5) <= kTieEps * fmax(1.0, fabs(cy)) ||
+                  fabs(fabs(cz - floor(cz)) - 0.5) <= kTieEps * fmax(1.0, fabs(cz));
           }
           px = (int)round(cx); px = px < G.X ? px : G.X - 1; px = px >= 0 ? px : 0;
           py = (int)round(cy); py = py < G.Y ? py : G.Y - 1; py = py >= 0 ? py : 0;
@@ -579,7 +563,7 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
     }
   }
   if (__any_sync(0xffffffffu, tie)) {
-    if (lane == 0) serial_ray<V, MODE>(G, r, sigma, pred_dist, gt_dist, grad_sigma, n, c, mode, ex.grad_pred, ex.grad_ray_pred, ex.grad_sigma_regul, ex.max_d);
+    if (lane == 0) serial_ray<V, MODE>(G, r, sigma, pred_dist, gt_dist, grad_sigma, n, c, mode, ex);
     return;
   }
   __syncwarp();
@@ -601,14 +585,7 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
     if (MERGE) {
       const bool head = ins && (k == 0 || vxs[k - 1] != idx);
       tail = ins && (k == N - 1 || vxs[k + 1] != idx);
-      hs = head ? k : -1;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, hs, o);
-        if (lane >= o) hs = max(hs, u);
-      }
-      hs = max(hs, carry_head);
-      carry_head = __shfl_sync(0xffffffffu, hs, 31);
+      hs = run_head(head, k, lane, carry_head);
       t0 = (hs > 0) ? ts[hs - 1] : 0.0;
     }
     const double dt = tail ? fmax(0.0, tk - t0) : 0.0;
@@ -635,8 +612,8 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
   }
   const double exp_d = pred_part + T_carry * d_last;    // + p_out * max_d
   double gt = r.gt_d;
-  if (MODE == 1 || MERGE || mode == 1) gt = fmin(gt, d_last);
-  if (MODE != 2 && lane == 0) {
+  if (MODE == M_LOSS_GRAD || MERGE || mode == 1) gt = fmin(gt, d_last);
+  if (MODE != M_FUSED_BWD && lane == 0) {
     pred_dist[(size_t)n * G.M + c] = (float)exp_d;
     gt_dist[(size_t)n * G.M + c] = (float)gt;
   }
@@ -644,13 +621,13 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
   // ---- phase 3: gradient emission, one record per lane
   const size_t ray = (size_t)n * G.M + c;
   double coef = 1.0;
-  if (MODE == 1) {
+  if (MODE == M_LOSS_GRAD) {
     if (mode == 0) coef = (exp_d >= gt) ? 1 : -1;
     else if (mode == 1) coef = (exp_d - gt);
     else if (mode == 2) coef = (exp_d >= gt) ? (1.0 / gt) : -(1.0 / gt);
   }
-  const float coef_f = (MODE == 2) ? __ldg(ex.grad_pred + ray) : 0.f;
-  const float* grp = (MODE == 2 && ex.grad_ray_pred) ? ex.grad_ray_pred + ray * ex.max_d : nullptr;
+  const float coef_f = (MODE == M_FUSED_BWD) ? __ldg(ex.grad_pred + ray) : 0.f;
+  const float* grp = (MODE == M_FUSED_BWD && ex.grad_ray_pred) ? ex.grad_ray_pred + ray * ex.max_d : nullptr;
   float* gs = grad_sigma + foff;
   float* gsr = grp ? ex.grad_sigma_regul + foff : nullptr;
   const double S0 = carry_U;
@@ -667,25 +644,18 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
     if (MERGE) {
       const bool head = ins && (k == 0 || vxs[k - 1] != idx);
       tail = ins && (k == N - 1 || vxs[k + 1] != idx);
-      int hs = head ? k : -1;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, hs, o);
-        if (lane >= o) hs = max(hs, u);
-      }
-      hs = max(hs, carry_head);
-      carry_head = __shfl_sync(0xffffffffu, hs, 31);
+      const int hs = run_head(head, k, lane, carry_head);
       t0 = (hs > 0) ? ts[hs - 1] : 0.0;
     }
-    int ord = 0;                                         // list slot of this segment (MODE 2: MAX_D cap, v2 slots)
-    if (MODE == 2) {
+    int ord = 0;                                         // list slot of this segment (MAX_D cap, v2 slots)
+    if (MODE == M_FUSED_BWD) {
       const unsigned tb = __ballot_sync(0xffffffffu, tail);
       ord = carry_ord + __popc(tb & ((1u << lane) - 1u));
       carry_ord += __popc(tb);
     }
     if (!tail) continue;
     const double dt = fmax(0.0, ts[k] - t0);
-    if (MODE == 1) {
+    if (MODE == M_LOSS_GRAD) {
       const float g = (float)(coef * (-dt * (S0 - us[k])));
       if (g != 0.f) red_add_f32(gs + idx, g);
     } else if (ord < ex.max_d) {
@@ -699,72 +669,6 @@ render_warp_kernel(Grid G, const float* __restrict__ sigma, const float* __restr
       }
     }
   }
-}
-
-// dvxlr.render / render_v2: forward + per-ray lists.
-__global__ void __launch_bounds__(kRayBlock)
-dvxlr_list_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
-                  const float* __restrict__ points, const float* __restrict__ tindex,
-                  const float* __restrict__ sigma_regul, float* __restrict__ pred_dist,
-                  float* __restrict__ gt_dist, float* __restrict__ dd_dsigma,
-                  float* __restrict__ indices, float* __restrict__ ray_pred,
-                  float* __restrict__ indicator, int max_d) {
-  const int n = blockIdx.y;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= G.M) return;
-  const Ray r = load_ray(G, origin, points, tindex, n, c);
-  if (!r.ok) return;
-  const size_t vol = (size_t)G.Z * G.Y * G.X;
-  const size_t foff = ((size_t)n * G.T + r.ts) * vol;
-  Composite comp;
-  {
-    Segmenter<true, Composite> seg(sigma + foff, G.Y, G.X, comp);
-    walk<V_DVXLR>(G, r, seg);
-    seg.finish();
-  }
-  if (comp.count == 0) return;
-  const size_t ray = (size_t)n * G.M + c;
-  pred_dist[ray] = (float)comp.pred();
-  gt_dist[ray] = (float)fmin(r.gt_d, comp.d_last);
-  ListSink sink{dd_dsigma ? dd_dsigma + ray * max_d : nullptr,
-                indices ? indices + ray * max_d * 3 : nullptr,
-                ray_pred ? ray_pred + ray * max_d : nullptr,
-                indicator ? indicator + ray * max_d : nullptr,
-                sigma_regul ? sigma_regul + foff : nullptr, G.Y, G.X, max_d, comp.S0, r.gt_d};
-  Segmenter<true, ListSink> seg(sigma + foff, G.Y, G.X, sink);
-  walk<V_DVXLR>(G, r, seg);
-  seg.finish();
-}
-
-// Fused backward of DifferentiableVoxelRendering[V2]: no lists.
-__global__ void __launch_bounds__(kRayBlock)
-dvxlr_fused_bwd_kernel(Grid G, const float* __restrict__ sigma, const float* __restrict__ origin,
-                       const float* __restrict__ points, const float* __restrict__ tindex,
-                       const float* __restrict__ grad_pred, const float* __restrict__ grad_ray_pred,
-                       float* __restrict__ grad_sigma, float* __restrict__ grad_sigma_regul,
-                       int max_d) {
-  const int n = blockIdx.y;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= G.M) return;
-  const Ray r = load_ray(G, origin, points, tindex, n, c);
-  if (!r.ok) return;
-  const size_t vol = (size_t)G.Z * G.Y * G.X;
-  const size_t foff = ((size_t)n * G.T + r.ts) * vol;
-  Composite comp;
-  {
-    Segmenter<true, Composite> seg(sigma + foff, G.Y, G.X, comp);
-    walk<V_DVXLR>(G, r, seg);
-    seg.finish();
-  }
-  if (comp.count == 0) return;
-  const size_t ray = (size_t)n * G.M + c;
-  const bool v2 = grad_ray_pred != nullptr;
-  ScatterSink sink{grad_sigma + foff, v2 ? grad_ray_pred + ray * max_d : nullptr,
-                   v2 ? grad_sigma_regul + foff : nullptr, G.Y, G.X, max_d, comp.S0,
-                   (double)grad_pred[ray], !v2};
-  Segmenter<true, ScatterSink> seg(sigma + foff, G.Y, G.X, sink);
-  walk<V_DVXLR>(G, r, seg);
-  seg.finish();
 }
 
 // dvxlr.get_grad_sigma[_v2]: one warp per ray, lanes stride over the list so reads are
@@ -832,12 +736,26 @@ bool warp_ray_config(const Grid& G, K kernel, int& cap, size_t& smem) {
   return true;
 }
 
-// relative distance below which two crossing times / a path coordinate and a .5 tie count as a near-tie
-// (render_warp_kernel): such rays take the serial traversal, whose decisions are the reference's
-constexpr double kTieEps = 1e-9;
-
 inline dim3 ray_grid(const Grid& G, int per_block) {
   return dim3((unsigned)((G.M + per_block - 1) / per_block), (unsigned)G.N);
+}
+
+// One ray per warp when the records fit (never for the lists), else one ray per thread.
+template <int V, int MODE>
+void launch_rays(const Grid& G, const float* sigma, const float* origin, const float* points,
+                 const float* tindex, float* pred_dist, float* gt_dist, float* grad_sigma, int mode,
+                 const RayExtra& ex, cudaStream_t stream) {
+  if constexpr (MODE != M_LISTS) {
+    int cap;
+    size_t smem;
+    if (warp_ray_config(G, render_warp_kernel<V, MODE>, cap, smem)) {
+      render_warp_kernel<V, MODE><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem, stream>>>(
+          G, sigma, origin, points, tindex, pred_dist, gt_dist, grad_sigma, mode, cap, ex);
+      return;
+    }
+  }
+  render_thread_kernel<V, MODE><<<ray_grid(G, kRayBlock), kRayBlock, 0, stream>>>(
+      G, sigma, origin, points, tindex, pred_dist, gt_dist, grad_sigma, mode, ex);
 }
 
 }  // namespace
@@ -868,16 +786,8 @@ extern "C" int vidar_dvr_render_forward(const float* sigma, const float* origin,
                 "dvr.render_forward: null pointer argument");
   VIDAR_REQUIRE(train_phase == 0 || train_phase == 1, "UNKNOWN PHASE NAME: %d", train_phase);
   if (M == 0) return VIDAR_OK;
-  int cap;
-  size_t smem;
-  if (warp_ray_config(G, render_warp_kernel<V_DVR_FWD, 0>, cap, smem)) {
-    render_warp_kernel<V_DVR_FWD, 0><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem,
-                                       (cudaStream_t)stream>>>(G, sigma, origin, points, tindex, pred_dist,
-                                                               gt_dist, nullptr, train_phase, cap, kTieEps, WarpRayExtra{});
-  } else {
-    forward_kernel<V_DVR_FWD><<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, pred_dist, gt_dist, train_phase);
-  }
+  launch_rays<V_DVR_FWD, M_FWD>(G, sigma, origin, points, tindex, pred_dist, gt_dist, nullptr, train_phase,
+                                RayExtra{}, (cudaStream_t)stream);
   return check_launch("dvr.render_forward");
 }
 
@@ -892,16 +802,8 @@ extern "C" int vidar_dvr_render(const float* sigma, const float* origin, const f
                 "dvr.render: null pointer argument");
   VIDAR_REQUIRE(loss_type >= 0 && loss_type <= 2, "UNKNOWN LOSS TYPE: %d", loss_type);
   if (M == 0) return VIDAR_OK;
-  int cap;
-  size_t smem;
-  if (warp_ray_config(G, render_warp_kernel<V_DVR_RENDER, 1>, cap, smem)) {
-    render_warp_kernel<V_DVR_RENDER, 1><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem,
-                                          (cudaStream_t)stream>>>(G, sigma, origin, points, tindex, pred_dist,
-                                                                  gt_dist, grad_sigma, loss_type, cap, kTieEps, WarpRayExtra{});
-  } else {
-    render_grad_kernel<<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, pred_dist, gt_dist, grad_sigma, loss_type);
-  }
+  launch_rays<V_DVR_RENDER, M_LOSS_GRAD>(G, sigma, origin, points, tindex, pred_dist, gt_dist, grad_sigma,
+                                        loss_type, RayExtra{}, (cudaStream_t)stream);
   return check_launch("dvr.render");
 }
 
@@ -914,16 +816,8 @@ extern "C" int vidar_dvxlr_forward(const float* sigma, const float* origin, cons
   VIDAR_REQUIRE(sigma && origin && points && tindex && pred_dist && gt_dist,
                 "dvxlr.forward: null pointer argument");
   if (M == 0) return VIDAR_OK;
-  int cap;
-  size_t smem;
-  if (warp_ray_config(G, render_warp_kernel<V_DVXLR, 0>, cap, smem)) {
-    // one ray per warp; consecutive records of one (rounded) voxel merge into a segment by a warp scan
-    render_warp_kernel<V_DVXLR, 0><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, pred_dist, gt_dist, nullptr, 1, cap, kTieEps, WarpRayExtra{});
-  } else {
-    forward_kernel<V_DVXLR><<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, pred_dist, gt_dist, 1);
-  }
+  launch_rays<V_DVXLR, M_FWD>(G, sigma, origin, points, tindex, pred_dist, gt_dist, nullptr, 1, RayExtra{},
+                              (cudaStream_t)stream);
   return check_launch("dvxlr.forward");
 }
 
@@ -944,9 +838,10 @@ extern "C" int vidar_dvxlr_render(const float* sigma, const float* origin, const
   VIDAR_REQUIRE(!v2 || (sigma_regul && ray_pred && indicator),
                 "dvxlr.render_v2: sigma_regul, ray_pred and indicator must all be given");
   if (M == 0) return VIDAR_OK;
-  dvxlr_list_kernel<<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
-      G, sigma, origin, points, tindex, sigma_regul, pred_dist, gt_dist, dd_dsigma, indices,
-      ray_pred, indicator, max_d);
+  launch_rays<V_DVXLR, M_LISTS>(G, sigma, origin, points, tindex, pred_dist, gt_dist, nullptr, 1,
+                                RayExtra{max_d, nullptr, nullptr, nullptr, dd_dsigma, indices, ray_pred,
+                                         indicator, sigma_regul},
+                                (cudaStream_t)stream);
   return check_launch("dvxlr.render");
 }
 
@@ -986,16 +881,8 @@ extern "C" int vidar_dvxlr_backward_fused(const float* sigma, const float* origi
                 "dvxlr.backward_fused: grad_ray_pred and grad_sigma_regul go together");
   VIDAR_REQUIRE(max_d > 0, "dvxlr.backward_fused: max_d must be positive");
   if (M == 0) return VIDAR_OK;
-  int cap;
-  size_t smem;
-  if (warp_ray_config(G, render_warp_kernel<V_DVXLR, 2>, cap, smem)) {
-    render_warp_kernel<V_DVXLR, 2><<<ray_grid(G, kWarpRaysPerBlock), kWarpRaysPerBlock * 32, smem, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, nullptr, nullptr, grad_sigma, 1, cap, kTieEps,
-        WarpRayExtra{grad_pred, grad_ray_pred, grad_sigma_regul, max_d});
-  } else {
-    dvxlr_fused_bwd_kernel<<<ray_grid(G, kRayBlock), kRayBlock, 0, (cudaStream_t)stream>>>(
-        G, sigma, origin, points, tindex, grad_pred, grad_ray_pred, grad_sigma, grad_sigma_regul,
-        max_d);
-  }
+  launch_rays<V_DVXLR, M_FUSED_BWD>(G, sigma, origin, points, tindex, nullptr, nullptr, grad_sigma, 1,
+                                    RayExtra{max_d, grad_pred, grad_ray_pred, grad_sigma_regul},
+                                    (cudaStream_t)stream);
   return check_launch("dvxlr.backward_fused");
 }
