@@ -101,6 +101,28 @@ int vidar_msda_sca_backward(const float* value, const int64_t* spatial_shapes,
                             float* grad_value, float* grad_offsets, float* grad_logits,
                             int B, int K, int H, int C, int L, int Q, int P, int D, void* stream);
 
+/* TemporalSelfAttention (temporal_self_attention.py:196-261) and the future decoder's deformable attention
+ *   (vidar_decoder.py:466-506) with their elementwise prologue and TSA's queue mean folded in.  G queue entries
+ *   per sample (TSA: num_bev_queue = 2; the decoder: 1):
+ *     attn = softmax_{L*P}(logits[b, q, h, g])
+ *     loc  = offsets[b, q, h, g, l, p] / (W_l, H_l) + ref_points[b*G + g, q, l]   (a true division, then an add)
+ *     out[b, q, h] = 1/G * sum_g  msda(value[b*G + g], loc, attn)[q, h]
+ *   value       [B*G, K, H, C]       queue entry g of sample b is value batch b*G + g
+ *   ref_points  [B*G, Q, L, 2]       normalised 2-D reference points, per level
+ *   offsets     [B, Q, H, G, L, P, 2]  raw output of the sampling_offsets Linear (pixels of level l)
+ *   logits      [B, Q, H, G, L*P]    raw output of the attention_weights Linear
+ *   out         [B, Q, H*C]          fully overwritten; the [B*G, Q, H*C] per-entry output never exists
+ * Requires L*P in {1, 2, 4, 8, 16, 32}, G*L*P <= 32 and head dim 16/32/64.
+ * Backward: grad_value [B*G, K, H, C] accumulated (caller zeroes), grad_offsets / grad_logits overwritten; the
+ * reference points carry no gradient. */
+int vidar_msda_tsa_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                           const float* ref_points, const float* offsets, const float* logits, float* out,
+                           int B, int G, int K, int H, int C, int L, int Q, int P, void* stream);
+int vidar_msda_tsa_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                            const float* ref_points, const float* offsets, const float* logits,
+                            const float* grad_out, float* grad_value, float* grad_offsets, float* grad_logits,
+                            int B, int G, int K, int H, int C, int L, int Q, int P, void* stream);
+
 /* Row-indirect variants: SpatialCrossAttention's rebatch / scatter-add (spatial_cross_attention.py:135-172)
  * folded into the op (SURVEY.md 8f-1).  A row is entry j of camera c's visible-pillar list:
  *   idx        [cams, Qd] int32   pillar of row j (ascending; entries >= count[c] unused), NULL: row j = pillar j

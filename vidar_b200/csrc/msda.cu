@@ -55,6 +55,12 @@ struct MsdaParams {
   const float* inv;    // [bs, Qd] output scale 1 / #cameras seeing the pillar, or nullptr
   int ncl, cam0, bs, Qd;   // cameras in this launch, first camera, batch size, pillars per batch element
   int S, s_lo, s_hi;   // the launch covers rows with (j / 64) % S in [s_lo, s_hi)   (rank sub-slices)
+  // Queue-mean prologue (SEG kernels: TemporalSelfAttention, the future decoder): an item (b, q, h) holds G segments
+  // of 2^seg_shift = L*P samples (LP = G*L*P).  Segment g samples value batch b*G + g, which lies g*Kv pixels past
+  // the item's slab (K = G*Kv); `loc` / `attn` hold the raw offsets / logits, `ref` is [B*G, Q, L, 2], and the
+  // output is the mean over g: the forward scales the weights, the backward grad_out, by qscale = 1/G.
+  int G, seg_shift, Kv;
+  float qscale;
 };
 
 // Decode one sample: pixel coordinates -> clamped base pixel, corner mask, fractions.
@@ -222,6 +228,39 @@ __device__ __forceinline__ void epi_decode(const MsdaParams& p, size_t refrow, i
   xy = epi_loc(off, Wl, Hl, r);
 }
 
+// SEG (TemporalSelfAttention, temporal_self_attention.py:196-261; the future decoder, vidar_decoder.py:466-506): the
+// softmax runs over aligned segments of 2^shift lanes, one (item, queue entry) each.  The butterfly goes from the
+// widest offset down, like warp_max / warp_sum and torch's warp softmax.  Every lane of the warp calls it (lanes
+// without a sample fill whole segments and pass a dummy logit).
+__device__ __forceinline__ float seg_max(float v, int shift) {
+  for (int o = (1 << shift) >> 1; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ float seg_sum(float v, int shift) {
+  for (int o = (1 << shift) >> 1; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float seg_softmax(float logit, int shift) {
+  const float e = expf(logit - seg_max(logit, shift));
+  return __fdiv_rn(e, seg_sum(e, shift));
+}
+// Sample sl (< G*L*P) of item (b, q, h), queue entry g = sl / (L*P) at level l: its location offsets / (W_l, H_l) +
+// ref[b*G + g, q, l] (epi_loc's order), its level's size and the level's start inside the item's G-batch slab.
+// `off` points at the sample's two raw offsets.
+__device__ __forceinline__ void seg_decode(const MsdaParams& p, long long item, int sl, const float* off,
+                                           float2& xy, int& start, int& Hl, int& Wl) {
+  const int g = sl >> p.seg_shift;
+  const int l = (sl & ((1 << p.seg_shift) - 1)) / p.P;
+  Hl = (int)__ldg(p.shapes + 2 * l);
+  Wl = (int)__ldg(p.shapes + 2 * l + 1);
+  const unsigned bq = (unsigned)item / (unsigned)p.H;
+  const unsigned b = bq / (unsigned)p.Q, q = bq - b * (unsigned)p.Q;
+  const size_t refrow = (((size_t)b * p.G + g) * p.Q + q) * p.L + l;
+  xy = epi_loc(__ldg(reinterpret_cast<const float2*>(off)), (float)Wl, (float)Hl,
+               __ldg(reinterpret_cast<const float2*>(p.ref) + refrow));
+  start = (int)__ldg(p.lsi + l) + g * p.Kv;
+}
+
 // Which (b,q,h) items does this warp own?  Returns false if none.
 //  ipw == 1 : block = 8 consecutive queries of one (b,h); blocks ordered (b, h, qtile).
 //  ipw  > 1 : ipw consecutive items in memory order (heads of the same query first).
@@ -316,8 +355,10 @@ __device__ __forceinline__ void store_item(const MsdaParams& p, float* __restric
 
 // MULTI = several items per warp (L*P a power of two < 32, one 32-sample chunk).
 // EPI = fused softmax / sampling-location epilogue (L*P == 32, !MULTI only).
+// SEG = the queue-mean prologue (G*L*P <= 32 samples per item, MULTI or not): softmax per segment, locations from
+// the raw offsets, the G value batches of an item in one slab, the output scaled by 1/G.
 // 6 blocks (48 warps) per SM: the register cap (42) is what the tuned round-1 kernel used (40)
-template <int CV, bool MULTI, bool EPI = false, bool IDX = false>
+template <int CV, bool MULTI, bool EPI = false, bool IDX = false, bool SEG = false>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 6)
 msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
   // The streaming hint (kStreamBytes, ldg4_na) applies to this kernel without IDX and nowhere else.  The backward
@@ -353,7 +394,19 @@ msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
     int base = 0, meta = 0;
     float w1 = 0.f, w2 = 0.f, w3 = 0.f, w4 = 0.f;
     const bool live = MULTI ? (item0 + (s >> p.lp_shift) < p.items) : (s < span);
-    if (live) {
+    // SEG: the softmax is a segment-wide reduction, so every lane takes part
+    const float sw = SEG ? seg_softmax(live ? __ldg(att0 + s) : 0.f, p.seg_shift) : 0.f;
+    if (SEG && live) {
+      int Hl, Wl, start;
+      float2 xy;
+      seg_decode(p, MULTI ? item0 + (s >> p.lp_shift) : item0, MULTI ? (s & (p.LP - 1)) : s, loc0 + 2 * s, xy, start,
+                 Hl, Wl);
+      float lh, lw;
+      decode_sample(xy.x, xy.y, Hl, Wl, start, base, meta, lh, lw, p.pix_stride);
+      if (NA && meta && (unsigned)(Hl * Wl) * (unsigned)p.C * 4u > kStreamBytes) meta |= kHintBit;
+      // the mean over the queue, folded into the weights (exact when G is a power of two)
+      corner_weights(meta, lh, lw, __fmul_rn(sw, p.qscale), w1, w2, w3, w4);
+    } else if (!SEG && live) {
       const int sl = MULTI ? (s & (p.LP - 1)) : s;
       const int l = sl / p.P;
       const int Hl = (int)__ldg(p.shapes + 2 * l), Wl = (int)__ldg(p.shapes + 2 * l + 1);
@@ -415,7 +468,7 @@ msda_forward_kernel(const MsdaParams p, float* __restrict__ out) {
 }
 
 // 4 blocks (32 warps) per SM = 64 registers, the round-1 operating point
-template <int CV, bool MULTI, bool EPI = false, bool IDX = false>
+template <int CV, bool MULTI, bool EPI = false, bool IDX = false, bool SEG = false>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 4)
 msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
                      float* __restrict__ grad_value, float* __restrict__ grad_loc,
@@ -443,6 +496,7 @@ msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
   // IDX: grad_out is the gradient of the BEV slot grid; the row's share is slot[pillar] / count
   if (!MULTI) go = IDX ? f4_scale(row.inv, ldg4(grad_out + (size_t)row.dense * p.C + cl * 4))
                        : ldg4(grad_out + (size_t)item0 * p.C + cl * 4);
+  if (SEG && !MULTI) go = f4_scale(p.qscale, go);   // through the mean over the queue
 
   for (int chunk = 0; chunk < nchunks; ++chunk) {
     const int s = chunk * 32 + lane;
@@ -450,18 +504,27 @@ msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
     float lh = 0.f, lw = 0.f, aw = 0.f, fH = 0.f, fW = 0.f;
     float w1 = 0.f, w2 = 0.f, w3 = 0.f, w4 = 0.f;
     const bool live = MULTI ? (item0 + (s >> p.lp_shift) < p.items) : (s < span);
+    const float sw = SEG ? seg_softmax(live ? __ldg(att0 + s) : 0.f, p.seg_shift) : 0.f;
     if (live) {
       const int sl = MULTI ? (s & (p.LP - 1)) : s;
-      const int l = sl / p.P;
-      const int Hl = (int)__ldg(p.shapes + 2 * l), Wl = (int)__ldg(p.shapes + 2 * l + 1);
+      int Hl, Wl, start;
       float2 xy;
-      if (EPI) {
-        epi_decode(p, row.refrow, s, (float)Wl, (float)Hl, loc0, att0, xy, aw);
+      if (SEG) {
+        seg_decode(p, MULTI ? item0 + (s >> p.lp_shift) : item0, sl, loc0 + 2 * s, xy, start, Hl, Wl);
+        aw = sw;
       } else {
-        xy = __ldg(reinterpret_cast<const float2*>(loc0) + s);
-        aw = __ldg(att0 + s);
+        const int l = sl / p.P;
+        Hl = (int)__ldg(p.shapes + 2 * l);
+        Wl = (int)__ldg(p.shapes + 2 * l + 1);
+        if (EPI) {
+          epi_decode(p, row.refrow, s, (float)Wl, (float)Hl, loc0, att0, xy, aw);
+        } else {
+          xy = __ldg(reinterpret_cast<const float2*>(loc0) + s);
+          aw = __ldg(att0 + s);
+        }
+        start = (int)__ldg(p.lsi + l);
       }
-      decode_sample(xy.x, xy.y, Hl, Wl, (int)__ldg(p.lsi + l), base, meta, lh, lw, p.pix_stride);
+      decode_sample(xy.x, xy.y, Hl, Wl, start, base, meta, lh, lw, p.pix_stride);
       fH = (float)Hl;
       fW = (float)Wl;
       corner_weights(meta, lh, lw, aw, w1, w2, w3, w4);
@@ -482,6 +545,7 @@ msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
         if (item < p.items) {
           slab = slab_offset(p, item) + cl * 4;
           go = ldg4(grad_out + (size_t)item * p.C + cl * 4);
+          if (SEG) go = f4_scale(p.qscale, go);
         } else {
           go = f4_zero();
         }
@@ -509,7 +573,17 @@ msda_backward_kernel(const MsdaParams p, const float* __restrict__ grad_out,
       if ((lane / NG) == it) r = t;
     }
     // ---- every lane finishes its own sample; coalesced stores
-    if (live) {
+    if (SEG) {
+      // grad_off = grad_loc / (W,H); grad_logit = w * (grad_w - sum_j w_j grad_w_j) over the sample's segment, a
+      // reduction every lane takes part in (without a sample: meta = 0 and aw = 0, so ga = 0)
+      float ga, gx, gy;
+      sample_grads(meta, lh, lw, aw, fW, fH, r, ga, gx, gy);
+      const float dot = seg_sum(aw * ga, p.seg_shift);
+      if (live) {
+        gatt0[s] = aw * (ga - dot);
+        reinterpret_cast<float2*>(gloc0)[s] = make_float2(__fdiv_rn(gx, fW), __fdiv_rn(gy, fH));
+      }
+    } else if (live) {
       float ga, gx, gy;
       sample_grads(meta, lh, lw, aw, fW, fH, r, ga, gx, gy);
       if (EPI) {
@@ -1143,6 +1217,7 @@ int fill_params(MsdaParams& p, const float* value, const int64_t* shapes, const 
   p.idx = nullptr; p.count = nullptr; p.inv = nullptr;
   p.ncl = B; p.cam0 = 0; p.bs = 1; p.Qd = Q;
   p.S = 1; p.s_lo = 0; p.s_hi = 1;
+  p.G = 1; p.seg_shift = 0; p.Kv = K; p.qscale = 1.f;
   return VIDAR_OK;
 }
 
@@ -1229,23 +1304,33 @@ void with_cv(int C, const F& f) {
 // The forward of every entry point, once its arguments are checked.  The plain op (!EPI && !IDX) takes the generic
 // kernel at head widths the vector kernels do not support (the fused epilogue and the row map require them), and
 // packs several items into a warp when L*P is small (set_ipw): the small kernel once every lane group gets an item
-// of its own, MULTI below that.  The row map (IDX) keeps fill_rows' one item per warp.
-template <bool EPI, bool IDX>
+// of its own, MULTI below that.  The row map (IDX) keeps fill_rows' one item per warp.  The queue-mean prologue
+// (SEG) packs items like the plain op, below head dim 64, but always into msda_forward_kernel, MULTI or not.
+template <bool EPI, bool IDX, bool SEG = false>
 int msda_forward(MsdaParams& p, float* out, cudaStream_t st, const char* who) {
   VIDAR_REQUIRE(out, "%s: null output", who);
-  if (!EPI && !IDX && !vec_ok(p)) {
+  if (!EPI && !IDX && !SEG && !vec_ok(p)) {
     const long long nb = (p.items * p.C + 255) / 256;
     VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
     msda_forward_generic_kernel<<<(unsigned)nb, 256, 0, st>>>(p, out);
     return check_launch(who);
   }
   if (!IDX) set_ipw(p, p.C / 4);
+  if (SEG && p.C == 64) p.ipw = 1;   // one item per warp: the MULTI forward spills at head dim 64
   const long long nb = num_blocks(p);
   VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
   const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
   with_cv(p.C, [&](auto cv) {
     constexpr int CV = decltype(cv)::value;
-    if constexpr (!EPI && !IDX) {
+    if constexpr (SEG) {
+      if constexpr (CV < 16) {
+        if (p.ipw > 1) {
+          msda_forward_kernel<CV, true, false, false, true><<<grid, block, 0, st>>>(p, out);
+          return;
+        }
+      }
+      msda_forward_kernel<CV, false, false, false, true><<<grid, block, 0, st>>>(p, out);
+    } else if constexpr (!EPI && !IDX) {
       if (p.ipw >= 32 / CV) msda_forward_small_kernel<CV><<<grid, block, 0, st>>>(p, out);
       else if (p.ipw > 1) msda_forward_kernel<CV, true><<<grid, block, 0, st>>>(p, out);
       else msda_forward_kernel<CV, false><<<grid, block, 0, st>>>(p, out);
@@ -1258,13 +1343,13 @@ int msda_forward(MsdaParams& p, float* out, cudaStream_t st, const char* who) {
 
 // The backward of every entry point, once its arguments are checked: the kernels the forward picks, or the tile
 // kernel for the row map where tile_backward_ok.
-template <bool EPI, bool IDX>
+template <bool EPI, bool IDX, bool SEG = false>
 int msda_backward(MsdaParams& p, const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
                   cudaStream_t st, const char* who) {
   VIDAR_REQUIRE(grad_out && grad_value && grad_loc && grad_attn, "%s: null gradient pointer", who);
   if (IDX && tile_backward_ok(p))
     return launch_rows_backward_tiled<EPI>(p, grad_out, grad_value, grad_loc, grad_attn, st, who);
-  if (!EPI && !IDX && !vec_ok(p)) {
+  if (!EPI && !IDX && !SEG && !vec_ok(p)) {
     cudaError_t e = cudaMemsetAsync(grad_loc, 0, sizeof(float) * 2 * (size_t)p.items * p.LP, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(grad_attn, 0, sizeof(float) * (size_t)p.items * p.LP, st);
     if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "%s: memset: %s", who, cudaGetErrorString(e));
@@ -1274,12 +1359,23 @@ int msda_backward(MsdaParams& p, const float* grad_out, float* grad_value, float
     return check_launch(who);
   }
   if (!IDX) set_ipw(p, p.C / 4);
+  if (SEG && p.C == 64) p.ipw = 1;   // one item per warp: the MULTI forward spills at head dim 64
   const long long nb = num_blocks(p);
   VIDAR_REQUIRE(nb < 2147483647LL, "%s: problem too large", who);
   const dim3 grid((unsigned)nb), block(kWarpsPerBlock * 32);
   with_cv(p.C, [&](auto cv) {
     constexpr int CV = decltype(cv)::value;
-    if constexpr (!EPI && !IDX) {
+    if constexpr (SEG) {
+      if constexpr (CV < 16) {
+        if (p.ipw > 1) {
+          msda_backward_kernel<CV, true, false, false, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc,
+                                                                                     grad_attn);
+          return;
+        }
+      }
+      msda_backward_kernel<CV, false, false, false, true><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc,
+                                                                                  grad_attn);
+    } else if constexpr (!EPI && !IDX) {
       if (p.ipw >= 32 / CV)
         msda_backward_small_kernel<CV><<<grid, block, 0, st>>>(p, grad_out, grad_value, grad_loc, grad_attn);
       else if (p.ipw > 1)
@@ -1361,6 +1457,57 @@ extern "C" int vidar_msda_sca_backward(const float* value, const int64_t* spatia
   rc = check_sca(p, ref_points, D, who);
   if (rc) return rc;
   return msda_backward<true, false>(p, grad_out, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream, who);
+}
+
+// ---- TemporalSelfAttention / the future decoder's deformable attention with the softmax, the sampling-location
+// arithmetic and TSA's mean over the queue folded in: items are (b, q, h) of the output, each with G*L*P samples
+static int check_tsa(MsdaParams& p, const float* ref, int G, const char* who) {
+  VIDAR_REQUIRE(ref, "%s: null reference points", who);
+  const int LP = p.LP;
+  VIDAR_REQUIRE(LP <= 32 && (LP & (LP - 1)) == 0,
+                "%s: the fused prologue needs num_levels * num_points in {1, 2, 4, 8, 16, 32} (got %d)", who, LP);
+  VIDAR_REQUIRE(G > 0 && G <= 32 / LP, "%s: num_queue * num_levels * num_points must be at most 32 (got %d x %d)",
+                who, G, LP);
+  VIDAR_REQUIRE(p.C == 16 || p.C == 32 || p.C == 64, "%s: head dim must be 16, 32 or 64 (got %d)", who, p.C);
+  // the G value batches of an item are one slab addressed with 32-bit offsets
+  VIDAR_REQUIRE((long long)G * p.K * p.H * p.C < (1LL << 25), "%s: problem too large", who);
+  p.Kv = p.K;
+  p.K = G * p.K;
+  VIDAR_REQUIRE(vec_ok(p), "%s: problem too large", who);
+  p.G = G;
+  p.seg_shift = 0;
+  while ((1 << p.seg_shift) < LP) ++p.seg_shift;
+  p.LP = G * LP;
+  p.qscale = 1.f / (float)G;
+  p.ref = ref;
+  return VIDAR_OK;
+}
+
+extern "C" int vidar_msda_tsa_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const float* ref_points, const float* offsets, const float* logits, float* out,
+                                      int B, int G, int K, int H, int C, int L, int Q, int P, void* stream) {
+  const char* who = "msda_tsa_forward";
+  MsdaParams p;
+  int rc = fill_params(p, value, spatial_shapes, level_start, offsets, logits, B, K, H, C, L, Q, P, B, who);
+  if (rc) return rc;
+  rc = check_tsa(p, ref_points, G, who);
+  if (rc) return rc;
+  return msda_forward<false, false, true>(p, out, (cudaStream_t)stream, who);
+}
+
+extern "C" int vidar_msda_tsa_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                       const float* ref_points, const float* offsets, const float* logits,
+                                       const float* grad_out, float* grad_value, float* grad_offsets,
+                                       float* grad_logits, int B, int G, int K, int H, int C, int L, int Q, int P,
+                                       void* stream) {
+  const char* who = "msda_tsa_backward";
+  MsdaParams p;
+  int rc = fill_params(p, value, spatial_shapes, level_start, offsets, logits, B, K, H, C, L, Q, P, B, who);
+  if (rc) return rc;
+  rc = check_tsa(p, ref_points, G, who);
+  if (rc) return rc;
+  return msda_backward<false, false, true>(p, grad_out, grad_value, grad_offsets, grad_logits, (cudaStream_t)stream,
+                                           who);
 }
 
 // ---- row-indirect entry points: SpatialCrossAttention's rebatch / scatter-add fused into the op ------

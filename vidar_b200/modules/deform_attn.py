@@ -11,8 +11,10 @@ classes, so the reference's config dicts build them and released checkpoints loa
   CustomMSDeformableAttention      decoder.py:132-345   (detection decoder, fine-tuning only)
 (paths under projects/mmdet3d_plugin/bevformer/modules/ of the reference).
 
-Every sampling step goes through `msda_apply` = MultiScaleDeformableAttnFunction_fp32.apply,
-the CUDA op in vidar_b200/csrc/msda.cu.  There is no PyTorch fallback branch (the
+Every sampling step runs the CUDA op in vidar_b200/csrc/msda.cu: `msda_apply` =
+MultiScaleDeformableAttnFunction_fp32.apply around the reference's statements, or by default (`fuse_epilogue`) a
+Function that takes the raw offsets / logits and runs the softmax and the sampling-location arithmetic (and
+TemporalSelfAttention's queue mean) inside the kernel.  There is no PyTorch fallback branch (the
 reference falls back to `multi_scale_deformable_attn_pytorch` on CPU tensors,
 spatial_cross_attention.py:392-394): CPU tensors raise.
 """
@@ -23,11 +25,12 @@ import torch
 import torch.nn as nn
 
 from .. import linear as _tc
-from ..msda import MSDeformAttn3DFusedFunction, MultiScaleDeformableAttnFunction_fp32
+from ..msda import MSDeformAttn3DFusedFunction, MSDeformAttnQueueFusedFunction, MultiScaleDeformableAttnFunction_fp32
 from ..registry import ATTENTION, BaseModule, build_attention, constant_init, xavier_init
 
 msda_apply = MultiScaleDeformableAttnFunction_fp32.apply
 msda3d_fused_apply = MSDeformAttn3DFusedFunction.apply
+msda_queue_fused_apply = MSDeformAttnQueueFusedFunction.apply
 
 
 TC_LINEAR = True      # Linear layers of these modules on the tensor cores (3xTF32, vidar_b200/linear.py) when the shape allows
@@ -61,6 +64,30 @@ def _ring_offsets(num_heads, num_groups, num_points):
     radius = torch.arange(1, num_points + 1, dtype=torch.float32)
     g = d.view(num_heads, 1, 1, 2) * radius.view(1, 1, num_points, 1)
     return g.expand(num_heads, num_groups, num_points, 2).reshape(-1).clone()
+
+
+def _queue_fusable(module, value, reference_points, offsets, logits, num_queue):
+    """Does TemporalSelfAttention / PredictionMSDeformableAttention take the fused op?  fp32 CUDA tensors outside
+    autocast, 2-D reference points and a shape the kernel takes; otherwise (CPU tensors, 4-D box reference points,
+    autocast) the reference's statements run around the plain op."""
+    if not (module.fuse_epilogue and value.is_cuda and reference_points.shape[-1] == 2
+            and not torch.is_autocast_enabled()):
+        return False
+    if any(t.dtype != torch.float32 for t in (value, reference_points, offsets, logits)):
+        return False
+    BG, num_value, H, C = value.shape
+    if tuple(reference_points.shape) != (BG, offsets.shape[1], module.num_levels, 2):
+        return False
+    return MSDeformAttnQueueFusedFunction.supported(module.num_levels, module.num_points, num_queue, C, num_value, H)
+
+
+def _check_num_value(module, spatial_shapes, num_value):
+    """The reference's `assert sum(H_l * W_l) == num_value`.  With the fused path enabled and the shapes on the GPU it
+    is a device-side assert, so the step never waits for the GPU."""
+    if module.fuse_epilogue and spatial_shapes.is_cuda:
+        torch._assert_async((spatial_shapes[:, 0] * spatial_shapes[:, 1]).sum() == num_value)
+    else:
+        assert (spatial_shapes[:, 0] * spatial_shapes[:, 1]).sum() == num_value
 
 
 def _wh(spatial_shapes):
@@ -345,6 +372,7 @@ class TemporalSelfAttention(BaseModule):
                                            num_bev_queue * num_heads * num_levels * num_points)
         self.value_proj = nn.Linear(embed_dims, embed_dims)
         self.output_proj = nn.Linear(embed_dims, embed_dims)
+        self.fuse_epilogue = True      # False: materialise sampling_locations / attention_weights like the reference
         self.init_weights()
 
     def init_weights(self):
@@ -376,7 +404,7 @@ class TemporalSelfAttention(BaseModule):
             query, value = query.permute(1, 0, 2), value.permute(1, 0, 2)
         bs, num_query, embed_dims = query.shape
         num_value = value.shape[1]
-        assert (spatial_shapes[:, 0] * spatial_shapes[:, 1]).sum() == num_value
+        _check_num_value(self, spatial_shapes, num_value)
         assert self.num_bev_queue == 2
         H, L, P, Qn = self.num_heads, self.num_levels, self.num_points, self.num_bev_queue
 
@@ -390,8 +418,21 @@ class TemporalSelfAttention(BaseModule):
         value = value.reshape(bs * Qn, num_value, H, -1)
 
         offsets = self.sampling_offsets(query).view(bs, num_query, H, Qn, L, P, 2)
-        weights = self.attention_weights(query).view(bs, num_query, H, Qn, L * P).softmax(-1)
-        weights = weights.view(bs, num_query, H, Qn, L, P)
+        logits = self.attention_weights(query).view(bs, num_query, H, Qn, L * P)
+        if _queue_fusable(self, value, reference_points, offsets, logits, Qn):
+            # softmax, sampling locations and the mean over the queue run inside the kernel
+            output = msda_queue_fused_apply(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
+        else:
+            output = self._sample(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
+        output = _linear(self.output_proj, output)
+        if not self.batch_first:
+            output = output.permute(1, 0, 2)
+        return self.dropout(output) + identity
+
+    def _sample(self, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+        """The reference's statements around the plain op (temporal_self_attention.py:196-261) -> [bs, nq, C]."""
+        bs, num_query, H, Qn, L, P, _ = offsets.shape
+        weights = logits.softmax(-1).view(bs, num_query, H, Qn, L, P)
         # queue axis next to batch: [bs*Qn, num_query, H, L, P(,2)]
         weights = weights.permute(0, 3, 1, 2, 4, 5).reshape(bs * Qn, num_query, H, L, P).contiguous()
         offsets = offsets.permute(0, 3, 1, 2, 4, 5, 6).reshape(bs * Qn, num_query, H, L, P, 2)
@@ -406,11 +447,7 @@ class TemporalSelfAttention(BaseModule):
 
         output = msda_apply(value, spatial_shapes, level_start_index, loc, weights, self.im2col_step)
         # mean over the queue (:255-261): [bs*Qn, nq, C] -> [bs, nq, C]
-        output = output.view(bs, Qn, num_query, embed_dims).mean(1)
-        output = _linear(self.output_proj, output)
-        if not self.batch_first:
-            output = output.permute(1, 0, 2)
-        return self.dropout(output) + identity
+        return output.view(bs, Qn, num_query, -1).mean(1)
 
 
 @ATTENTION.register_module()
@@ -435,6 +472,7 @@ class PredictionMSDeformableAttention(BaseModule):
         self.attention_weights = nn.Linear(embed_dims, num_heads * num_levels * num_points)
         self.value_proj = nn.Linear(embed_dims, embed_dims)
         self.output_proj = nn.Linear(embed_dims, embed_dims)
+        self.fuse_epilogue = True      # False: materialise sampling_locations / attention_weights like the reference
         self.init_weights()
 
     def init_weights(self):
@@ -456,7 +494,7 @@ class PredictionMSDeformableAttention(BaseModule):
             query = query + query_pos
         bs, num_query, _ = query.shape
         num_value = value.shape[1]
-        assert (spatial_shapes[:, 0] * spatial_shapes[:, 1]).sum() == num_value
+        _check_num_value(self, spatial_shapes, num_value)
         H, L, P = self.num_heads, self.num_levels, self.num_points
 
         value = _linear(self.value_proj, value)
@@ -464,8 +502,23 @@ class PredictionMSDeformableAttention(BaseModule):
             value = value.masked_fill(key_padding_mask[..., None], 0.0)
         value = value.view(bs, num_value, H, -1)
         offsets = self.sampling_offsets(query).view(bs, num_query, H, L, P, 2)
-        weights = self.attention_weights(query).view(bs, num_query, H, L * P).softmax(-1)
-        weights = weights.view(bs, num_query, H, L, P)
+        logits = self.attention_weights(query).view(bs, num_query, H, L * P)
+        if _queue_fusable(self, value, reference_points, offsets, logits, 1):
+            # softmax and the sampling-location arithmetic run inside the kernel
+            output = msda_queue_fused_apply(value, spatial_shapes, level_start_index, reference_points,
+                                            offsets.view(bs, num_query, H, 1, L, P, 2),
+                                            logits.view(bs, num_query, H, 1, L * P))
+        else:
+            output = self._sample(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
+        output = _linear(self.output_proj, output)
+        if not self.batch_first:
+            output = output.permute(1, 0, 2)
+        return self.dropout(output) + identity
+
+    def _sample(self, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+        """The reference's statements around the plain op (vidar_decoder.py:466-506) -> [bs, nq, C]."""
+        bs, num_query, H, L, P, _ = offsets.shape
+        weights = logits.softmax(-1).view(bs, num_query, H, L, P)
         if reference_points.shape[-1] == 2:
             loc = reference_points[:, :, None, :, None, :] + offsets / _wh(spatial_shapes)[None, None, None, :, None, :]
         elif reference_points.shape[-1] == 4:
@@ -473,12 +526,7 @@ class PredictionMSDeformableAttention(BaseModule):
                    + offsets / P * reference_points[:, :, None, :, None, 2:] * 0.5)
         else:
             raise ValueError(f"Last dim of reference_points must be 2 or 4, but get {reference_points.shape[-1]} instead.")
-
-        output = msda_apply(value, spatial_shapes, level_start_index, loc, weights, self.im2col_step)
-        output = _linear(self.output_proj, output)
-        if not self.batch_first:
-            output = output.permute(1, 0, 2)
-        return self.dropout(output) + identity
+        return msda_apply(value, spatial_shapes, level_start_index, loc, weights, self.im2col_step)
 
 
 @ATTENTION.register_module()

@@ -231,3 +231,80 @@ class MSDeformAttn3DFusedFunction(Function):
                 _lib.ptr(grad_logits), B, K, H, C, L, Q, P, D, _lib.stream_ptr(value.device)))
         return grad_value, None, None, None, grad_offsets, grad_logits
 
+
+class MSDeformAttnQueueFusedFunction(Function):
+    """TemporalSelfAttention's and the future decoder's sampling with their elementwise prologue and TSA's queue
+    mean inside the kernel (temporal_self_attention.py:196-261, vidar_decoder.py:466-506): per (query, head, queue
+    entry g) softmax over the L*P logits, loc = offsets / (W_l, H_l) + reference_points[b*G + g, q, l], and the mean
+    of the G per-entry outputs.  Never materialises `sampling_locations`, `attention_weights`, the [B*G, Q, H*C]
+    per-entry output or their gradients.
+
+    apply(value [B*G,K,H,C], spatial_shapes, level_start_index, reference_points [B*G,Q,L,2],
+          offsets [B,Q,H,G,L,P,2] (raw Linear output), logits [B,Q,H,G,L*P]) -> [B,Q,H*C]
+    G = 2 for TemporalSelfAttention, 1 for the decoder.  Gradients: value, offsets, logits."""
+
+    @staticmethod
+    def supported(num_levels, num_points, num_queue, head_dim, num_value=0, num_heads=1):
+        """The shapes the kernel takes; num_value / num_heads (when given) also bound the G value batches of an
+        item to 2^25 floats, the vector kernels' 32-bit slab offsets."""
+        lp = num_levels * num_points
+        return (lp in (1, 2, 4, 8, 16, 32) and 0 < num_queue * lp <= 32 and head_dim in (16, 32, 64)
+                and num_queue * num_value * num_heads * head_dim < 2 ** 25)
+
+    @staticmethod
+    def forward(ctx, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+        value = _lib.aligned(value.float().contiguous())
+        ref = _lib.aligned(reference_points.float().contiguous())
+        offsets = _lib.aligned(offsets.float().contiguous())
+        logits = _lib.aligned(logits.float().contiguous())
+        spatial_shapes = spatial_shapes.contiguous()
+        level_start_index = level_start_index.contiguous()
+        _lib.require_cuda(value=value, spatial_shapes=spatial_shapes, level_start_index=level_start_index,
+                          reference_points=ref, offsets=offsets, logits=logits)
+        if value.dim() != 4:
+            raise RuntimeError(f"value must be [bs * num_queue, num_keys, num_heads, dim], got {tuple(value.shape)}")
+        if spatial_shapes.dtype != torch.int64 or level_start_index.dtype != torch.int64:
+            raise RuntimeError("spatial_shapes / level_start_index must be int64 tensors")
+        if spatial_shapes.dim() != 2 or spatial_shapes.shape[1] != 2 or level_start_index.numel() != spatial_shapes.shape[0]:
+            raise RuntimeError("spatial_shapes must be [num_levels, 2] and level_start_index [num_levels]")
+        BG, K, H, C = value.shape
+        L = spatial_shapes.shape[0]
+        if offsets.dim() != 7 or offsets.shape[2] != H or offsets.shape[4] != L or offsets.shape[6] != 2:
+            raise RuntimeError("offsets must be [bs, num_queries, num_heads, num_queue, num_levels, num_points, 2], "
+                               f"got {tuple(offsets.shape)}")
+        B, Q, _, G, _, P, _ = offsets.shape
+        if B * G != BG:
+            raise RuntimeError(f"value batch ({BG}) must be bs * num_queue ({B} x {G})")
+        if tuple(ref.shape) != (BG, Q, L, 2):
+            raise RuntimeError(f"reference_points must be {(BG, Q, L, 2)}, got {tuple(ref.shape)}")
+        if tuple(logits.shape) != (B, Q, H, G, L * P):
+            raise RuntimeError(f"logits must be {(B, Q, H, G, L * P)}, got {tuple(logits.shape)}")
+        out = torch.empty((B, Q, H * C), dtype=torch.float32, device=value.device)
+        ctx.save_for_backward(value, spatial_shapes, level_start_index, ref, offsets, logits)
+        ctx.dims = (B, G, K, H, C, L, Q, P)
+        if out.numel() == 0:
+            return out
+        with torch.cuda.device(value.device):
+            _lib.check(_lib.lib().vidar_msda_tsa_forward(
+                _lib.ptr(value), _lib.ptr(spatial_shapes), _lib.ptr(level_start_index), _lib.ptr(ref), _lib.ptr(offsets),
+                _lib.ptr(logits), _lib.ptr(out), B, G, K, H, C, L, Q, P, _lib.stream_ptr(value.device)))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        value, spatial_shapes, level_start_index, ref, offsets, logits = ctx.saved_tensors
+        B, G, K, H, C, L, Q, P = ctx.dims
+        grad_value = torch.zeros_like(value)
+        grad_offsets = torch.empty_like(offsets)      # fully overwritten by the kernel
+        grad_logits = torch.empty_like(logits)
+        if grad_output.numel():
+            grad_output = _lib.aligned(grad_output.float().contiguous())
+            with torch.cuda.device(value.device):
+                _lib.check(_lib.lib().vidar_msda_tsa_backward(
+                    _lib.ptr(value), _lib.ptr(spatial_shapes), _lib.ptr(level_start_index), _lib.ptr(ref),
+                    _lib.ptr(offsets), _lib.ptr(logits), _lib.ptr(grad_output), _lib.ptr(grad_value),
+                    _lib.ptr(grad_offsets), _lib.ptr(grad_logits), B, G, K, H, C, L, Q, P,
+                    _lib.stream_ptr(value.device)))
+        return grad_value, None, None, None, grad_offsets, grad_logits
+
