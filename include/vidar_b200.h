@@ -622,6 +622,23 @@ int vidar_dcnv3_backward(const void* input, const void* offset, const void* mask
                          int pad_h, int pad_w, int dilation_h, int dilation_w, float offset_scale, int im2col_step,
                          void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (ix) GridMask (models/utils/grid_mask.py GridMask.forward) from its numpy draws, in one launch.
+ *   x, out  [N, C, h, w] contiguous, `dtype` VIDAR_DTYPE_F32, _F16 or _BF16 (anything else returns VIDAR_E_INVALID)
+ *   offset  [h, w] (dtype) or NULL
+ *   out = x * mask                       (offset NULL)
+ *   out = x * mask + offset * (1 - mask) (offset given)
+ * in `dtype`: every product is exact (mask is 0 or 1) and the sum rounds once, as the reference's statements do.
+ * mask [h, w] is the reference's: stripes of period d and length l from st_h / st_w (rows when use_h, columns when
+ * use_w) on an (int(1.5 h), int(1.5 w)) frame of ones, rotated by PIL's Image.rotate(r) (nearest, fill 0), centre
+ * crop, inverted when mode == 1; it is evaluated per pixel in registers, never stored.
+ * Needs 1 <= h, w <= 8192, d >= 2, 0 <= l <= d, 0 <= st_h, st_w < d; use_h, use_w and mode 0 or 1; buffers
+ * aligned to their elements.  16-byte vectors when h*w is a multiple of 4 (fp32) / 8 (16-bit) and x, offset and out
+ * are 16-byte aligned.  out may not overlap x or offset.  N*C == 0 is a no-op.  One launch on `stream`, no scratch,
+ * no host sync.  The backward (d out / d x = mask) is the same call on grad_out with offset NULL. */
+int vidar_grid_mask_apply(const void* x, const void* offset, void* out, int dtype, int N, int C, int h, int w, int d,
+                          int l, int st_h, int st_w, int r, int use_h, int use_w, int mode, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

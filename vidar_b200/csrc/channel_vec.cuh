@@ -1,4 +1,5 @@
-// Channel vectors of a channel-last feature map, shared by the deformable sampling kernels (dcn.cu, dcnv3.cu).
+// Channel vectors of a channel-last feature map, shared by the deformable sampling kernels (dcn.cu, dcnv3.cu) and,
+// as vectors of consecutive pixels of one plane, by the GridMask kernel (grid_mask.cu).
 //
 // Storage type T is float, __half or __nv_bfloat16.  Every value is converted to fp32 on load (`to_f`) and rounded
 // once on a 16-bit store (`store1`).  Vec<T, V> handles V consecutive channels as fp32 values in registers:
@@ -92,6 +93,12 @@ template <typename S> struct Vec<S, 8> {
     red_add_v4(p + 4, v.b);
   }
 };
+
+// Element i of a register vector of Vec<T, V> (float, float4 or F8); i is a compile-time constant once the caller's
+// loop over the V elements is unrolled, so the vector stays in registers.
+__device__ __forceinline__ float& lane(float& v, int) { return v; }
+__device__ __forceinline__ float& lane(float4& v, int i) { return i == 0 ? v.x : i == 1 ? v.y : i == 2 ? v.z : v.w; }
+__device__ __forceinline__ float& lane(F8& v, int i) { return i < 4 ? lane(v.a, i) : lane(v.b, i - 4); }
 
 // The vector width of storage type T: 16 bytes.
 template <typename T> constexpr int kVec = 16 / sizeof(T);

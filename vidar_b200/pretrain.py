@@ -38,6 +38,7 @@ import torch.nn.functional as F
 
 from . import bev_geometry, sca, sharding, synthetic
 from . import modules as _modules  # noqa: F401  (registers the attention classes)
+from .grid_mask import GridMask
 from .head import ViDARRayHead
 from .modules.deform_attn import _linear
 from .registry import build_attention
@@ -275,14 +276,25 @@ class SyntheticViDAR(nn.Module):
     `backbone_autocast` = torch.float16 or torch.bfloat16 runs the backbone and FPN of `extract_feat` under
     torch.autocast("cuda", dtype) and casts the FPN outputs to fp32 before the camera and level embeddings: what the
     reference's `auto_fp16` on `extract_feat` and the `force_fp32` ops after it amount to in its fp16 mode.  The
-    default None runs everything in fp32.  The setting holds no state (the state_dict does not change)."""
+    default None runs everything in fp32.  The setting holds no state (the state_dict does not change).
+
+    `grid_mask=True` adds the image augmentation of every ViDAR config (use_grid_mask=True with vidar.py:45-53's
+    `GridMask(use_h=True, use_w=True, rotate=1, offset=False, ratio=0.5, mode=1, prob=0.7)`, `vidar_b200.grid_mask`):
+    in training mode the current frame's images are masked before the backbone (vidar.py:139-140).  The history
+    frames go through it in eval mode, as `obtain_history_bev` runs them: one prob-gate draw, no mask.  The draws come
+    from numpy's global generator, so under a process group every rank must seed numpy with the same value -- as the
+    reference's training script does (mmdet's init_random_seed broadcasts rank 0's seed, set_random_seed seeds numpy
+    on every rank) -- and every rank draws once per call, also a rank whose backbone runs no camera; then each rank
+    masks its own cameras with the same mask.  The default False leaves the graph as it was."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
-                 latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None):
+                 latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None,
+                 grid_mask=False):
         super().__init__()
         if backbone_autocast not in (None, torch.float16, torch.bfloat16):
             raise ValueError(f"backbone_autocast must be None, torch.float16 or torch.bfloat16 (got {backbone_autocast})")
         self.backbone_autocast = backbone_autocast
+        self.grid_mask = GridMask(True, True, rotate=1, offset=False, ratio=0.5, mode=1, prob=0.7) if grid_mask else None
         self.num_cams, self.future_frames, self.history_frames = num_cams, future_frames, history_frames
         self.bev_h, self.bev_w = bev_hw
         BEV_H, BEV_W = bev_hw          # noqa: N806  (shadows the module defaults below)
@@ -350,8 +362,9 @@ class SyntheticViDAR(nn.Module):
             self.timings.append((name, e))
 
     # ---- image features of one frame -> [cams, K, bs, C] (only this rank's SCA cameras are filled) ----
-    def extract_feat(self, img):
-        """img [bs, cams, 3, H, W] -> (feat_flatten [cams, K, bs, C], spatial_shapes, level_start_index)."""
+    def extract_feat(self, img, draw=None):
+        """img [bs, cams, 3, H, W] -> (feat_flatten [cams, K, bs, C], spatial_shapes, level_start_index).  `draw`: a
+        GridMask draw (`self.grid_mask.sample`) applied to the images before the backbone."""
         import torch.distributed as dist
         bs = img.shape[0]
         world = dist.get_world_size(self.process_group) if self.process_group is not None else 1
@@ -360,6 +373,8 @@ class SyntheticViDAR(nn.Module):
         per_cam = {}
         if mine:
             x = img[:, mine].reshape(bs * len(mine), *img.shape[2:])
+            if draw is not None:
+                x = self.grid_mask.masked(x, draw)
             if self.backbone_autocast is None:
                 outs = self.neck(self.backbone(x))
             else:
@@ -463,13 +478,16 @@ class SyntheticViDAR(nn.Module):
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
         img_metas = [dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)]) for b in range(bs)]
         prev_bev = None
+        if self.grid_mask is not None and T > 1:                                     # the history's eval-mode call
+            self.grid_mask.sample(*img.shape[-2:], training=False)
         with torch.no_grad():                                                        # obtain_history_bev
             for t in range(T - 1):
                 feats, shapes, lsi = self.extract_feat(img[:, t])
                 self._mark(f"hist{t}.backbone")
                 prev_bev = self.encode(feats, shapes, lsi, img_metas, can_bus, prev_bev)
                 self._mark(f"hist{t}.encoder")
-        feats, shapes, lsi = self.extract_feat(img[:, T - 1])
+        draw = self.grid_mask.sample(*img.shape[-2:]) if self.grid_mask is not None else None
+        feats, shapes, lsi = self.extract_feat(img[:, T - 1], draw)
         self._mark("cur.backbone")
         ref_bev = self.encode(feats, shapes, lsi, img_metas, can_bus, prev_bev)
         self._mark("cur.encoder")
