@@ -331,31 +331,24 @@ int vidar_ray_gumbel_backward(const float* sigma, const float* origin, const flo
  *   grid_num waypoints of step grid_step / (min(Hb,Wb)//2) (:101-104); eps (:80,147).
  *   Supported: D a power of two <= 32, G in {1, 2, 4, 8, 16} (the reference default
  *   pred_height=1, reduction=16, embed_dims=256 is D=1, G=16).
- * ---------------------------------------------------------------------------------- */
-int vidar_latent_render_forward(const float* occ, const float* feat, float* prob, float* pooled,
-                                float* aux, int bs, int D, int G, int Hb, int Wb, int grid_num,
-                                float grid_step, float eps, int act, void* stream);
-
-/* aux (may be NULL everywhere): [3, bs, Hb, Wb, D] floats the forward fills (product of the
- * non-zero transmittance factors, count of zero factors, sum of sampled probabilities) so the
- * backward does not have to march the rays again to recompute them.
+ *   aux    [3, bs, Hb, Wb, D]  filled by the forward (product of the non-zero transmittance
+ *          factors, count of zero factors, sum of sampled probabilities) and read by the backward,
+ *          so that it does not march the rays again to recompute them.
  *
- * Backward.  grad_prob [bs,Hb,Wb,D] = gradient reaching `prob` from outside the core (the
- * final product, :158-160); grad_pooled [bs,Hb*Wb,D*G]; pooled = forward output (needed with aux).
- * grad_prob_total [bs,Hb,Wb,D] is scratch (fully overwritten).  grad_occ, grad_feat:
- * caller-zeroed, shaped like occ, feat. */
-int vidar_latent_render_backward(const float* occ, const float* feat, const float* prob,
-                                 const float* pooled, const float* aux, const float* grad_prob,
-                                 const float* grad_pooled, float* grad_prob_total, float* grad_occ,
-                                 float* grad_feat, int bs, int D, int G, int Hb, int Wb,
-                                 int grid_num, float grid_step, float eps, int act, void* stream);
-
-/* The same four kernels, one phase per call, on a range [cell0, cell0+ncells) of the
- * bs*Hb*Wb BEV cells (row-major): when the cells are sharded over GPUs the host places a
- * collective on the small maps between the phases (vidar_b200/modules/latent_rendering.py).
+ * One phase per call, on a range [cell0, cell0+ncells) of the bs*Hb*Wb BEV cells (row-major):
+ * when the cells are sharded over GPUs the host places a collective on the small maps between
+ * the phases (vidar_b200/modules/latent_rendering.py).  Forward: prob_forward, then
+ * pool_forward on the complete prob map.  Backward: pool_backward adds the gradient that
+ * reaches the prob map through the ray pooling to grad_prob_map; prob_backward reads
+ * grad_prob_total = that sum plus grad_prob [bs,Hb,Wb,D], the gradient reaching `prob` from
+ * outside the core (the final product, :158-160).  grad_pooled is [bs,Hb*Wb,D*G].
+ * aux and pooled (the forward's outputs) must not be NULL.
  * A range with cell0 < 0, ncells < 0 or cell0 + ncells > bs*Hb*Wb is rejected.
- * Outputs are indexed by GLOBAL cell; scatter targets (grad_*) are caller-zeroed full maps
- * that receive this range's contributions. */
+ * Outputs are indexed by GLOBAL cell.  The scatter targets grad_prob_map, grad_feat and
+ * grad_occ (shaped like prob, feat and occ) are full maps that this range's contributions are
+ * added to: the caller zeroes them, or starts grad_prob_map as a copy of grad_prob so that it
+ * ends as grad_prob_total.
+ * ---------------------------------------------------------------------------------- */
 int vidar_latent_prob_forward(const float* occ, float* prob, float* aux, int bs, int D, int Hb,
                               int Wb, int grid_num, float grid_step, int act,
                               long long cell0, long long ncells, void* stream);

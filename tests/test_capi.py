@@ -57,8 +57,16 @@ def test_argument_validation_of_the_fused_entry_points():
     """Shape contracts of the fused ops are checked before anything touches the device, so they can be
     exercised on a GPU-less host: every call below must return VIDAR_E_INVALID with a message."""
     L = _lib.lib()
-    N = None
+    N, X = None, ctypes.c_void_p(0x1000)
+    # the LatentRendering core on an empty cell range: a missing check would return success, not launch
+    lr = (1, 16, 4, 4, 8, 0.5)                      # bs, D, Hb, Wb, grid_num, grid_step
+    lr_g = (1, 16, 1, 4, 4, 8, 0.5, 1e-3)           # bs, D, G, Hb, Wb, grid_num, grid_step, eps
     cases = [
+        (L.vidar_latent_prob_forward, (X, X, N) + lr + (1, 0, 0, N), b"null pointer"),
+        (L.vidar_latent_pool_forward, (X, X, X, N) + lr_g + (0, 0, N), b"null pointer"),
+        (L.vidar_latent_pool_backward, (X, X, X, N, X, X, X) + lr_g + (0, 0, N), b"null pointer"),
+        (L.vidar_latent_pool_backward, (X, X, N, X, X, X, X) + lr_g + (0, 0, N), b"null pointer"),
+        (L.vidar_latent_prob_backward, (X, N, X, X) + lr + (1, 0, 0, N), b"null pointer"),
         (L.vidar_latent_proj_in_forward, (N, N, N, N, N, N, N, 10, 64, 16, 16, N), b"embed_dims must be 128 or 256"),
         (L.vidar_latent_proj_in_backward, (N,) * 10 + (10, 256, 20, 16, N), b"pred_height + rank"),
         (L.vidar_latent_proj_out_forward, (N, N, N, N, N, 10, 256, 24, 8, N), b"embed_dims / pred_height"),

@@ -8,25 +8,9 @@ import torch
 
 from oracle import latent_render_ref as ref
 from tests.parity import close
-from tests.test_latent_core_gpu import ACT, EPS, NAN, _check_core, _inputs, _oracle
+from tests.test_latent_core_gpu import ACT, EPS, _abi_core, _check_core, _inputs, _oracle
 from vidar_b200 import _lib
 from vidar_b200.sharding import shard_range
-
-
-def _abi_backward(cuda, occ, feat, gp, gq, grid_num, grid_step, act, aux_mode):
-    """forward + backward through the C ABI; aux_mode: "aux" (aux + pooled, as the module runs it) or "none"."""
-    bs, Hb, Wb, D = occ.shape
-    G = feat.shape[-1] // D
-    L, st, P = _lib.lib(), _lib.stream_ptr(cuda), _lib.ptr
-    o, f, gpd, gqd = (t.to(cuda) for t in (occ, feat, gp, gq))
-    dims = (bs, D, G, Hb, Wb, grid_num, grid_step, EPS, ACT[act], st)
-    prob, pooled = torch.full_like(o, NAN), torch.full((bs, Hb * Wb, D * G), NAN, device=cuda)
-    aux = torch.full((3,) + tuple(o.shape), NAN, device=cuda) if aux_mode == "aux" else None
-    _lib.check(L.vidar_latent_render_forward(P(o), P(f), P(prob), P(pooled), P(aux), *dims))
-    total, go, gf = torch.full_like(o, NAN), torch.zeros_like(o), torch.zeros_like(f)
-    _lib.check(L.vidar_latent_render_backward(P(o), P(f), P(prob), P(pooled if aux is not None else None), P(aux),
-                                              P(gpd), P(gqd), P(total), P(go), P(gf), *dims))
-    return go, gf, total
 
 
 @pytest.fixture(scope="module")
@@ -37,14 +21,13 @@ def bench_shape_oracle():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("aux_mode", ["aux", "none"])
-def test_bench_shape(cuda, bench_shape_oracle, aux_mode):
+def test_bench_shape(cuda, bench_shape_oracle):
     """1 x 200 x 200, pred_height 16, one channel per height, grid_num 256, step 0.5, sigmoid: bench.py's core."""
     (occ, feat, gp, gq), (go64, gf64, gt64) = bench_shape_oracle
-    go, gf, total = _abi_backward(cuda, occ, feat, gp, gq, 256, 0.5, "sigmoid", aux_mode)
-    close(total, gt64, f"{aux_mode}: grad_prob_total")
-    close(go, go64, f"{aux_mode}: grad occ")
-    close(gf, gf64, f"{aux_mode}: grad feat")
+    *_, total, go, gf = _abi_core(cuda, occ, feat, gp, gq, 256, 0.5, "sigmoid")
+    close(total, gt64, "grad_prob_total")
+    close(go, go64, "grad occ")
+    close(gf, gf64, "grad feat")
 
 
 # (bs, Hb, Wb, D, grid_num, grid_step, act): G = 1 so both backward kernels take the bundle path
@@ -67,18 +50,6 @@ EDGES = {
 def test_bundle_edges(cuda, name):
     bs, Hb, Wb, D, grid_num, grid_step, act = EDGES[name]
     _check_core(cuda, bs, Hb, Wb, D, 1, grid_num, grid_step, act, seed=Hb * 31 + Wb)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", list(EDGES)[:2] + ["2x2", "9x12"])
-def test_bundle_edges_without_aux(cuda, name):
-    bs, Hb, Wb, D, grid_num, grid_step, act = EDGES[name]
-    occ, feat, gp, gq = _inputs(bs, Hb, Wb, D, 1, seed=Hb + Wb)
-    _, _, ((go64, gf64, gt64),) = _oracle(occ, feat, (gp,), gq, grid_num, grid_step, act)
-    go, gf, total = _abi_backward(cuda, occ, feat, gp, gq, grid_num, grid_step, act, "none")
-    close(total, gt64, "grad_prob_total")
-    close(go, go64, "grad occ")
-    close(gf, gf64, "grad feat")
 
 
 @pytest.mark.gpu

@@ -2,7 +2,7 @@
 
 Covers every <VEC, G> instantiation of the pool kernels and both VEC of the prob kernels, BEVs with and
 without a centre cell, the march bounds over grid_step / grid_num, saturated activations (exactly-zero
-transmittance factors), every combination of the optional `aux` buffer through the C ABI, and the
+transmittance factors), the `aux` buffer the forward fills and the backward reads through the C ABI, and the
 phase-wise entry points on cell ranges, the way the cell-sharded core calls them."""
 import os
 import re
@@ -143,41 +143,43 @@ def test_saturated_activations(cuda, D, G, act):
     _check_core(cuda, bs, Hb, Wb, D, G, grid_num, grid_step, act, seed=D + G, occ=occ)
 
 
-def _ptrs(*ts):
-    return [_lib.ptr(t) for t in ts]
+def _abi_core(cuda, occ, feat, gp, gq, grid_num, grid_step, act):
+    """The four phase entry points on all cells, in the single-GPU core's order: prob and pool forward, then the pool
+    backward into a copy of grad_prob and the prob backward from that sum.  The forward's outputs start as NaN, so a
+    cell left unwritten shows.  Returns prob, pooled, aux, grad_prob_total, grad occ, grad feat."""
+    bs, Hb, Wb, D = occ.shape
+    G = feat.shape[-1] // D
+    L, st, P = _lib.lib(), _lib.stream_ptr(cuda), _lib.ptr
+    o, f, gpd, gqd = (t.to(cuda) for t in (occ, feat, gp, gq))
+    cells, a = bs * Hb * Wb, ACT[act]
+    prob, pooled = torch.full_like(o, NAN), torch.full((bs, Hb * Wb, D * G), NAN, device=cuda)
+    aux = torch.full((3,) + tuple(o.shape), NAN, device=cuda)
+    _lib.check(L.vidar_latent_prob_forward(P(o), P(prob), P(aux), bs, D, Hb, Wb, grid_num, grid_step, a, 0, cells, st))
+    _lib.check(L.vidar_latent_pool_forward(P(prob), P(f), P(pooled), P(aux), bs, D, G, Hb, Wb, grid_num, grid_step, EPS,
+                                           0, cells, st))
+    total, go, gf = gpd.clone(), torch.zeros_like(o), torch.zeros_like(f)
+    _lib.check(L.vidar_latent_pool_backward(P(prob), P(f), P(pooled), P(aux), P(gqd), P(total), P(gf), bs, D, G, Hb, Wb,
+                                            grid_num, grid_step, EPS, 0, cells, st))
+    _lib.check(L.vidar_latent_prob_backward(P(o), P(aux), P(total), P(go), bs, D, Hb, Wb, grid_num, grid_step, a, 0,
+                                            cells, st))
+    return prob, pooled, aux, total, go, gf
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("D,G,vec,act", MATRIX, ids=MATRIX_IDS)
-def test_aux_buffer_combinations(cuda, D, G, vec, act):
-    """Forward with and without aux; backward with (aux, pooled), (aux, NULL) -- the pool backward then
-    recomputes its sums -- and (NULL, NULL), where both backward kernels re-march the rays."""
+def test_aux_written_and_read_by_backward(cuda, D, G, vec, act):
+    """The forward fills every cell of aux, and the backward that reads aux and pooled matches the oracle."""
     bs, Hb, Wb, grid_num, grid_step = 2, 7, 10, 24, 0.5
     i = MATRIX.index((D, G, vec, act))
     occ, feat, gp, gq = _inputs(bs, Hb, Wb, D, G, seed=200 + i)
     p64, q64, ((go64, gf64, gt64),) = _oracle(occ, feat, (gp,), gq, grid_num, grid_step, act)
-    L, st = _lib.lib(), _lib.stream_ptr(cuda)
-    o, f, gpd, gqd = (t.to(cuda) for t in (occ, feat, gp, gq))
-    dims = (bs, D, G, Hb, Wb, grid_num, grid_step, EPS, ACT[act], st)
-    outs = []
-    for with_aux in (True, False):
-        prob = torch.full_like(o, NAN)
-        pooled = torch.full((bs, Hb * Wb, D * G), NAN, device=cuda)
-        aux = torch.full((3,) + tuple(o.shape), NAN, device=cuda) if with_aux else None
-        _lib.check(L.vidar_latent_render_forward(*_ptrs(o, f, prob, pooled, aux), *dims))
-        outs.append((prob, pooled, aux))
-    (prob, pooled, aux), (prob_na, pooled_na, _) = outs
-    assert torch.equal(prob, prob_na) and torch.equal(pooled, pooled_na), "aux changed the forward"
+    prob, pooled, aux, total, go, gf = _abi_core(cuda, occ, feat, gp, gq, grid_num, grid_step, act)
     assert not aux.isnan().any(), "aux not fully written"
     close(prob, p64, "prob")
     close(pooled, q64, "pooled")
-    for a, pl, what in ((aux, pooled, "aux+pooled"), (aux, None, "aux only"), (None, None, "no aux")):
-        total = torch.full_like(o, NAN)
-        go, gf = torch.zeros_like(o), torch.zeros_like(f)
-        _lib.check(L.vidar_latent_render_backward(*_ptrs(o, f, prob, pl, a, gpd, gqd, total, go, gf), *dims))
-        close(total, gt64, f"{what}: grad_prob_total")
-        close(go, go64, f"{what}: grad occ")
-        close(gf, gf64, f"{what}: grad feat")
+    close(total, gt64, "grad_prob_total")
+    close(go, go64, "grad occ")
+    close(gf, gf64, "grad feat")
 
 
 def _range_sets(total, HW):

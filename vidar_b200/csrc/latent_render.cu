@@ -22,9 +22,9 @@
 // lanes cover one waypoint's heights with one 16-byte load per bilinear corner and
 // 32/LPW waypoints are in flight per step; |g_k| grows linearly in k, so the march stops at
 // the cell (phase 1) or at the BEV border (phase 2) instead of visiting all G waypoints
-// behind a mask.  Products / sums over waypoints are finished with warp shuffles; only
-// prob (D floats) and pooled (D*g floats) are written per cell.  Backward kernels recompute
-// the forward quantities and scatter with vector reductions.
+// behind a mask.  Products / sums over waypoints are finished with warp shuffles; per cell the
+// forward writes prob (D floats), pooled (D*g floats) and its sums over the waypoints to aux
+// (3*D floats).  Backward kernels read those sums and scatter with vector reductions.
 // Backward dispatch, by shape: the phase 2 backward with VEC 4 and G 1 (every D in {4, 8, 16, 32} with one
 // feature channel per height, the shipped configuration) runs in angular bundles that sum their scatter in
 // shared memory (latent_pool_bwd_bundle_kernel); other VEC / G and the phase 1 backward use the per-cell kernels.
@@ -244,10 +244,8 @@ latent_prob_fwd_kernel(LrDims L, const float* __restrict__ occ, float* __restric
     for (int v = 0; v < VEC; ++v) out[v] = (nz[v] > 0.f ? 0.f : tnz[v]) * activate(L.act, x[v]);
     const size_t o = ((size_t)b * HW + u) * L.D + ch;
     V<VEC>::st(prob + o, out);
-    if (aux_t) {          // saved for the backward: no second march there
-      V<VEC>::st(aux_t + o, tnz);
-      V<VEC>::st(aux_nz + o, nz);
-    }
+    V<VEC>::st(aux_t + o, tnz);     // saved for the backward: no second march there
+    V<VEC>::st(aux_nz + o, nz);
   }
 }
 
@@ -264,36 +262,9 @@ latent_prob_bwd_kernel(LrDims L, const float* __restrict__ occ, const float* __r
   const float* omap = occ + (size_t)b * HW * L.D;
   float* gmap = grad_occ + (size_t)b * HW * L.D;
   float tnz[VEC], nz[VEC];
-#pragma unroll
-  for (int v = 0; v < VEC; ++v) { tnz[v] = 1.f; nz[v] = 0.f; }
   const int kend = march_end(L, c.lenG), kchk = march_check(L, c.lenG);
-  if (aux_t) {            // forward saved the products: skip the recomputation march
-    V<VEC>::ld(aux_t + ((size_t)b * HW + u) * L.D + ch, tnz);
-    V<VEC>::ld(aux_nz + ((size_t)b * HW + u) * L.D + ch, nz);
-  }
-  for (int k0 = 0; !aux_t && k0 < kend; k0 += WPI) {
-    const int k = k0 + slot;
-    if (k < kend) {
-      float gx, gy;
-      if (waypoint(L, c, k, kchk, c.lenG, gx, gy)) {
-        float x[VEC];
-        sample<VEC>(omap, L.D, ch, bilinear_setup(gx, gy, L.Hb, L.Wb), x);
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) {
-          const float f = 1.f - activate(L.act, x[v]);
-          if (f == 0.f) nz[v] += 1.f; else tnz[v] *= f;
-        }
-      }
-    }
-  }
-  if (!aux_t) {
-#pragma unroll
-    for (int v = 0; v < VEC; ++v)
-      for (int off = LPW; off < 32; off <<= 1) {
-        tnz[v] *= __shfl_xor_sync(0xffffffffu, tnz[v], off);
-        nz[v] += __shfl_xor_sync(0xffffffffu, nz[v], off);
-      }
-  }
+  V<VEC>::ld(aux_t + ((size_t)b * HW + u) * L.D + ch, tnz);     // the forward's products
+  V<VEC>::ld(aux_nz + ((size_t)b * HW + u) * L.D + ch, nz);
   float g[VEC], xG[VEC], aG[VEC];
   V<VEC>::ld(grad_prob + ((size_t)b * HW + u) * L.D + ch, g);
   const Bil bG = bilinear_setup(c.cgx, c.cgy, L.Hb, L.Wb);
@@ -396,7 +367,7 @@ latent_pool_fwd_kernel(LrDims L, const float* __restrict__ prob, const float* __
     for (int v = 0; v < VEC; ++v)
 #pragma unroll
       for (int j = 0; j < G; ++j) o[(ch + v) * G + j] = N[v * G + j] / (S[v] + L.eps);
-    if (aux_s) V<VEC>::st(aux_s + ((size_t)b * HW + u) * L.D + ch, S);
+    V<VEC>::st(aux_s + ((size_t)b * HW + u) * L.D + ch, S);
   }
 }
 
@@ -413,22 +384,13 @@ latent_pool_bwd_kernel(LrDims L, const float* __restrict__ prob, const float* __
   float* gpm = grad_prob_map + (size_t)b * HW * L.D;
   float* gfm = grad_feat + (size_t)b * HW * L.D * G;
   float S[VEC], N[VEC * G];
-  if (aux_s) {            // forward saved S; N = pooled * (S + eps)
-    V<VEC>::ld(aux_s + ((size_t)b * HW + u) * L.D + ch, S);
-    const float* po = pooled + ((size_t)b * HW + u) * L.D * G;
+  // forward saved S; N = pooled * (S + eps)
+  V<VEC>::ld(aux_s + ((size_t)b * HW + u) * L.D + ch, S);
+  const float* po = pooled + ((size_t)b * HW + u) * L.D * G;
 #pragma unroll
-    for (int v = 0; v < VEC; ++v)
+  for (int v = 0; v < VEC; ++v)
 #pragma unroll
-      for (int j = 0; j < G; ++j) N[v * G + j] = __ldg(po + (ch + v) * G + j) * (S[v] + L.eps);
-  } else {
-    pool_accumulate<VEC, G>(L, c, pmap, fmap, ch, slot, WPI, S, N);
-#pragma unroll
-    for (int v = 0; v < VEC; ++v)
-      for (int off = LPW; off < 32; off <<= 1) S[v] += __shfl_xor_sync(0xffffffffu, S[v], off);
-#pragma unroll
-    for (int v = 0; v < VEC * G; ++v)
-      for (int off = LPW; off < 32; off <<= 1) N[v] += __shfl_xor_sync(0xffffffffu, N[v], off);
-  }
+    for (int j = 0; j < G; ++j) N[v * G + j] = __ldg(po + (ch + v) * G + j) * (S[v] + L.eps);
   // pooled_c = N_c / (S_d + eps)
   float gN[VEC * G], gS[VEC];
   const float* gp = grad_pooled + ((size_t)b * HW + u) * L.D * G;
@@ -529,9 +491,8 @@ inline size_t bundle_smem_bytes(int D) {
 }
 
 // latent_pool_bwd_kernel<4, 1> on the cells of `order`, one CTA per kBundle consecutive ones.  map0 = prob,
-// grad_in = grad_pooled, out0 = grad_feat, out1 = grad_prob_map; aux0 / aux1 = the forward's S and pooled, or
-// NULL to re-march.  prologue: a warp per cell forms gN and gS as latent_pool_bwd_kernel does.  Then per chunk of
-// kChunk waypoints:
+// grad_in = grad_pooled, out0 = grad_feat, out1 = grad_prob_map; aux0 / aux1 = the forward's S and pooled.
+// prologue: a warp per cell forms gN and gS as latent_pool_bwd_kernel does.  Then per chunk of kChunk waypoints:
 //   A1  thread = (waypoint, cell): waypoint, mask, bilinear footprint; the box origin is the warp's minimum
 //       corner; ballots give each box pixel's cells and the cells with a corner outside the box.
 //   A2  thread = (waypoint, cell, float4): gathers of prob and feat, gN pg and gS + gN f into shared memory.
@@ -547,7 +508,7 @@ latent_pool_bwd_bundle_kernel(LrDims L, const int* __restrict__ order, const flo
   BundleSmem& sm = *reinterpret_cast<BundleSmem*>(smem_raw);
   float* rows = reinterpret_cast<float*>(smem_raw + sizeof(BundleSmem));   // [rows][kBundle][D]
   float* vec = rows + 2 * kBundle * L.D;                                    // [2][kChunk][kBundle][D]
-  const int D = L.D, LPW = D / VEC, WPI = 32 / LPW, HW = L.Hb * L.Wb;
+  const int D = L.D, LPW = D / VEC, HW = L.Hb * L.Wb;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slot = lane / LPW, ch = (lane % LPW) * VEC;
 
@@ -564,19 +525,9 @@ latent_pool_bwd_bundle_kernel(LrDims L, const int* __restrict__ order, const flo
     const size_t o = ((size_t)b * HW + u) * D + ch;
     {   // pooled_c = N_c / (S_d + eps)
       float S[VEC], N[VEC];
-      if (aux0) {
-        V<VEC>::ld(aux0 + o, S);
+      V<VEC>::ld(aux0 + o, S);
 #pragma unroll
-        for (int v = 0; v < VEC; ++v) N[v] = __ldg(aux1 + o + v) * (S[v] + L.eps);
-      } else {
-        pool_accumulate<VEC, 1>(L, cg, map0 + (size_t)b * HW * D, feat + (size_t)b * HW * D, ch, slot, WPI, S, N);
-#pragma unroll
-        for (int v = 0; v < VEC; ++v)
-          for (int off = LPW; off < 32; off <<= 1) {
-            S[v] += __shfl_xor_sync(0xffffffffu, S[v], off);
-            N[v] += __shfl_xor_sync(0xffffffffu, N[v], off);
-          }
-      }
+      for (int v = 0; v < VEC; ++v) N[v] = __ldg(aux1 + o + v) * (S[v] + L.eps);
       float gN[VEC], gS[VEC];
 #pragma unroll
       for (int v = 0; v < VEC; ++v) {
@@ -821,19 +772,14 @@ using namespace vidar;
     }                                                                                  \
   } while (0)
 
-// aux: optional [3, bs, Hb, Wb, D] floats written by the forward (product of non-zero factors,
-// number of zero factors, sum of sampled probabilities) and read by the backward, which then skips
-// its recomputation marches.  NULL = forward saves nothing / backward recomputes.
-#define AUX_T(a) (a)
-#define AUX_NZ(a, n) ((a) ? (a) + (n) : nullptr)
-#define AUX_S(a, n) ((a) ? (a) + 2 * (n) : nullptr)
-
+// aux: [3, bs, Hb, Wb, D] floats written by the forward (product of non-zero factors, number of
+// zero factors, sum of sampled probabilities) and read by the backward instead of a second march.
 static int prob_fwd(const LrDims& L, int vec, const float* occ, float* prob, float* aux, cudaStream_t st) {
   if (L.ncells == 0) return VIDAR_OK;
   const size_t n = (size_t)L.bs * L.Hb * L.Wb * L.D;
   const dim3 grid(lr_blocks(L)), block(kCellsPerBlock * 32);
-  if (vec == 4) latent_prob_fwd_kernel<4><<<grid, block, 0, st>>>(L, occ, prob, AUX_T(aux), AUX_NZ(aux, n));
-  else latent_prob_fwd_kernel<1><<<grid, block, 0, st>>>(L, occ, prob, AUX_T(aux), AUX_NZ(aux, n));
+  if (vec == 4) latent_prob_fwd_kernel<4><<<grid, block, 0, st>>>(L, occ, prob, aux, aux + n);
+  else latent_prob_fwd_kernel<1><<<grid, block, 0, st>>>(L, occ, prob, aux, aux + n);
   return check_launch("LatentRendering.prob_forward");
 }
 
@@ -841,7 +787,7 @@ static int pool_fwd(const LrDims& L, int vec, int G, const float* prob, const fl
                     float* aux, cudaStream_t st) {
   if (L.ncells == 0) return VIDAR_OK;
   const size_t n = (size_t)L.bs * L.Hb * L.Wb * L.D;
-  LR_DISPATCH_VG(latent_pool_fwd_kernel, L, prob, feat, pooled, AUX_S(aux, n));
+  LR_DISPATCH_VG(latent_pool_fwd_kernel, L, prob, feat, pooled, aux + 2 * n);
   return check_launch("LatentRendering.pool_forward");
 }
 
@@ -850,13 +796,12 @@ static int pool_bwd(const LrDims& L, int vec, int G, const float* prob, const fl
                     cudaStream_t st) {
   if (L.ncells == 0) return VIDAR_OK;
   const size_t n = (size_t)L.bs * L.Hb * L.Wb * L.D;
-  const float* as = (aux && pooled) ? aux + 2 * n : nullptr;
   if (vec == 4 && G == 1) {
-    const int rc = pool_bwd_bundled(L, prob, feat, grad_pooled, grad_feat, grad_prob_map, as, pooled, st,
+    const int rc = pool_bwd_bundled(L, prob, feat, grad_pooled, grad_feat, grad_prob_map, aux + 2 * n, pooled, st,
                                     "LatentRendering.pool_backward");
     if (rc) return rc;
   } else {
-    LR_DISPATCH_VG(latent_pool_bwd_kernel, L, prob, feat, grad_pooled, grad_prob_map, grad_feat, as, pooled);
+    LR_DISPATCH_VG(latent_pool_bwd_kernel, L, prob, feat, grad_pooled, grad_prob_map, grad_feat, aux + 2 * n, pooled);
   }
   return check_launch("LatentRendering.pool_backward");
 }
@@ -866,50 +811,13 @@ static int prob_bwd(const LrDims& L, int vec, const float* occ, const float* aux
   if (L.ncells == 0) return VIDAR_OK;
   const size_t n = (size_t)L.bs * L.Hb * L.Wb * L.D;
   const dim3 grid(lr_blocks(L)), block(kCellsPerBlock * 32);
-  if (vec == 4) latent_prob_bwd_kernel<4><<<grid, block, 0, st>>>(L, occ, grad_prob_total, grad_occ, aux, aux ? aux + n : nullptr);
-  else latent_prob_bwd_kernel<1><<<grid, block, 0, st>>>(L, occ, grad_prob_total, grad_occ, aux, aux ? aux + n : nullptr);
+  if (vec == 4) latent_prob_bwd_kernel<4><<<grid, block, 0, st>>>(L, occ, grad_prob_total, grad_occ, aux, aux + n);
+  else latent_prob_bwd_kernel<1><<<grid, block, 0, st>>>(L, occ, grad_prob_total, grad_occ, aux, aux + n);
   return check_launch("LatentRendering.prob_backward");
 }
 
-extern "C" int vidar_latent_render_forward(const float* occ, const float* feat, float* prob, float* pooled,
-                                           float* aux, int bs, int D, int G, int Hb, int Wb, int grid_num,
-                                           float grid_step, float eps, int act, void* stream) {
-  LrDims L;
-  int vec;
-  int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, act, vec, "LatentRendering.forward", 0,
-                    (long long)bs * Hb * Wb);
-  if (rc) return rc;
-  VIDAR_REQUIRE(occ && feat && prob && pooled, "LatentRendering.forward: null pointer argument");
-  rc = prob_fwd(L, vec, occ, prob, aux, (cudaStream_t)stream);
-  if (rc) return rc;
-  return pool_fwd(L, vec, G, prob, feat, pooled, aux, (cudaStream_t)stream);
-}
-
-extern "C" int vidar_latent_render_backward(const float* occ, const float* feat, const float* prob,
-                                            const float* pooled, const float* aux, const float* grad_prob,
-                                            const float* grad_pooled, float* grad_prob_total, float* grad_occ,
-                                            float* grad_feat, int bs, int D, int G, int Hb, int Wb,
-                                            int grid_num, float grid_step, float eps, int act, void* stream) {
-  LrDims L;
-  int vec;
-  int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, act, vec, "LatentRendering.backward", 0,
-                    (long long)bs * Hb * Wb);
-  if (rc) return rc;
-  VIDAR_REQUIRE(occ && feat && prob && grad_prob && grad_pooled && grad_prob_total && grad_occ && grad_feat,
-                "LatentRendering.backward: null pointer argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  // grad_prob_total starts as a copy of the upstream grad_prob; phase 2 adds the gradient that
-  // reaches the prob map through the ray pooling; phase 1 consumes the sum.
-  cudaError_t e = cudaMemcpyAsync(grad_prob_total, grad_prob, sizeof(float) * (size_t)bs * Hb * Wb * D,
-                                  cudaMemcpyDeviceToDevice, st);
-  if (e != cudaSuccess) return set_error(VIDAR_E_CUDA, "LatentRendering.backward: memcpy: %s", cudaGetErrorString(e));
-  rc = pool_bwd(L, vec, G, prob, feat, pooled, aux, grad_pooled, grad_prob_total, grad_feat, st);
-  if (rc) return rc;
-  return prob_bwd(L, vec, occ, aux, grad_prob_total, grad_occ, st);
-}
-
-// ---- phase-wise entry points on a cell range: lets the host put a collective between the
-// phases when the BEV cells are sharded over GPUs (SURVEY.md 8e).
+// ---- entry points: one phase per call on a cell range, so the host can put a collective between
+// the phases when the BEV cells are sharded over GPUs (SURVEY.md 8e).
 extern "C" int vidar_latent_prob_forward(const float* occ, float* prob, float* aux, int bs, int D, int Hb,
                                          int Wb, int grid_num, float grid_step, int act, long long cell0,
                                          long long ncells, void* stream) {
@@ -917,7 +825,7 @@ extern "C" int vidar_latent_prob_forward(const float* occ, float* prob, float* a
   int vec;
   int rc = check_lr(L, bs, D, 1, Hb, Wb, grid_num, grid_step, 0.f, act, vec, "LatentRendering.prob_forward", cell0, ncells);
   if (rc) return rc;
-  VIDAR_REQUIRE(occ && prob, "LatentRendering.prob_forward: null pointer argument");
+  VIDAR_REQUIRE(occ && prob && aux, "LatentRendering.prob_forward: null pointer argument");
   return prob_fwd(L, vec, occ, prob, aux, (cudaStream_t)stream);
 }
 
@@ -928,7 +836,7 @@ extern "C" int vidar_latent_pool_forward(const float* prob, const float* feat, f
   int vec;
   int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, 1, vec, "LatentRendering.pool_forward", cell0, ncells);
   if (rc) return rc;
-  VIDAR_REQUIRE(prob && feat && pooled, "LatentRendering.pool_forward: null pointer argument");
+  VIDAR_REQUIRE(prob && feat && pooled && aux, "LatentRendering.pool_forward: null pointer argument");
   return pool_fwd(L, vec, G, prob, feat, pooled, aux, (cudaStream_t)stream);
 }
 
@@ -941,7 +849,8 @@ extern "C" int vidar_latent_pool_backward(const float* prob, const float* feat, 
   int vec;
   int rc = check_lr(L, bs, D, G, Hb, Wb, grid_num, grid_step, eps, 1, vec, "LatentRendering.pool_backward", cell0, ncells);
   if (rc) return rc;
-  VIDAR_REQUIRE(prob && feat && grad_pooled && grad_prob_map && grad_feat, "LatentRendering.pool_backward: null pointer argument");
+  VIDAR_REQUIRE(prob && feat && pooled && aux && grad_pooled && grad_prob_map && grad_feat,
+                "LatentRendering.pool_backward: null pointer argument");
   return pool_bwd(L, vec, G, prob, feat, pooled, aux, grad_pooled, grad_prob_map, grad_feat, (cudaStream_t)stream);
 }
 
@@ -953,6 +862,6 @@ extern "C" int vidar_latent_prob_backward(const float* occ, const float* aux, co
   int vec;
   int rc = check_lr(L, bs, D, 1, Hb, Wb, grid_num, grid_step, 0.f, act, vec, "LatentRendering.prob_backward", cell0, ncells);
   if (rc) return rc;
-  VIDAR_REQUIRE(occ && grad_prob_total && grad_occ, "LatentRendering.prob_backward: null pointer argument");
+  VIDAR_REQUIRE(occ && aux && grad_prob_total && grad_occ, "LatentRendering.prob_backward: null pointer argument");
   return prob_bwd(L, vec, occ, aux, grad_prob_total, grad_occ, (cudaStream_t)stream);
 }

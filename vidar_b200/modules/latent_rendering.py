@@ -25,64 +25,30 @@ from ..registry import ATTENTION, BaseModule
 _ACT = {"exp": 0, "sigmoid": 1}
 
 
+def _shard(n, group):
+    """(world, c0, count): this rank's contiguous share [c0, c0 + count) of n BEV cells over `group`; all of them
+    when `group` is None, has one rank or no process group is initialised."""
+    if group is None:
+        return 1, 0, n
+    import torch.distributed as dist
+    from ..sharding import shard_range
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    if world == 1:
+        return 1, 0, n
+    lo, hi = shard_range(n, dist.get_rank(group), world)
+    return world, lo, hi - lo
+
+
 class _LatentRenderCore(torch.autograd.Function):
-    """(occ [bs,Hb,Wb,D], feat [bs,Hb,Wb,D*G]) -> (prob [bs,Hb,Wb,D], pooled [bs,Hb*Wb,D*G])."""
+    """(occ [bs,Hb,Wb,D], feat [bs,Hb,Wb,D*G]) -> (prob [bs,Hb,Wb,D], pooled [bs,Hb*Wb,D*G]).
 
-    @staticmethod
-    def forward(ctx, occ, feat, grid_num, grid_step, eps, act):
-        _lib.require_cuda(occ=occ.contiguous(), feat=feat.contiguous())
-        occ, feat = occ.float().contiguous(), feat.float().contiguous()
-        bs, Hb, Wb, D = occ.shape
-        Ca = feat.shape[-1]
-        if feat.shape[:3] != occ.shape[:3] or Ca % D != 0:
-            raise RuntimeError("feat must be [bs, Hb, Wb, pred_height * k]")
-        prob = torch.empty_like(occ)
-        pooled = torch.empty((bs, Hb * Wb, Ca), dtype=torch.float32, device=occ.device)
-        # forward by-products the backward would otherwise re-march the rays for (3 x 2.56 MB)
-        aux = torch.empty((3,) + tuple(occ.shape), dtype=torch.float32, device=occ.device)
-        with torch.cuda.device(occ.device):
-            _lib.check(_lib.lib().vidar_latent_render_forward(
-                _lib.ptr(occ), _lib.ptr(feat), _lib.ptr(prob), _lib.ptr(pooled), _lib.ptr(aux), bs, D, Ca // D,
-                Hb, Wb, int(grid_num), float(grid_step), float(eps), int(act), _lib.stream_ptr(occ.device)))
-        ctx.save_for_backward(occ, feat, prob, pooled, aux)
-        ctx.cfg = (int(grid_num), float(grid_step), float(eps), int(act))
-        return prob, pooled
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_prob, grad_pooled):
-        occ, feat, prob, pooled, aux = ctx.saved_tensors
-        grid_num, grid_step, eps, act = ctx.cfg
-        bs, Hb, Wb, D = occ.shape
-        Ca = feat.shape[-1]
-        grad_prob = grad_prob.float().contiguous()
-        grad_pooled = grad_pooled.float().contiguous()
-        scratch = torch.empty_like(occ)
-        grad_occ = torch.zeros_like(occ)
-        grad_feat = torch.zeros_like(feat)
-        with torch.cuda.device(occ.device):
-            _lib.check(_lib.lib().vidar_latent_render_backward(
-                _lib.ptr(occ), _lib.ptr(feat), _lib.ptr(prob), _lib.ptr(pooled), _lib.ptr(aux), _lib.ptr(grad_prob),
-                _lib.ptr(grad_pooled), _lib.ptr(scratch), _lib.ptr(grad_occ), _lib.ptr(grad_feat), bs, D, Ca // D,
-                Hb, Wb, grid_num, grid_step, eps, act, _lib.stream_ptr(occ.device)))
-        return grad_occ, grad_feat, None, None, None, None
-
-
-class _ShardedLatentRenderCore(torch.autograd.Function):
-    """Same op with the BEV cells sharded over the ranks of `group` (SURVEY.md 8e).  Inputs and
-    outputs are replicated; each rank marches only its contiguous share of the cells and the
-    2.56 MB maps are all-reduced between the phases:
+    With `group` of more than one rank the BEV cells are sharded over its ranks (SURVEY.md 8e).  Inputs and
+    outputs are replicated; each rank marches only its contiguous share of the cells and the 2.56 MB maps are
+    all-reduced between the phases:
       forward : prob(local cells) -> all_reduce(prob) -> pooled(local cells) -> all_reduce(pooled)
       backward: pool-bwd(local) -> all_reduce(grad_prob_map, grad_feat) -> prob-bwd(local)
                 -> all_reduce(grad_occ).
     Upstream gradients must be replicated (they are: everything after this op is)."""
-
-    @staticmethod
-    def _range(n, group):
-        import torch.distributed as dist
-        from ..sharding import shard_range
-        lo, hi = shard_range(n, dist.get_rank(group), dist.get_world_size(group))
-        return lo, hi - lo
 
     @staticmethod
     def forward(ctx, occ, feat, grid_num, grid_step, eps, act, group):
@@ -91,21 +57,28 @@ class _ShardedLatentRenderCore(torch.autograd.Function):
         occ, feat = occ.float().contiguous(), feat.float().contiguous()
         bs, Hb, Wb, D = occ.shape
         Ca = feat.shape[-1]
-        c0, n = _ShardedLatentRenderCore._range(bs * Hb * Wb, group)
-        prob = torch.zeros_like(occ)
-        pooled = torch.zeros((bs, Hb * Wb, Ca), dtype=torch.float32, device=occ.device)
-        aux = torch.empty((3,) + tuple(occ.shape), dtype=torch.float32, device=occ.device)   # only this rank's cells are filled / read
+        if feat.shape[:3] != occ.shape[:3] or Ca % D != 0:
+            raise RuntimeError("feat must be [bs, Hb, Wb, pred_height * k]")
+        world, c0, n = _shard(bs * Hb * Wb, group)
+        alloc = torch.zeros if world > 1 else torch.empty           # other ranks' cells enter the all-reduce as 0
+        prob = alloc(tuple(occ.shape), dtype=torch.float32, device=occ.device)
+        pooled = alloc((bs, Hb * Wb, Ca), dtype=torch.float32, device=occ.device)
+        # the forward's sums, read by the backward instead of a second march (3 x 2.56 MB); only this rank's cells
+        # are filled / read
+        aux = torch.empty((3,) + tuple(occ.shape), dtype=torch.float32, device=occ.device)
         L = _lib.lib()
         with torch.cuda.device(occ.device):
             st = _lib.stream_ptr(occ.device)
             _lib.check(L.vidar_latent_prob_forward(_lib.ptr(occ), _lib.ptr(prob), _lib.ptr(aux), bs, D, Hb, Wb,
                                                    int(grid_num), float(grid_step), int(act), c0, n, st))
-            dist.all_reduce(prob, group=group)
+            if world > 1:
+                dist.all_reduce(prob, group=group)
             _lib.check(L.vidar_latent_pool_forward(_lib.ptr(prob), _lib.ptr(feat), _lib.ptr(pooled), _lib.ptr(aux), bs, D,
                                                    Ca // D, Hb, Wb, int(grid_num), float(grid_step), float(eps), c0, n, st))
-            dist.all_reduce(pooled, group=group)
+            if world > 1:
+                dist.all_reduce(pooled, group=group)
         ctx.save_for_backward(occ, feat, prob, pooled, aux)
-        ctx.cfg = (int(grid_num), float(grid_step), float(eps), int(act), group, c0, n)
+        ctx.cfg = (int(grid_num), float(grid_step), float(eps), int(act), group, world, c0, n)
         return prob, pooled
 
     @staticmethod
@@ -113,14 +86,20 @@ class _ShardedLatentRenderCore(torch.autograd.Function):
     def backward(ctx, grad_prob, grad_pooled):
         import torch.distributed as dist
         occ, feat, prob, pooled, aux = ctx.saved_tensors
-        grid_num, grid_step, eps, act, group, c0, n = ctx.cfg
+        grid_num, grid_step, eps, act, group, world, c0, n = ctx.cfg
         bs, Hb, Wb, D = occ.shape
         Ca = feat.shape[-1]
         grad_pooled = grad_pooled.float().contiguous()
-        # one buffer [2, ...] so the two partial maps travel in a single all-reduce
-        both = torch.zeros((2,) + tuple(occ.shape), dtype=torch.float32, device=occ.device) if Ca == D else None
-        gpm = both[0] if both is not None else torch.zeros_like(occ)
-        gfe = both[1] if both is not None else torch.zeros_like(feat)
+        both = None
+        if world > 1:
+            # one buffer [2, ...] so the two partial maps travel in a single all-reduce
+            both = torch.zeros((2,) + tuple(occ.shape), dtype=torch.float32, device=occ.device) if Ca == D else None
+            gpm = both[0] if both is not None else torch.zeros_like(occ)
+            gfe = both[1] if both is not None else torch.zeros_like(feat)
+        else:
+            # the total gradient reaching the prob map starts as the upstream grad_prob; phase 2 adds to it
+            gpm = torch.empty_like(occ).copy_(grad_prob)
+            gfe = torch.zeros_like(feat)
         grad_occ = torch.zeros_like(occ)
         L = _lib.lib()
         with torch.cuda.device(occ.device):
@@ -128,23 +107,18 @@ class _ShardedLatentRenderCore(torch.autograd.Function):
             _lib.check(L.vidar_latent_pool_backward(_lib.ptr(prob), _lib.ptr(feat), _lib.ptr(pooled), _lib.ptr(aux),
                                                     _lib.ptr(grad_pooled), _lib.ptr(gpm), _lib.ptr(gfe), bs, D, Ca // D,
                                                     Hb, Wb, grid_num, grid_step, eps, c0, n, st))
-            if both is not None:
-                dist.all_reduce(both, group=group)
-            else:
-                dist.all_reduce(gpm, group=group)
-                dist.all_reduce(gfe, group=group)
-            total = (gpm + grad_prob.float()).contiguous()
-            _lib.check(L.vidar_latent_prob_backward(_lib.ptr(occ), _lib.ptr(aux), _lib.ptr(total), _lib.ptr(grad_occ), bs, D,
+            if world > 1:
+                if both is not None:
+                    dist.all_reduce(both, group=group)
+                else:
+                    dist.all_reduce(gpm, group=group)
+                    dist.all_reduce(gfe, group=group)
+                gpm = (gpm + grad_prob.float()).contiguous()
+            _lib.check(L.vidar_latent_prob_backward(_lib.ptr(occ), _lib.ptr(aux), _lib.ptr(gpm), _lib.ptr(grad_occ), bs, D,
                                                     Hb, Wb, grid_num, grid_step, act, c0, n, st))
-            dist.all_reduce(grad_occ, group=group)
+            if world > 1:
+                dist.all_reduce(grad_occ, group=group)
         return grad_occ, gfe.clone() if both is not None else gfe, None, None, None, None, None
-
-
-def _group_world(group):
-    if group is None:
-        return 1
-    import torch.distributed as dist
-    return dist.get_world_size(group) if dist.is_initialized() else 1
 
 
 class _FusedLatentRendering(torch.autograd.Function):
@@ -165,11 +139,10 @@ class _FusedLatentRendering(torch.autograd.Function):
         only its rows of the output are returned (row-wise consumers -- LayerNorm, FFN -- need no more): the two
         41 MB all-gathers of the replicated mode disappear."""
         import torch.distributed as dist
-        from ..sharding import gather_rows, shard_range
+        from ..sharding import gather_rows
         _lib.require_cuda(embed=embed.contiguous())
         params = [p.detach().float().contiguous() for p in (w_occ, b_occ, w_feat, b_feat, w_b, b_b)]
         w_occ, b_occ, w_feat, b_feat, w_b, b_b = params
-        world = _group_world(group)
         D, A = w_occ.shape[0], w_feat.shape[0]
         if rows_io is not None:
             bs, Hb, Wb = rows_io
@@ -177,8 +150,8 @@ class _FusedLatentRendering(torch.autograd.Function):
         else:
             bs, Hb, Wb, E = embed.shape
         R = bs * Hb * Wb
-        c0, c1 = shard_range(R, dist.get_rank(group), world) if world > 1 else (0, R)
-        n = c1 - c0
+        world, c0, n = _shard(R, group)
+        c1 = c0 + n
         if rows_io is not None:
             if embed.numel() != n * E:
                 raise RuntimeError(f"rows_io: expected this rank's {n} rows of {E} channels, got {tuple(embed.shape)}")
@@ -285,11 +258,7 @@ def fused_projection_supported(E, D, A):
 def latent_render_core(occ, feat, grid_num, grid_step, eps, act, group=None):
     """(occ, feat) -> (prob, pooled).  `group`: a torch.distributed process group over which the BEV
     cells are sharded (None or a 1-rank group = single GPU)."""
-    if group is not None:
-        import torch.distributed as dist
-        if dist.is_initialized() and dist.get_world_size(group) > 1:
-            return _ShardedLatentRenderCore.apply(occ, feat, grid_num, grid_step, eps, act, group)
-    return _LatentRenderCore.apply(occ, feat, grid_num, grid_step, eps, act)
+    return _LatentRenderCore.apply(occ, feat, grid_num, grid_step, eps, act, group)
 
 
 @ATTENTION.register_module()
