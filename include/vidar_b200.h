@@ -632,6 +632,31 @@ int vidar_dcnv3_backward(const void* input, const void* offset, const void* mask
 int vidar_grid_mask_apply(const void* x, const void* offset, void* out, int dtype, int N, int C, int h, int w, int d,
                           int l, int st_h, int st_w, int r, int use_h, int use_w, int mode, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (x) The multi-view image pipeline of the pre-training configs (datasets/pipelines/transform_3d.py
+ * PhotoMetricDistortionMultiViewImage, NormalizeMultiviewImage, PadMultiViewImage; augmentation.py
+ * CropResizeFlipImage) from one frame's uint8 images, in two launches on `stream`, bit for bit the reference's
+ * cv2 / PIL / numpy statements.
+ *   src      [N, H, W, 3] uint8 BGR (device), 1 <= N <= 64
+ *   mid      [N, crop_h, out_w, 3] uint8 (device): the intermediate between the two passes, the only scratch
+ *   out      [N, 3, Hp, Wp] float32 (device), every element written
+ *   photo_i  host int32 [N, 8] (brightness, contrast, saturation, hue gates, mode 1, perm[3]) and
+ *   photo_f  host float [N, 4] (brightness delta, contrast factor, saturation factor, hue delta): one image's
+ *            photometric draws each (both NULL: no photometric step); copied into the kernel arguments
+ *   crop box (crop_x, crop_y, crop_x + crop_w, crop_y + crop_h) of the image, zero outside it; then Pillow's
+ *   bicubic resize to (out_w, out_h) and, with flip, the left-right flip
+ *   htaps    [out_w, 2 + hk] int32 (device): per output column (xmin, count, count weights in 2^-22, zero-padded
+ *            to hk); given exactly when out_w != crop_w.  vtaps [out_h, 2 + vk] likewise for rows.
+ *   to_rgb swaps channels 0 and 2; then out = f32(double(x - mean[c]) * stdinv[c]) with mean host float[3] and
+ *   stdinv host double[3]; pixels at y >= out_h or x >= out_w are pad_val[c] (host float[3]).
+ * Needs every side in [1, 8192], out_h <= Hp, out_w <= Wp, gates 0 or 1, perm a permutation of (0, 1, 2).  No
+ * host sync. */
+int vidar_image_aug_apply(const unsigned char* src, unsigned char* mid, float* out, int N, int H, int W,
+                          const int32_t* photo_i, const float* photo_f, int crop_x, int crop_y, int crop_w,
+                          int crop_h, int out_w, int out_h, const int32_t* htaps, int hk, const int32_t* vtaps, int vk,
+                          int flip, int to_rgb, const float* mean, const double* stdinv, const float* pad_val, int Hp,
+                          int Wp, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -193,3 +193,69 @@ def load(dotted):
     """e.g. load('modules.spatial_cross_attention') -> module object of the reference file."""
     install()
     return importlib.import_module(f"vidar_ref.{dotted}")
+
+
+REF_PIPELINES = "/root/reference/projects/mmdet3d_plugin/datasets/pipelines"
+
+
+def install_pipelines():
+    """Load the reference's image transforms (datasets/pipelines/transform_3d.py and augmentation.py) with
+    stand-ins for what they take from mmcv and mmdet: `bgr2hsv`, `hsv2bgr`, `imnormalize`, `impad`,
+    `impad_to_multiple`, `parallel.DataContainer` and `datasets.builder.PIPELINES`.  The stand-ins restate mmcv 1.x's
+    published definitions (mmcv/image/colorspace.py, photometric.py, geometric.py): the same cv2 calls with the same
+    arguments.  -> {class name: class} of both files."""
+    import numbers
+
+    import cv2
+    import numpy as np
+    install()
+
+    def imnormalize(img, mean, std, to_rgb=True):
+        img = img.copy().astype(np.float32)
+        assert img.dtype != np.uint8
+        mean = np.float64(mean.reshape(1, -1))
+        stdinv = 1 / np.float64(std.reshape(1, -1))
+        if to_rgb:
+            cv2.cvtColor(img, cv2.COLOR_BGR2RGB, img)
+        cv2.subtract(img, mean, img)
+        cv2.multiply(img, stdinv, img)
+        return img
+
+    def impad(img, *, shape=None, padding=None, pad_val=0, padding_mode="constant"):
+        assert (shape is not None) ^ (padding is not None)
+        if shape is not None:
+            padding = (0, 0, shape[1] - img.shape[1], shape[0] - img.shape[0])
+        if isinstance(pad_val, tuple):
+            assert len(pad_val) == img.shape[-1]
+        elif not isinstance(pad_val, numbers.Number):
+            raise TypeError(f"pad_val must be a int or a tuple. But received {type(pad_val)}")
+        border = {"constant": cv2.BORDER_CONSTANT}[padding_mode]
+        return cv2.copyMakeBorder(img, padding[1], padding[3], padding[0], padding[2], border, value=pad_val)
+
+    def impad_to_multiple(img, divisor, pad_val=0):
+        pad_h = int(np.ceil(img.shape[0] / divisor)) * divisor
+        pad_w = int(np.ceil(img.shape[1] / divisor)) * divisor
+        return impad(img, shape=(pad_h, pad_w), pad_val=pad_val)
+
+    class DataContainer:
+        def __init__(self, data, stack=False, padding_value=0, cpu_only=False, pad_dims=2):
+            self.data, self.stack, self.cpu_only = data, stack, cpu_only
+
+    mmcv = sys.modules["mmcv"]
+    mmcv.bgr2hsv = lambda img: cv2.cvtColor(img, cv2.COLOR_BGR2HSV)
+    mmcv.hsv2bgr = lambda img: cv2.cvtColor(img, cv2.COLOR_HSV2BGR)
+    mmcv.imnormalize, mmcv.impad, mmcv.impad_to_multiple = imnormalize, impad, impad_to_multiple
+    parallel = types.ModuleType("mmcv.parallel")
+    parallel.DataContainer = DataContainer
+    sys.modules["mmcv.parallel"] = parallel
+    pipelines = _Registry()
+    for name in ("mmdet.datasets", "mmdet.datasets.builder"):
+        m = _Permissive(name)
+        m.__path__ = []
+        m.PIPELINES = pipelines
+        sys.modules[name] = m
+    for fname in ("transform_3d.py", "augmentation.py"):
+        spec = importlib.util.spec_from_file_location(f"vidar_ref_pipelines_{fname[:-3]}",
+                                                      os.path.join(REF_PIPELINES, fname))
+        spec.loader.exec_module(importlib.util.module_from_spec(spec))
+    return pipelines.modules

@@ -1,0 +1,360 @@
+"""The multi-view image pipeline of ViDAR's pre-training configs on the H100 (vidar_1_8_nusc_3future.py:279-317):
+
+    PhotoMetricDistortionMultiViewImage -> CropResizeFlipImage(ida_aug_conf) -> NormalizeMultiviewImage
+      -> PadMultiViewImage
+
+The four classes take the reference's constructor arguments (datasets/pipelines/transform_3d.py:7-185,
+augmentation.py:10-202).  Used as dataloader transforms, their `__call__(results)` does only the host work: the
+same draws from the same generators in the same order (numpy's global generator for the photometric gates and
+factors and the flip, the stdlib `random` for the resize, cached in `results['aug_param']` so that the later
+frames of a queue reuse it), the `cam2img` / `lidar2img` / `img_norm_cfg` / shape keys as the reference sets them,
+and a record of what to do to the pixels in `results['img_aug']`.  `results['img']` is left as loaded (uint8).
+
+`apply_multiview(img, results)` then runs the recorded chain on the device, on the current stream, in two launches
+(csrc/image_aug.cu, include/vidar_b200.h §x): uint8 [N, H, W, 3] BGR in, float32 [N, 3, Hp, Wp] out, bit for bit
+what the reference's cv2 / PIL / numpy statements give -- including numpy's wrapping `np.uint8` cast of pixels
+that brightness and contrast push past 255 or below 0.  The per-image draws travel in the kernel arguments; the
+resample taps are computed on the host in float64 by Pillow's rules, cached per (input size, output size, device)
+and uploaded once from pinned memory without blocking.  No host sync.  CUDA tensors only.
+"""
+import random
+from dataclasses import dataclass, field
+
+import numpy as np
+import torch
+
+from . import _lib
+
+MAX_IMAGES = 64
+MAX_SIDE = 8192
+PRECISION_BITS = 22
+
+
+@dataclass(frozen=True)
+class PhotoDraw:
+    """One image's photometric draws; None where the step's gate was closed.  `mode` 1 puts contrast before the
+    HSV round trip, 0 after it; `perm` is the channel permutation."""
+    delta: float = None
+    mode: int = 0
+    alpha: float = None
+    sat: float = None
+    hue: float = None
+    perm: tuple = None
+
+
+@dataclass
+class ImageAugPlan:
+    """What `apply_multiview` does to one frame's images, recorded by the transforms in `results['img_aug']`."""
+    n: int
+    src_hw: tuple
+    photo: list = None                 # [PhotoDraw] per image, or None
+    crop: tuple = None                 # (x0, y0, x1, y1)
+    dims: tuple = None                 # (w, h) after the resize
+    flip: bool = False
+    mean: np.ndarray = field(default_factory=lambda: np.zeros(3, np.float32))
+    std: np.ndarray = field(default_factory=lambda: np.ones(3, np.float32))
+    to_rgb: bool = False
+    normalized: bool = False
+    pad_hw: tuple = None
+    pad_val: tuple = (0.0, 0.0, 0.0)
+
+    @property
+    def hw(self):
+        """(h, w) of the images after the steps recorded so far."""
+        if self.pad_hw is not None:
+            return self.pad_hw
+        return (self.dims[1], self.dims[0]) if self.dims is not None else tuple(self.src_hw)
+
+
+def _plan(results, step):
+    """results['img_aug'], created at the first step; raises when `step` comes out of the order the device chain
+    runs (photometric, crop / resize / flip, normalise, pad; each at most once)."""
+    imgs = results["img"]
+    plan = results.get("img_aug")
+    if plan is None:
+        shapes = {tuple(im.shape) for im in imgs}
+        if len(imgs) == 0 or len(shapes) != 1 or len(next(iter(shapes))) != 3 or next(iter(shapes))[2] != 3:
+            raise ValueError(f"image pipeline: results['img'] must be images of one [H, W, 3] shape (got {shapes})")
+        plan = results["img_aug"] = ImageAugPlan(len(imgs), next(iter(shapes))[:2])
+    elif plan.n != len(imgs):
+        raise ValueError(f"image pipeline: {len(imgs)} images, the recorded steps saw {plan.n}")
+    done = {"photo": plan.photo is not None, "crop": plan.crop is not None, "norm": plan.normalized,
+            "pad": plan.pad_hw is not None}
+    order = ["photo", "crop", "norm", "pad"]
+    later = order[order.index(step):]
+    if any(done[s] for s in later):
+        raise ValueError(f"image pipeline: step '{step}' after {[s for s in order if done[s]]}; the device chain "
+                         "runs photometric distortion, crop / resize / flip, normalisation and padding in this order, "
+                         "each at most once")
+    return plan
+
+
+class PhotoMetricDistortionMultiViewImage:
+    """transform_3d.py:98-185: per image, numpy draws for brightness, mode, contrast, saturation, hue and the
+    channel swap, in the reference's order (contrast before the HSV round trip when mode == 1)."""
+
+    def __init__(self, brightness_delta=32, contrast_range=(0.5, 1.5), saturation_range=(0.5, 1.5), hue_delta=18):
+        self.brightness_delta = brightness_delta
+        self.contrast_lower, self.contrast_upper = contrast_range
+        self.saturation_lower, self.saturation_upper = saturation_range
+        self.hue_delta = hue_delta
+
+    def draw(self):
+        """One image's draws from numpy's global generator -> PhotoDraw."""
+        rnd = np.random
+        delta = alpha = sat = hue = perm = None
+        if rnd.randint(2):
+            delta = rnd.uniform(-self.brightness_delta, self.brightness_delta)
+        mode = rnd.randint(2)
+        if mode == 1 and rnd.randint(2):
+            alpha = rnd.uniform(self.contrast_lower, self.contrast_upper)
+        if rnd.randint(2):
+            sat = rnd.uniform(self.saturation_lower, self.saturation_upper)
+        if rnd.randint(2):
+            hue = rnd.uniform(-self.hue_delta, self.hue_delta)
+        if mode == 0 and rnd.randint(2):
+            alpha = rnd.uniform(self.contrast_lower, self.contrast_upper)
+        if rnd.randint(2):
+            perm = tuple(int(c) for c in rnd.permutation(3))
+        return PhotoDraw(delta, int(mode), alpha, sat, hue, perm)
+
+    def __call__(self, results):
+        plan = _plan(results, "photo")
+        plan.photo = [self.draw() for _ in range(plan.n)]
+        return results
+
+
+class CropResizeFlipImage:
+    """augmentation.py:9-202: one crop / resize / flip per frame, drawn (stdlib `random.choice` for the height,
+    `np.random.choice([0, 1])` for the flip when `rand_flip`) or taken from results['aug_param'].  Updates
+    `cam2img[:3, :3]` with the crop / resize matrix (which, as in the reference, leaves the flip out) and sets
+    `lidar2img = cam2img @ lidar2cam`."""
+
+    def __init__(self, data_aug_conf=None, training=True, debug=False):
+        if debug:
+            raise ValueError("CropResizeFlipImage: debug=True (drawing projected points into saved images) is not "
+                             "supported")
+        self.data_aug_conf = data_aug_conf
+        self.training = training
+        self.debug = debug
+
+    def _sample_augmentation(self, results):
+        if "CropResizeFlipImage_param" in results["aug_param"]:
+            return results["aug_param"]["CropResizeFlipImage_param"]
+        conf = self.data_aug_conf
+        crop = conf["crop"]
+        resized_h = random.choice(conf["reisze"])
+        if not self.training and len(conf["reisze"]) != 1:
+            raise ValueError("CropResizeFlipImage: training=False needs exactly one entry in 'reisze'")
+        resized_w = resized_h / (crop[3] - crop[1]) * (crop[2] - crop[0])
+        resize = resized_h / (crop[3] - crop[1])
+        resize_dims = (int(resized_w), int(resized_h))
+        flip = False
+        if self.training and conf["rand_flip"] and np.random.choice([0, 1]):
+            flip = True
+        results["aug_param"]["CropResizeFlipImage_param"] = (resize, resize_dims, crop, flip)
+        return resize, resize_dims, crop, flip
+
+    def __call__(self, results):
+        if "mono_ann_idx" in results:
+            raise ValueError("CropResizeFlipImage: the DD3D mono annotations ('mono_ann_idx') are not supported")
+        plan = _plan(results, "crop")
+        if "aug_param" not in results:
+            results["aug_param"] = {}
+        resize, resize_dims, crop, flip = self._sample_augmentation(results)
+        x0, y0, x1, y1 = (int(round(v)) for v in crop)
+        w, h = (int(v) for v in resize_dims)
+        if not (0 < x1 - x0 <= MAX_SIDE and 0 < y1 - y0 <= MAX_SIDE and 0 < w <= MAX_SIDE and 0 < h <= MAX_SIDE):
+            raise ValueError(f"CropResizeFlipImage: crop {crop} -> {resize_dims} is outside 1..{MAX_SIDE} pixels")
+        ida_mat = np.eye(3)
+        ida_mat[:2, :2] *= resize
+        ida_mat[:2, 2] -= np.array(crop[:2]) * resize
+        for i in range(plan.n):
+            results["cam2img"][i][:3, :3] = np.matmul(ida_mat, results["cam2img"][i][:3, :3])
+        results["lidar2img"] = [np.matmul(results["cam2img"][i], results["lidar2cam"][i])
+                                for i in range(len(results["lidar2cam"]))]
+        plan.crop, plan.dims, plan.flip = (x0, y0, x1, y1), (w, h), bool(flip)
+        return results
+
+
+class NormalizeMultiviewImage:
+    """transform_3d.py:61-95 (mmcv.imnormalize): optional BGR -> RGB, then (x - mean) / std per channel."""
+
+    def __init__(self, mean, std, to_rgb=True):
+        self.mean = np.array(mean, dtype=np.float32)
+        self.std = np.array(std, dtype=np.float32)
+        self.to_rgb = to_rgb
+        if self.mean.shape != (3,) or self.std.shape != (3,):
+            raise ValueError("NormalizeMultiviewImage: mean and std need 3 values")
+
+    def __call__(self, results):
+        plan = _plan(results, "norm")
+        plan.mean, plan.std, plan.to_rgb, plan.normalized = self.mean, self.std, bool(self.to_rgb), True
+        results["img_norm_cfg"] = dict(mean=self.mean, std=self.std, to_rgb=self.to_rgb)
+        return results
+
+
+class PadMultiViewImage:
+    """transform_3d.py:7-58 (mmcv.impad / impad_to_multiple): bottom / right padding to `size` or to multiples of
+    `size_divisor`.  A number `pad_val` fills channel 0 only and leaves 0 in the others, as cv2.copyMakeBorder does
+    with a scalar; a 3-tuple fills each channel."""
+
+    def __init__(self, size=None, size_divisor=None, pad_val=0):
+        if (size is None) == (size_divisor is None):
+            raise ValueError("PadMultiViewImage: give exactly one of size and size_divisor")
+        self.size = size
+        self.size_divisor = size_divisor
+        self.pad_val = pad_val
+
+    def __call__(self, results):
+        plan = _plan(results, "pad")
+        h, w = plan.hw
+        if self.size is not None:
+            hp, wp = int(self.size[0]), int(self.size[1])
+            if hp < h or wp < w:
+                raise ValueError(f"PadMultiViewImage: size {self.size} is smaller than the image ({h}, {w})")
+        else:
+            d = self.size_divisor
+            hp, wp = -(-h // d) * d, -(-w // d) * d
+        if hp > MAX_SIDE or wp > MAX_SIDE:
+            raise ValueError(f"PadMultiViewImage: padded size ({hp}, {wp}) is over {MAX_SIDE}")
+        pv = self.pad_val
+        if isinstance(pv, tuple):
+            if len(pv) != 3:
+                raise ValueError(f"PadMultiViewImage: a tuple pad_val needs 3 values (got {pv})")
+            plan.pad_val = tuple(float(v) for v in pv)
+        else:
+            plan.pad_val = (float(pv), 0.0, 0.0)
+        results["ori_shape"] = [(h, w, 3)] * plan.n
+        plan.pad_hw = (hp, wp)
+        results["img_shape"] = [(hp, wp, 3)] * plan.n
+        results["pad_shape"] = [(hp, wp, 3)] * plan.n
+        results["pad_fixed_size"] = self.size
+        results["pad_size_divisor"] = self.size_divisor
+        return results
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# device step
+# ---------------------------------------------------------------------------------------------------------------
+def bicubic_taps(in_size, out_size):
+    """Pillow's antialiased BICUBIC taps (Resample.c precompute_coeffs + normalize_coeffs_8bpc), in float64 in its
+    order of operations -> int32 [out_size, 2 + ksize]: per output pixel (xmin, count, weights in 2^-22 units)."""
+    scale = in_size / out_size
+    filterscale = max(scale, 1.0)
+    support = 2.0 * filterscale
+    ksize = int(np.ceil(support)) * 2 + 1
+    ss = 1.0 / filterscale
+    table = np.zeros((out_size, 2 + ksize), np.int32)
+    for xx in range(out_size):
+        center = (xx + 0.5) * scale
+        xmin = max(int(center - support + 0.5), 0)
+        xmax = min(int(center + support + 0.5), in_size) - xmin
+        ws = []
+        for x in range(xmax):
+            t = abs((x + xmin - center + 0.5) * ss)
+            if t < 1.0:
+                ws.append((1.5 * t - 2.5) * t * t + 1)
+            elif t < 2.0:
+                ws.append((((t - 5) * t + 8) * t - 4) * -0.5)
+            else:
+                ws.append(0.0)
+        total = 0.0
+        for v in ws:
+            total += v
+        table[xx, 0], table[xx, 1] = xmin, xmax
+        for x, v in enumerate(ws):
+            v = v / total if total != 0.0 else v
+            table[xx, 2 + x] = int(-0.5 + v * (1 << PRECISION_BITS)) if v < 0 else int(0.5 + v * (1 << PRECISION_BITS))
+    return table
+
+
+_TAPS = {}
+
+
+def _taps(in_size, out_size, device):
+    """Device copy of bicubic_taps(in_size, out_size), made once per device from pinned memory without blocking
+    (the pinned buffer is kept with it, so the copy never reads freed memory)."""
+    key = (in_size, out_size, device)
+    if key not in _TAPS:
+        host = torch.from_numpy(bicubic_taps(in_size, out_size)).pin_memory()
+        _TAPS[key] = (host.to(device, non_blocking=True), host)
+    return _TAPS[key][0]
+
+
+def _check(img, plan, cams):
+    """Every argument check of apply_multiview, before any CUDA call; the device check comes last, so the others can
+    be tested without a GPU."""
+    if not isinstance(plan, ImageAugPlan):
+        raise ValueError("apply_multiview: results has no recorded image steps (run the transforms first)")
+    if plan.photo is not None and plan.crop is None:
+        raise ValueError("apply_multiview: photometric distortion without CropResizeFlipImage is not supported (the "
+                         "uint8 cast of the distorted pixels happens there)")
+    if not isinstance(img, torch.Tensor):
+        raise TypeError(f"apply_multiview: img must be a tensor (got {type(img).__name__})")
+    if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[-1] != 3:
+        raise ValueError(f"apply_multiview: img must be uint8 [N, H, W, 3] (got {img.dtype} {tuple(img.shape)})")
+    if tuple(img.shape[1:3]) != tuple(plan.src_hw):
+        raise ValueError(f"apply_multiview: images are {tuple(img.shape[1:3])}, the steps were recorded for "
+                         f"{tuple(plan.src_hw)}")
+    if len(cams) != img.shape[0] or any(not 0 <= c < plan.n for c in cams) or len(set(cams)) != len(cams):
+        raise ValueError(f"apply_multiview: cams {list(cams)} must name the {img.shape[0]} images given, out of "
+                         f"{plan.n}")
+    if not 1 <= img.shape[0] <= MAX_IMAGES:
+        raise ValueError(f"apply_multiview: {img.shape[0]} images per call (at most {MAX_IMAGES})")
+    if not img.is_cuda:
+        raise RuntimeError("apply_multiview: img must be a CUDA tensor")
+
+
+def apply_multiview(img, results, cams=None):
+    """Run the steps recorded in results['img_aug'] on img, uint8 [N, H, W, 3] BGR on a CUDA device -> float32
+    [N, 3, Hp, Wp], on the current stream.  `cams`: which of the frame's images img holds (default all, in order),
+    so a rank can process only its cameras with the frame's draws."""
+    plan = results.get("img_aug") if isinstance(results, dict) else None
+    cams = list(range(plan.n)) if cams is None and isinstance(plan, ImageAugPlan) else list(cams or [])
+    _check(img, plan, cams)
+    n, H, W = img.shape[:3]
+    x0, y0, x1, y1 = plan.crop if plan.crop is not None else (0, 0, W, H)
+    ow, oh = plan.dims if plan.dims is not None else (W, H)
+    cw, ch = x1 - x0, y1 - y0
+    hp, wp = plan.pad_hw if plan.pad_hw is not None else (oh, ow)
+    photo_i = photo_f = None
+    if plan.photo is not None:
+        photo_i = np.zeros((n, 8), np.int32)
+        photo_f = np.zeros((n, 4), np.float32)
+        for k, c in enumerate(cams):
+            d = plan.photo[c]
+            photo_i[k] = (d.delta is not None, d.alpha is not None, d.sat is not None, d.hue is not None,
+                          d.mode == 1, *(d.perm or (0, 1, 2)))
+            photo_f[k] = [v if v is not None else 0.0 for v in (d.delta, d.alpha, d.sat, d.hue)]
+    mean = np.ascontiguousarray(plan.mean, np.float32)
+    stdinv = 1 / plan.std.astype(np.float64)
+    pad_val = np.asarray(plan.pad_val, np.float32)
+    img = img.contiguous()
+    dev = img.device
+    with torch.cuda.device(dev):
+        htaps = _taps(cw, ow, dev) if ow != cw else None
+        vtaps = _taps(ch, oh, dev) if oh != ch else None
+        mid = torch.empty((n, ch, ow, 3), dtype=torch.uint8, device=dev)
+        out = torch.empty((n, 3, hp, wp), dtype=torch.float32, device=dev)
+
+        def host(a):
+            return None if a is None else a.ctypes.data
+
+        _lib.check(_lib.lib().vidar_image_aug_apply(
+            _lib.ptr(img), _lib.ptr(mid), _lib.ptr(out), n, H, W, host(photo_i), host(photo_f), x0, y0, cw, ch, ow,
+            oh, _lib.ptr(htaps), htaps.shape[1] - 2 if htaps is not None else 0, _lib.ptr(vtaps),
+            vtaps.shape[1] - 2 if vtaps is not None else 0, int(plan.flip), int(plan.to_rgb), host(mean),
+            host(stdinv), host(pad_val), hp, wp, _lib.stream_ptr(dev)))
+    return out
+
+
+def config_pipeline(ida_aug_conf=None):
+    """The four transforms of the pre-training config (vidar_1_8_nusc_3future.py:41-51, 303-314)."""
+    conf = ida_aug_conf if ida_aug_conf is not None else dict(
+        reisze=[720, 765, 810, 855, 900, 945, 990, 1035, 1080], crop=(0, 0, 1600, 900), H=900, W=1600, rand_flip=True)
+    return [PhotoMetricDistortionMultiViewImage(),
+            CropResizeFlipImage(data_aug_conf=conf, training=True, debug=False),
+            NormalizeMultiviewImage(mean=[103.530, 116.280, 123.675], std=[1.0, 1.0, 1.0], to_rgb=False),
+            PadMultiViewImage(size_divisor=32)]
+

@@ -29,6 +29,7 @@ Sharding over a process group (one sample on all ranks -- the reference has repl
     (`sharding.allreduce_partial_grads`), the counterpart of the reference's DDP all-reduce
     (apis/mmdet_train.py:72-81).
 """
+import copy
 import math
 
 import numpy as np
@@ -38,6 +39,7 @@ import torch.nn.functional as F
 
 from . import bev_geometry, sca, sharding, synthetic
 from . import modules as _modules  # noqa: F401  (registers the attention classes)
+from . import image_aug
 from .grid_mask import GridMask
 from .head import ViDARRayHead
 from .modules.deform_attn import _linear
@@ -285,12 +287,24 @@ class SyntheticViDAR(nn.Module):
     from numpy's global generator, so under a process group every rank must seed numpy with the same value -- as the
     reference's training script does (mmdet's init_random_seed broadcasts rank 0's seed, set_random_seed seeds numpy
     on every rank) -- and every rank draws once per call, also a rank whose backbone runs no camera; then each rank
-    masks its own cameras with the same mask.  The default False leaves the graph as it was."""
+    masks its own cameras with the same mask.  The default False leaves the graph as it was.
+
+    `image_pipeline=True` runs the pre-training config's image transforms (vidar_1_8_nusc_3future.py:303-314,
+    `vidar_b200.image_aug.config_pipeline`, held in `self.image_transforms`) on every history and current frame, in
+    the dataset's order (oldest first; the first frame draws the crop / resize / flip and the later ones reuse it
+    through `aug_param`): forward_train then takes uint8 BGR frames img [1, T, cams, H, W, 3] with `cam2img` and
+    `lidar2cam` [1, cams, 4, 4] instead of lidar2img (`synthetic_sample(..., raw_images=True)`), and each frame's
+    `img_metas` (lidar2img, img_shape = the padded shape) come from its transforms.  The host draws of all frames
+    come first, as the dataloader makes them before the step; then each frame's images go through
+    `apply_multiview` before the backbone (and GridMask, when on).  bs must be 1 (samples_per_gpu=1).  Under a
+    process group every rank draws for all cameras -- numpy and `random` seeded alike on every rank -- and processes
+    only its backbone cameras.  The default False leaves the graph as it was."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
                  latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None,
-                 grid_mask=False):
+                 grid_mask=False, image_pipeline=False):
         super().__init__()
+        self.image_transforms = image_aug.config_pipeline() if image_pipeline else None
         if backbone_autocast not in (None, torch.float16, torch.bfloat16):
             raise ValueError(f"backbone_autocast must be None, torch.float16 or torch.bfloat16 (got {backbone_autocast})")
         self.backbone_autocast = backbone_autocast
@@ -364,12 +378,22 @@ class SyntheticViDAR(nn.Module):
     # ---- image features of one frame -> [cams, K, bs, C] (only this rank's SCA cameras are filled) ----
     def extract_feat(self, img, draw=None):
         """img [bs, cams, 3, H, W] -> (feat_flatten [cams, K, bs, C], spatial_shapes, level_start_index).  `draw`: a
-        GridMask draw (`self.grid_mask.sample`) applied to the images before the backbone."""
+        GridMask draw (`self.grid_mask.sample`) applied to the images before the backbone.  With the image pipeline,
+        img is (results of the frame's transforms, its uint8 frames [1, cams, H, W, 3])."""
         import torch.distributed as dist
-        bs = img.shape[0]
         world = dist.get_world_size(self.process_group) if self.process_group is not None else 1
         rank = dist.get_rank(self.process_group) if world > 1 else 0
         mine = self.my_backbone_cams if world > 1 else list(range(self.num_cams))
+        if self.image_transforms is not None:
+            results, raw = img
+            pipe = image_aug.apply_multiview(raw[0, mine], results, mine) if mine else None
+            if mine == list(range(self.num_cams)):
+                img = pipe[None]
+            else:                                       # only this rank's cameras are filled (and read)
+                img = raw.new_empty((1, self.num_cams, 3, *results["img_aug"].pad_hw), dtype=torch.float32)
+                if mine:
+                    img[0, mine] = pipe
+        bs = img.shape[0]
         per_cam = {}
         if mine:
             x = img[:, mine].reshape(bs * len(mine), *img.shape[2:])
@@ -469,27 +493,57 @@ class SyntheticViDAR(nn.Module):
         return torch.stack(preds, 1)
 
     # ---- history BEV, current BEV, future roll-outs, head (vidar.py:239-387 and :392-437) ----
-    def _next_bev_preds(self, img, lidar2img, can_bus, future_frames):
+    def frame_transforms(self, img, cam2img, lidar2cam):
+        """The host half of the image pipeline for every frame of img uint8 [1, T, cams, H, W, 3], in the dataset's
+        order -> [results] per frame (`apply_multiview` input and img_metas)."""
+        if img.dim() != 6 or img.shape[0] != 1 or img.dtype != torch.uint8 or img.shape[-1] != 3:
+            raise ValueError(f"image_pipeline: img must be uint8 [1, T, cams, H, W, 3] (bs 1, samples_per_gpu=1; got "
+                             f"{img.dtype} {tuple(img.shape)})")
+        if cam2img is None or lidar2cam is None:
+            raise ValueError("image_pipeline: forward needs cam2img and lidar2cam")
+        frames, aug_param = [], None
+        for t in range(img.shape[1]):
+            results = dict(img=list(img[0, t]), cam2img=[np.array(m, np.float64) for m in cam2img[0]],
+                           lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]])
+            if aug_param is not None:
+                results["aug_param"] = copy.deepcopy(aug_param)
+            for transform in self.image_transforms:
+                results = transform(results)
+            aug_param = copy.deepcopy(results["aug_param"])
+            frames.append(results)
+        return frames
+
+    def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None):
         """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + future_frames, inter, pred_frame, bs, Q, 16]: the history
         BEV of the first T - 1 frames (no grad), the current frame's BEV as ref_bev, `future_frames` roll-outs with a
-        queue of length 1, then the head."""
+        queue of length 1, then the head.  With the image pipeline, img is uint8 [1, T, cams, H, W, 3] and the
+        camera matrices come from cam2img / lidar2cam."""
         bs, T = img.shape[:2]
         dev = img.device
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
-        img_metas = [dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)]) for b in range(bs)]
+        if self.image_transforms is not None:
+            frames = self.frame_transforms(img, cam2img, lidar2cam)
+            inputs = [(r, img[:, t]) for t, r in enumerate(frames)]
+            metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"])] for r in frames]
+            hw = frames[-1]["img_aug"].pad_hw
+        else:
+            inputs = [img[:, t] for t in range(T)]
+            metas = [[dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)])
+                      for b in range(bs)]] * T
+            hw = img.shape[-2:]
         prev_bev = None
         if self.grid_mask is not None and T > 1:                                     # the history's eval-mode call
-            self.grid_mask.sample(*img.shape[-2:], training=False)
+            self.grid_mask.sample(*hw, training=False)
         with torch.no_grad():                                                        # obtain_history_bev
             for t in range(T - 1):
-                feats, shapes, lsi = self.extract_feat(img[:, t])
+                feats, shapes, lsi = self.extract_feat(inputs[t])
                 self._mark(f"hist{t}.backbone")
-                prev_bev = self.encode(feats, shapes, lsi, img_metas, can_bus, prev_bev)
+                prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
                 self._mark(f"hist{t}.encoder")
-        draw = self.grid_mask.sample(*img.shape[-2:]) if self.grid_mask is not None else None
-        feats, shapes, lsi = self.extract_feat(img[:, T - 1], draw)
+        draw = self.grid_mask.sample(*hw) if self.grid_mask is not None else None
+        feats, shapes, lsi = self.extract_feat(inputs[T - 1], draw)
         self._mark("cur.backbone")
-        ref_bev = self.encode(feats, shapes, lsi, img_metas, can_bus, prev_bev)
+        ref_bev = self.encode(feats, shapes, lsi, metas[T - 1], can_bus, prev_bev)
         self._mark("cur.encoder")
         inter_num = len(self.bev_pred_head)
         next_bev_feats = [ref_bev.unsqueeze(0).repeat(inter_num, 1, 1, 1)]
@@ -503,11 +557,12 @@ class SyntheticViDAR(nn.Module):
         return self.forward_head(next_bev_feats)                                        # [F, inter, pred_frame, bs, Q, 16]
 
     # ---- one training forward (vidar.py:239-387) -> dict of losses ----
-    def forward_train(self, img, lidar2img, gt_points, can_bus=None):
+    def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None):
         """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
         (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
-        frame index 0 = current .. future_frames)."""
-        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames)
+        frame index 0 = current .. future_frames).  With the image pipeline: img uint8 [1, T, cams, H, W, 3] and
+        host cam2img / lidar2cam [1, cams, 4, 4]; lidar2img is not read."""
+        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames, cam2img, lidar2cam)
         valid_frames = list(range(1 + self.future_frames))
         losses = {}
         for i in range(self.pred_frame_num):                                            # vidar_head_v1.py:179-218
@@ -545,11 +600,23 @@ class SyntheticViDAR(nn.Module):
 # ------------------------------------------------------------------------------------------------
 # synthetic sample + step
 # ------------------------------------------------------------------------------------------------
-def synthetic_sample(device, frames=4, cams=6, img_hw=synthetic.IMG_HW, rays_per_frame=10000, future_frames=3, seed=0,
-                     bev_hw=(BEV_H, BEV_W)):
-    """6 x 3 x 928 x 1600 N(0,1) frames, a nuScenes-like rig, LiDAR-like future point clouds (SURVEY.md 8d cfg4)."""
+def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000, future_frames=3, seed=0,
+                     bev_hw=(BEV_H, BEV_W), raw_images=False):
+    """6 x 3 x 928 x 1600 N(0,1) frames, a nuScenes-like rig, LiDAR-like future point clouds (SURVEY.md 8d cfg4).
+    `raw_images=True` (for `SyntheticViDAR(image_pipeline=True)`): seeded uniform uint8 BGR frames
+    [1, frames, cams, 900, 1600, 3] (img_hw defaults to the camera size) and the rig's host `cam2img` / `lidar2cam`
+    [1, cams, 4, 4] float64 as well."""
     g = torch.Generator(device=device).manual_seed(seed)
-    img = torch.randn(1, frames, cams, 3, img_hw[0], img_hw[1], device=device, generator=g)
+    extra = {}
+    if raw_images:
+        img_hw = img_hw or (900, 1600)
+        img = torch.randint(0, 256, (1, frames, cams, img_hw[0], img_hw[1], 3), device=device, generator=g,
+                            dtype=torch.uint8)
+        cam2img, lidar2cam = synthetic.camera_rig_split(cams)
+        extra = dict(cam2img=cam2img[None], lidar2cam=lidar2cam[None])
+    else:
+        img_hw = img_hw or synthetic.IMG_HW
+        img = torch.randn(1, frames, cams, 3, img_hw[0], img_hw[1], device=device, generator=g)
     lidar2img = synthetic.camera_rig(cams).numpy()[None]                     # host side, like img_metas
     pts = []
     _, origin, points, tindex = synthetic.dvr_inputs_lidar(M=rays_per_frame * (1 + future_frames), T=1 + future_frames, seed=seed,
@@ -560,7 +627,7 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=synthetic.IMG_HW, rays_per
                     p[:, 1] / bev_hw[0] * (PC_RANGE[4] - PC_RANGE[1]) + PC_RANGE[1],
                     p[:, 2] / HEIGHTS * (PC_RANGE[5] - PC_RANGE[2]) + PC_RANGE[2]], -1)
     pts.append(torch.from_numpy(np.concatenate([xyz, tindex[0][:, None]], -1).astype(np.float32)).to(device))
-    return dict(img=img, lidar2img=lidar2img, gt_points=pts)
+    return dict(img=img, lidar2img=lidar2img, gt_points=pts, **extra)
 
 
 def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
@@ -572,7 +639,8 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
     if record:
         model._mark("start")
     optimizer.zero_grad(set_to_none=True)
-    losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"])
+    losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"], cam2img=sample.get("cam2img"),
+                                 lidar2cam=sample.get("lidar2cam"))
     loss = sum(losses.values())
     (loss if scaler is None else scaler.scale(loss)).backward()
     model._mark("backward")

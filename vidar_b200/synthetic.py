@@ -105,3 +105,23 @@ def camera_rig(cams=6, img_hw=(900, 1600), f=1266.0, pp=(816.0, 491.0), cam_heig
         E[:3, 3] = -R @ pos
         mats.append(K @ E)
     return torch.from_numpy(np.stack(mats, 0).astype(np.float32))
+
+
+def camera_rig_split(cams=6, f=1266.0, pp=(816.0, 491.0), cam_height=1.5, seed=0):
+    """(cam2img, lidar2cam), each [cams, 4, 4] float64, of camera_rig's rig: the intrinsics and the extrinsics that
+    the reference's image pipeline keeps apart (CropResizeFlipImage rescales cam2img, then forms
+    lidar2img = cam2img @ lidar2cam).  Their product is camera_rig(cams) before its float32 cast."""
+    yaws = np.deg2rad([0.0, 55.0, -55.0, 110.0, -110.0, 180.0])[:cams]
+    rng = np.random.default_rng(seed)
+    K = np.array([[f, 0, pp[0], 0], [0, f, pp[1], 0], [0, 0, 1, 0], [0, 0, 0, 1]], np.float64)
+    exts = []
+    for yaw in yaws:
+        yaw = yaw + rng.normal(0, 0.01)
+        fwd = np.array([np.cos(yaw), np.sin(yaw), 0.0])
+        right = np.array([np.sin(yaw), -np.cos(yaw), 0.0])
+        R = np.stack([right, np.array([0.0, 0.0, -1.0]), fwd], 0)
+        E = np.eye(4)
+        E[:3, :3] = R
+        E[:3, 3] = -R @ (fwd * 1.0 + np.array([0, 0, cam_height]))
+        exts.append(E)
+    return np.stack([K] * len(exts), 0), np.stack(exts, 0)
