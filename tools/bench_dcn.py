@@ -23,43 +23,18 @@ import argparse
 import contextlib
 import json
 import os
-import subprocess
 import sys
 
-import numpy as np
 import torch
 import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tools.gpu_timing import card, event_ms  # noqa: E402
 from vidar_b200 import _lib, dcn  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
 SHAPES = {"stage3": (6, 256, 58, 100), "stage4": (6, 512, 29, 50)}
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-
-
-def timed(fns, steps, warmup):
-    """{name: median ms} of each zero-argument callable, the callables alternating."""
-    for fn in fns.values():
-        for _ in range(warmup):
-            fn()
-    torch.cuda.synchronize()
-    ms = {k: [] for k in fns}
-    for _ in range(steps):
-        for k, fn in fns.items():
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            fn()
-            b.record()
-            b.synchronize()
-            ms[k].append(a.elapsed_time(b))
-    return {k: round(float(np.median(v)), 4) for k, v in ms.items()}
 
 
 def layer(shape, steps, warmup):
@@ -122,9 +97,9 @@ def layer(shape, steps, warmup):
 
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-    fwd = timed(dict(ours=ours_f, torchvision=tv_f, cudnn_conv=conv_f), steps, warmup)
-    fwdbwd = timed(dict(ours=ours_fb, torchvision=tv_fb, cudnn_conv=conv_fb), steps, warmup)
-    kern = timed(dict(im2col=im2col, col2im=col2im, gemm=gemm), steps, warmup)
+    fwd = event_ms(dict(ours=ours_f, torchvision=tv_f, cudnn_conv=conv_f), steps, warmup)
+    fwdbwd = event_ms(dict(ours=ours_fb, torchvision=tv_fb, cudnn_conv=conv_fb), steps, warmup)
+    kern = event_ms(dict(im2col=im2col, col2im=col2im, gemm=gemm), steps, warmup)
     side = N * 27 * H * W * 4                                       # offsets + mask
     im2col_bytes = N * H * W * C * 4 + side + M * K * 4             # input once, columns written
     col2im_bytes = M * K * 4 + N * H * W * C * 4 * 2 + side * 2     # grad_cols + input read, grad_input, grad_off/mask
@@ -190,11 +165,11 @@ def layer_half(shape, dt, steps, warmup):
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     name = str(dt).replace("torch.", "")
-    fwd = timed({f"ours_{name}": op_f(half[:4]), "ours_float32": op_f((x, off, mask, w)), f"cudnn_conv_{name}": conv_f},
-                steps, warmup)
-    fwdbwd = timed({f"ours_{name}": op_fb(leaves16, half[4]), "ours_float32": op_fb(leaves32, gy),
-                    f"cudnn_conv_{name}": conv_fb}, steps, warmup)
-    kern = timed(dict(im2col=im2col, col2im=col2im), steps, warmup)
+    fwd = event_ms({f"ours_{name}": op_f(half[:4]), "ours_float32": op_f((x, off, mask, w)),
+                    f"cudnn_conv_{name}": conv_f}, steps, warmup)
+    fwdbwd = event_ms({f"ours_{name}": op_fb(leaves16, half[4]), "ours_float32": op_fb(leaves32, gy),
+                       f"cudnn_conv_{name}": conv_fb}, steps, warmup)
+    kern = event_ms(dict(im2col=im2col, col2im=col2im), steps, warmup)
     side = N * 27 * H * W
     im2col_bytes = N * H * W * C * s + side * s + M * K * s                          # input once, columns written
     col2im_bytes = M * K * s + N * H * W * C * (s + 4) + side * (s + 4)             # + fp32 grad_input / offset / mask
@@ -222,7 +197,7 @@ def backbone(steps, warmup, amp=None):
             sum(f.float().mean() for f in feats).backward()
         return fn
 
-    return timed({k: run(m) for k, m in models.items()}, steps, warmup)
+    return event_ms({k: run(m) for k, m in models.items()}, steps, warmup)
 
 
 def main():

@@ -16,7 +16,6 @@ grad_input, grad_offset and grad_mask, 3*C + 54*C/16 values.  `GB/s` is that min
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -25,37 +24,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import dcnv3_ref, msda_ref  # noqa: E402
+from tools.gpu_timing import card, event_ms  # noqa: E402
 from vidar_b200.dcnv3 import ext  # noqa: E402
 
 STAGES = [(232, 400), (116, 200), (58, 100), (29, 50)]
 MODELS = {"T": [64, 128, 256, 512], "B": [112, 224, 448, 896]}
 CG, BATCH, K = 16, 6, 9
 DTYPES = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = "power limit unknown"
-    return f"{name}, {q}"
-
-
-def timed(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(iters):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        times.append(a.elapsed_time(b))
-    return sorted(times)[len(times) // 2]
 
 
 def min_bytes(C, H, W, esize):
@@ -87,7 +62,7 @@ def main():
         ref = build_ref_dcnv3.load()
     except (FileNotFoundError, ImportError, OSError):
         ref = None
-    print(f"# {card()}; batch {BATCH}, group_channels {CG}, kernel 3; median of {a.iters} (ms)")
+    print(f"# {json.dumps(card())}; batch {BATCH}, group_channels {CG}, kernel 3; median of {a.iters} (ms)")
     print("| model | stage | dtype | op fwd | op fwd+bwd | fwd GB/s | fwd+bwd GB/s | ref fwd | ref fwd+bwd | "
           "eager fwd | eager fwd+bwd |")
     print("|---|---|---|---|---|---|---|---|---|---|---|")
@@ -102,20 +77,21 @@ def main():
                 mask = torch.softmax(torch.randn(BATCH, H, W, G, K, device=dev, generator=g), -1).reshape(
                     BATCH, H, W, -1).to(dt)
                 gy = torch.randn(BATCH, H, W, C, device=dev, generator=g).to(dt)
-                f = timed(lambda: ext.dcnv3_forward(x, off, mask, *args, 256), a.iters, a.warmup)
-                fb = timed(lambda: (ext.dcnv3_forward(x, off, mask, *args, 256),
-                                    ext.dcnv3_backward(x, off, mask, *args, gy, 256)), a.iters, a.warmup)
+                f = event_ms(lambda: ext.dcnv3_forward(x, off, mask, *args, 256), a.iters, a.warmup)
+                fb = event_ms(lambda: (ext.dcnv3_forward(x, off, mask, *args, 256),
+                                       ext.dcnv3_backward(x, off, mask, *args, gy, 256)), a.iters, a.warmup)
                 bf, bb = min_bytes(C, H, W, x.element_size())
                 row = dict(model=model, stage=si + 1, dtype=dname, fwd_ms=f, fwd_bwd_ms=fb,
                            fwd_gbs=bf / f / 1e6, fwd_bwd_gbs=(bf + bb) / fb / 1e6, min_fwd_mb=bf / 1e6,
                            min_bwd_mb=bb / 1e6)
                 if ref is not None and dt != torch.bfloat16:
-                    row["ref_fwd_ms"] = timed(lambda: ref.dcnv3_forward(x, off, mask, *args, 256), a.iters, a.warmup)
-                    row["ref_fwd_bwd_ms"] = timed(lambda: (ref.dcnv3_forward(x, off, mask, *args, 256),
-                                                           ref.dcnv3_backward(x, off, mask, *args, gy, 256)),
-                                                  a.iters, a.warmup)
-                row["eager_fwd_ms"] = timed(lambda: eager(x, off, mask, args), a.iters, a.warmup)
-                row["eager_fwd_bwd_ms"] = timed(lambda: eager(x, off, mask, args, gy), a.iters, a.warmup)
+                    row["ref_fwd_ms"] = event_ms(lambda: ref.dcnv3_forward(x, off, mask, *args, 256), a.iters,
+                                                 a.warmup)
+                    row["ref_fwd_bwd_ms"] = event_ms(lambda: (ref.dcnv3_forward(x, off, mask, *args, 256),
+                                                              ref.dcnv3_backward(x, off, mask, *args, gy, 256)),
+                                                     a.iters, a.warmup)
+                row["eager_fwd_ms"] = event_ms(lambda: eager(x, off, mask, args), a.iters, a.warmup)
+                row["eager_fwd_bwd_ms"] = event_ms(lambda: eager(x, off, mask, args, gy), a.iters, a.warmup)
                 fmt = lambda k: f"{row[k]:.3f}" if k in row else "-"  # noqa: E731
                 print(f"| {model} | {si + 1} ({H}x{W}, C {C}) | {dname} | {fmt('fwd_ms')} | {fmt('fwd_bwd_ms')} | "
                       f"{row['fwd_gbs']:.0f} | {row['fwd_bwd_gbs']:.0f} | {fmt('ref_fwd_ms')} | "

@@ -6,19 +6,16 @@ tests/eval_cases.py.
             boolean-masked clouds (this package's CUDA Chamfer), then compute_ray_errors with numpy on the host
             around a device NN search (eval_utils.py:185-225, restated by oracle/eval_ref.py), with its syncs
 
-Wall-clock time of each call ending in a device synchronise (both paths end on the host), CUDA events around
-the batched call as a cross-check; median of --reps after --warmup.  Prints one JSON line with the card, its
-power limit and SM clock read in the same run.
+Wall-clock time of each call ending in a device synchronise (both paths end on the host), and CUDA events around
+the batched call in a run of their own as a cross-check; median of --reps after --warmup.  Prints one JSON line with
+the card, its power limit and SM clock read in the same run.
 
     python tools/bench_eval.py [--points 30000] [--frames 7] [--reps 20] [--ref-reps 5]
 """
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -27,15 +24,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import eval_ref  # noqa: E402
 from tests.eval_cases import PC_RANGE, frame  # noqa: E402
+from tools.gpu_timing import card, event_ms, host_ms  # noqa: E402
 from vidar_b200 import chamfer, evaluate  # noqa: E402
-
-
-def gpu_info():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip().splitlines()
-    name, power, sm, sm_max = [x.strip() for x in out[0].split(",")]
-    return dict(gpu=name, power_limit=power, sm_clock=sm, sm_clock_max=sm_max)
 
 
 def per_pair(pred_pcds, gt_pcds, origin, dev):
@@ -91,28 +81,17 @@ def main():
     gt_pcds = [[torch.from_numpy(g).to(dev) for _, g, _ in frs]]
     origin = torch.from_numpy(np.stack([o for _, _, o in frs]))[None].to(dev)
 
-    for _ in range(a.warmup):
-        evaluate.frame_metrics(pred_pcds, gt_pcds, origin, PC_RANGE)
-    torch.cuda.synchronize()
-    wall, ev = [], []
-    for _ in range(a.reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0 = time.perf_counter()
-        e0.record()
-        got = evaluate.frame_metrics(pred_pcds, gt_pcds, origin, PC_RANGE)
-        e1.record()
-        torch.cuda.synchronize()
-        wall.append(time.perf_counter() - t0)
-        ev.append(e0.elapsed_time(e1) / 1e3)
+    def batched():
+        return evaluate.frame_metrics(pred_pcds, gt_pcds, origin, PC_RANGE)
 
-    per_pair(pred_pcds[0], gt_pcds[0], origin[0], dev)
-    torch.cuda.synchronize()
-    ref = []
-    for _ in range(a.ref_reps):
-        t0 = time.perf_counter()
-        want = per_pair(pred_pcds[0], gt_pcds[0], origin[0], dev)
-        torch.cuda.synchronize()
-        ref.append(time.perf_counter() - t0)
+    def reference():
+        return per_pair(pred_pcds[0], gt_pcds[0], origin[0], dev)
+
+    t = host_ms(batched, a.reps, a.warmup)
+    t_events = event_ms(batched, a.reps, a.warmup)
+    got = batched()
+    want = reference()                                         # also the reference's warm-up
+    t_ref = host_ms(reference, a.ref_reps, 0)
 
     worst = 0.0
     for f in range(a.frames):
@@ -120,13 +99,11 @@ def main():
         for m, w in zip(("chamfer_distance", "l1_error", "absrel_error"), want[f]):
             worst = max(worst, abs(g[m] - float(w)) / max(abs(float(w)), 1e-30))
     pairs = sum(3 * len(p) * len(g) for p, g, _ in frs)       # candidates scanned by the three searches
-    t = statistics.median(wall)
     print(json.dumps(dict(
         metric="eval_frame_metrics", frames=a.frames, points=[len(g) for _, g, _ in frs],
-        batched_ms=round(t * 1e3, 3), batched_events_ms=round(statistics.median(ev) * 1e3, 3),
-        per_pair_ms=round(statistics.median(ref) * 1e3, 1), speedup=round(statistics.median(ref) / t, 1),
-        nn_pairs_per_s=float(f"{pairs / t:.4g}"), reps=a.reps, ref_reps=a.ref_reps, max_rel_diff=worst,
-        **gpu_info())))
+        batched_ms=round(t, 3), batched_events_ms=round(t_events, 3), per_pair_ms=round(t_ref, 1),
+        speedup=round(t_ref / t, 1), nn_pairs_per_s=float(f"{pairs / (t * 1e-3):.4g}"), reps=a.reps,
+        ref_reps=a.ref_reps, max_rel_diff=worst, **card())))
 
 
 if __name__ == "__main__":

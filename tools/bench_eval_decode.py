@@ -7,22 +7,20 @@ process.
 Shape: bs 1, 7 frames (current + 6 future), 200 x 200 x 16 sigma of the current head frame, ray_grid_num 512,
 `--gt` GT points per frame, seeded rigid frame transforms in img_metas.  Both paths end in host numbers, so each call
 is timed with a host clock around the synchronised call (median of --steps, the paths alternating, both warmed up).
-Per path: vidar_b200 kernel launches and host syncs per call (counted under torch.cuda.set_sync_debug_mode("warn")),
-and the largest relative difference of the four metrics between the paths.  The card's name, power limit and SM
+Per path: vidar_b200 kernel launches and host syncs per call (counted by tools/gpu_timing.py's count_syncs), and
+the largest relative difference of the four metrics between the paths.  The card's name, power limit and SM
 clock are read in the same run.  Prints one JSON line."""
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
-import warnings
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tools.gpu_timing import card, count_syncs, host_ms  # noqa: E402
 from vidar_b200 import _lib, evaluate  # noqa: E402
 from vidar_b200.head import ViDARRayHeadV1  # noqa: E402
 
@@ -31,12 +29,6 @@ HISTORY_QUEUE_LENGTH, PRED_HISTORY = 4, 3
 HEAD_FRAMES = PRED_HISTORY + 2
 PC_RANGE = [-51.2, -51.2, -5.0, 51.2, 51.2, 3.0]
 METRICS = ("chamfer_distance", "l1_error", "absrel_error", "count")
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def _rigid(rng):
@@ -77,20 +69,6 @@ def unfused(head, pd, gt, kw):
     return evaluate.frame_metrics(dec["pred_pcds"], dec["gt_pcds"], dec["origin"], kw["tgt_pc_range"])
 
 
-def count_syncs(fn, *args):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as rec:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            fn(*args)
-        finally:
-            torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
-    syncs = [w for w in rec if "called a synchronizing CUDA operation" in str(w.message)]
-    return len(syncs), sorted({f"{os.path.relpath(w.filename, ROOT)}:{w.lineno}" for w in syncs})
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -102,30 +80,20 @@ def main():
     head = ViDARRayHeadV1(HISTORY_QUEUE_LENGTH, pred_history_frame_num=PRED_HISTORY, pred_future_frame_num=1,
                           per_frame_loss_weight=(0.1,) * HEAD_FRAMES, ray_grid_num=NUM_WAY,
                           loss_weight=np.ones((F, 1)))
-    paths = {"evaluate": fused, "frame_metrics(get_point_cloud_prediction)": unfused}
     pd, gt, kw = inputs(a.gt)
+    paths = {"evaluate": lambda: fused(head, pd, gt, kw),
+             "frame_metrics(get_point_cloud_prediction)": lambda: unfused(head, pd, gt, kw)}
     name = card()
-    res = {k: dict(s=[]) for k in paths}
-    outs = {}
+    res, outs = {}, {}
     with torch.no_grad():
+        ms = host_ms(paths, a.steps, a.warmup)                  # the two paths alternating
         for k, fn in paths.items():
-            for _ in range(a.warmup):
-                fn(head, pd, gt, kw)
-            torch.cuda.synchronize()
             n0 = _lib.launch_count()
-            outs[k] = fn(head, pd, gt, kw)
+            outs[k] = fn()
             torch.cuda.synchronize()
-            res[k]["launches"] = _lib.launch_count() - n0
-        for _ in range(a.steps):
-            for k, fn in paths.items():                  # alternate the two paths
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                fn(head, pd, gt, kw)
-                torch.cuda.synchronize()
-                res[k]["s"].append(time.perf_counter() - t0)
-        for k, fn in paths.items():
-            res[k]["host_syncs"], res[k]["sync_sites"] = count_syncs(fn, head, pd, gt, kw)
-            res[k]["median_ms"] = round(1e3 * float(np.median(res[k].pop("s"))), 3)
+            res[k] = dict(launches=_lib.launch_count() - n0)
+            res[k]["host_syncs"], res[k]["sync_sites"] = count_syncs(fn)
+            res[k]["median_ms"] = round(ms[k], 3)
     fo, uo = (outs[k] for k in paths)
     rel = 0.0
     for f in uo:

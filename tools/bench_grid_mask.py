@@ -7,7 +7,7 @@ crop on the host, a pageable `.cuda()` upload, `1 - mask`, `x * mask`) against `
     `1 - mask` and multiply on an uploaded mask; its algorithmic bytes (read x, write out) over 3.35 TB/s, the H100
     SXM data-sheet HBM3 bandwidth;
   * blocking: behind a ~50 ms device sleep, how long the host takes to return from the call, and whether the call
-    raises under torch.cuda.set_sync_debug_mode("error") -- observed, not assumed;
+    makes a synchronising CUDA call (tools/gpu_timing.py's count_syncs) -- observed, not assumed;
   * step: `pretrain.train_step` with the cfg's GridMask (prob forced to 1 so every step masks), device op vs
     reference statements, alternated.
 The card's name, power limit and SM clock are read in the same run.
@@ -17,8 +17,6 @@ The card's name, power limit and SM clock are read in the same run.
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 import time
 
@@ -29,6 +27,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import grid_mask_ref  # noqa: E402
+from tools.gpu_timing import card, count_syncs, event_ms, host_ms  # noqa: E402
 from vidar_b200 import grid_mask, pretrain  # noqa: E402
 
 SHAPE = (6, 3, 928, 1600)
@@ -46,57 +45,15 @@ def reference_statements(module, x, draw):
     return (x.view(-1, h, w) * mask.expand_as(x.view(-1, h, w))).view(n, c, h, w)
 
 
-def host_ms(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    t = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        t.append((time.perf_counter() - t0) * 1e3)
-    return statistics.median(t)
-
-
-def event_ms(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    t = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        t.append(a.elapsed_time(b))
-    return statistics.median(t)
-
-
 def blocking(fn):
-    """(host ms to return from fn behind a ~50 ms device sleep, whether fn raises under sync debug mode "error")."""
+    """(host ms to return from fn behind a ~50 ms device sleep, whether fn makes a synchronising CUDA call)."""
     torch.cuda.synchronize()
     torch.cuda._sleep(50_000_000)
     t0 = time.perf_counter()
     fn()
     ret = (time.perf_counter() - t0) * 1e3
     torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode("error")
-    try:
-        fn()
-        synced = False
-    except RuntimeError:
-        synced = True
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
-    torch.cuda.synchronize()
-    return ret, synced
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else torch.cuda.get_device_name()
+    return ret, count_syncs(fn)[0] > 0
 
 
 def op_bench(dev):
@@ -113,11 +70,11 @@ def op_bench(dev):
         nbytes = 2 * x.numel() * x.element_size()
         r = {}
         for name, fn in (("reference", lambda: reference_statements(m, x, draw)), ("device", lambda: m.masked(x, draw))):
-            r[name] = dict(host_ms=host_ms(fn))
+            r[name] = dict(host_ms=host_ms(fn, 20, 3))
         # with the draws included, as a forward call makes them (the reference's numpy draws are the same)
-        r["device"]["host_ms_with_draws"] = host_ms(lambda: m(x))
-        r["reference"]["kernel_ms"] = event_ms(lambda: x * (1 - dev_mask).expand_as(x))
-        r["device"]["kernel_ms"] = event_ms(lambda: grid_mask.grid_mask_apply(x, draw, True, True, 1))
+        r["device"]["host_ms_with_draws"] = host_ms(lambda: m(x), 20, 3)
+        r["reference"]["kernel_ms"] = event_ms(lambda: x * (1 - dev_mask).expand_as(x), 20, 3)
+        r["device"]["kernel_ms"] = event_ms(lambda: grid_mask.grid_mask_apply(x, draw, True, True, 1), 20, 3)
         for name in r:
             r[name]["kernel_bytes_share_of_peak"] = nbytes / (r[name]["kernel_ms"] * 1e-3) / PEAK_BW
             ret, synced = blocking(lambda: (reference_statements(m, x, draw) if name == "reference"
@@ -136,21 +93,15 @@ def step_bench(dev, steps):
     sample = pretrain.synthetic_sample(dev)
     device_masked = model.grid_mask.masked
     paths = {"device": device_masked, "reference": lambda x, draw: reference_statements(model.grid_mask, x, draw)}
-    times = {k: [] for k in paths}
-    np.random.seed(0)
-    for k in paths:                                            # warm up both
+
+    def run(k):
         model.grid_mask.masked = paths[k]
         pretrain.train_step(model, opt, sample)
-    for i in range(steps):
-        for k in (("device", "reference") if i % 2 == 0 else ("reference", "device")):
-            model.grid_mask.masked = paths[k]
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            pretrain.train_step(model, opt, sample)
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t0) * 1e3)
+
+    np.random.seed(0)
+    med, ms = host_ms({k: lambda k=k: run(k) for k in paths}, steps, 1, raw=True)     # alternating
     model.grid_mask.masked = device_masked
-    return {k: dict(median_ms=statistics.median(v), all_ms=v) for k, v in times.items()}
+    return {k: dict(median_ms=med[k], all_ms=ms[k]) for k in paths}
 
 
 def main():

@@ -7,31 +7,24 @@ Shape: bs 1, 4 valid frames, 200 x 200 x 16 sigma, ray_grid_num 512, 10 000 dens
 dense grid), CE + dense (use_dist_loss=False, the vidar_pretrain configuration).  Both paths get the same inputs
 and the same pre-drawn Gumbel noise, so their outputs are compared at the timed size.  Per path: median time of
 loss + backward by CUDA events, vidar_b200 kernel launches per call, and host syncs per call counted in a separate
-pass under torch.cuda.set_sync_debug_mode("warn").  The card's name and power limit are read in the same run.
+pass (tools/gpu_timing.py's count_syncs).  The card's name, power limit and SM clocks are read in the same run.
 Prints one JSON line per GT size."""
 import argparse
 import json
 import os
-import subprocess
 import sys
-import warnings
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tools.gpu_timing import card, count_syncs, event_ms  # noqa: E402
 from vidar_b200 import _lib  # noqa: E402
 from vidar_b200.head import ViDARRayHead  # noqa: E402
 
 F, H, W, Z, NUM_WAY = 4, 200, 200, 16, 512
 PC_RANGE = [-51.2, -51.2, -5.0, 51.2, 51.2, 3.0]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def inputs(gt_per_frame, seed=0):
@@ -58,20 +51,6 @@ def call(head, preds, gt, kw):
     return out, p.grad
 
 
-def count_syncs(head, preds, gt, kw):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as rec:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            call(head, preds, gt, kw)
-        finally:
-            torch.cuda.set_sync_debug_mode("default")
-    torch.cuda.synchronize()
-    syncs = [w for w in rec if "called a synchronizing CUDA operation" in str(w.message)]
-    return len(syncs), sorted({f"{os.path.relpath(w.filename, ROOT)}:{w.lineno}" for w in syncs})
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -88,26 +67,16 @@ def main():
     name = card()
     for n_gt in a.gt:
         preds, gt, kw = inputs(n_gt)
-        res = {k: dict(ms=[]) for k in heads}
-        outs = {}
-        for k, h in heads.items():
-            for _ in range(a.warmup):
-                call(h, preds, gt, kw)
+        calls = {k: (lambda h=h: call(h, preds, gt, kw)) for k, h in heads.items()}
+        ms = event_ms(calls, a.steps, a.warmup)                 # the two paths alternating
+        res, outs = {}, {}
+        for k, fn in calls.items():
             n0 = _lib.launch_count()
-            outs[k] = call(h, preds, gt, kw)
+            outs[k] = fn()
             torch.cuda.synchronize()
-            res[k]["launches"] = _lib.launch_count() - n0
-        for _ in range(a.steps):
-            for k, h in heads.items():                 # alternate the two paths
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                call(h, preds, gt, kw)
-                e1.record()
-                e1.synchronize()
-                res[k]["ms"].append(e0.elapsed_time(e1))
-        for k, h in heads.items():
-            res[k]["syncs"], res[k]["sync_sites"] = count_syncs(h, preds, gt, kw)
-            res[k]["median_ms"] = round(float(np.median(res[k].pop("ms"))), 3)
+            res[k] = dict(launches=_lib.launch_count() - n0)
+            res[k]["syncs"], res[k]["sync_sites"] = count_syncs(fn)
+            res[k]["median_ms"] = round(ms[k], 3)
         (ob, gb), (op, gp) = outs["batched"], outs["per_pair"]
         ob, op = ({k: float(v.detach()) for k, v in o.items()} for o in (ob, op))
         cmp = {k: dict(batched=ob[k], per_pair=op[k], rel_diff=abs(ob[k] - op[k]) / max(abs(op[k]), 1e-30)) for k in ob}

@@ -9,8 +9,8 @@ sigma, ray_grid_num 512, 10 000 dense rays per frame (the 50 x 50 x 4 dense grid
 the shipped per-frame and frame loss weights; `--gt` GT points per source frame (9 source frames), random rigid
 frame transforms.  Both paths get the same inputs and the same pre-drawn Gumbel noise, so their outputs are
 compared at the timed size.  Per path: median time of loss + backward by CUDA events, vidar_b200 kernel launches per
-call, and host syncs per call counted in a separate pass under torch.cuda.set_sync_debug_mode("warn").  The card's
-name and power limit are read in the same run.  Prints one JSON line per GT size."""
+call, and host syncs per call counted in a separate pass (tools/gpu_timing.py's count_syncs).  The card's name,
+power limit and SM clocks are read in the same run.  Prints one JSON line per GT size."""
 import argparse
 import json
 import os
@@ -21,7 +21,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from tools.bench_head_loss import card, count_syncs  # noqa: E402
+from tools.gpu_timing import card, count_syncs, event_ms  # noqa: E402
 from vidar_b200 import _lib  # noqa: E402
 from vidar_b200.head import ViDARRayHeadV1  # noqa: E402
 
@@ -82,27 +82,16 @@ def main():
     name = card()
     for n_gt in a.gt:
         preds, gt, kw = inputs(n_gt)
-        res = {k: dict(ms=[]) for k in heads}
-        outs = {}
-        for k, h in heads.items():
-            for _ in range(a.warmup):
-                call(h, preds, gt, kw)
-            torch.cuda.synchronize()
+        calls = {k: (lambda h=h: call(h, preds, gt, kw)) for k, h in heads.items()}
+        ms = event_ms(calls, a.steps, a.warmup)                 # the two paths alternating
+        res, outs = {}, {}
+        for k, fn in calls.items():
             n0 = _lib.launch_count()
-            outs[k] = call(h, preds, gt, kw)
+            outs[k] = fn()
             torch.cuda.synchronize()
-            res[k]["launches"] = _lib.launch_count() - n0
-        for _ in range(a.steps):
-            for k, h in heads.items():                 # alternate the two paths
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                call(h, preds, gt, kw)
-                e1.record()
-                e1.synchronize()
-                res[k]["ms"].append(e0.elapsed_time(e1))
-        for k, h in heads.items():
-            res[k]["syncs"], res[k]["sync_sites"] = count_syncs(h, preds, gt, kw)   # the same call: 4 valid frames
-            res[k]["median_ms"] = round(float(np.median(res[k].pop("ms"))), 3)
+            res[k] = dict(launches=_lib.launch_count() - n0)
+            res[k]["syncs"], res[k]["sync_sites"] = count_syncs(fn)
+            res[k]["median_ms"] = round(ms[k], 3)
         (ob, gb), (op, gp) = outs["batched"], outs["per_head_frame"]
         ob, op = ({k: float(v.detach()) for k, v in o.items()} for o in (ob, op))
         cmp = {k: dict(batched=ob[k], per_head_frame=op[k], rel_diff=abs(ob[k] - op[k]) / max(abs(op[k]), 1e-30))

@@ -19,10 +19,7 @@ import argparse
 import json
 import os
 import random
-import statistics
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -31,43 +28,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import image_aug_ref  # noqa: E402
+from tools.gpu_timing import card, event_ms, host_ms  # noqa: E402
 from vidar_b200 import image_aug, pretrain  # noqa: E402
 
 N, H, W = 6, 900, 1600
 PEAK_BW = 3.35e12
-
-
-def host_ms(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    t = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        t.append((time.perf_counter() - t0) * 1e3)
-    return statistics.median(t)
-
-
-def event_ms(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    t = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        t.append(a.elapsed_time(b))
-    return statistics.median(t)
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else torch.cuda.get_device_name()
 
 
 def transforms(h, photo):
@@ -110,24 +75,19 @@ def op_bench(dev):
                                           plan.flip, plan.mean, plan.std, plan.to_rgb, plan.pad_hw, plan.pad_val)
             assert np.array_equal(out[0].permute(1, 2, 0).cpu().numpy().view(np.uint32), want.view(np.uint32))
             nbytes = src.numel() + out.numel() * 4
-            r = dict(out_shape=list(out.shape), kernel_ms=event_ms(lambda: image_aug.apply_multiview(src, results)))
+            r = dict(out_shape=list(out.shape),
+                     kernel_ms=event_ms(lambda: image_aug.apply_multiview(src, results), 20, 3))
             r["algorithmic_bytes"] = nbytes
             r["kernel_GBps"] = nbytes / (r["kernel_ms"] * 1e-3) / 1e9
             r["kernel_bytes_share_of_peak"] = nbytes / (r["kernel_ms"] * 1e-3) / PEAK_BW
             r["host_ms_with_draws"] = host_ms(lambda: image_aug.apply_multiview(
-                src, frame_results(list(src), steps)))
+                src, frame_results(list(src), steps)), 20, 3)
             r["h2d_bytes_uint8_frame"] = src.numel()
             r["h2d_bytes_reference_float32"] = N * 3 * hp * wp * 4
             if has_cv2_pil():
-                t = []
-                for _ in range(3):
-                    t0 = time.perf_counter()
-                    for n in range(N):
-                        image_aug_ref.pipeline_statements(src_host[n], plan.photo[n] if photo else None, plan.crop,
-                                                          plan.dims, plan.flip, plan.mean, plan.std, plan.to_rgb,
-                                                          plan.pad_hw, plan.pad_val[0])
-                    t.append((time.perf_counter() - t0) * 1e3)
-                r["reference_cpu_ms_per_frame"] = statistics.median(t)
+                r["reference_cpu_ms_per_frame"] = host_ms(lambda: [image_aug_ref.pipeline_statements(
+                    src_host[n], plan.photo[n] if photo else None, plan.crop, plan.dims, plan.flip, plan.mean,
+                    plan.std, plan.to_rgb, plan.pad_hw, plan.pad_val[0]) for n in range(N)], 3, 0)
                 r["host_cpus"] = os.cpu_count()
             else:
                 r["reference_cpu_ms_per_frame"] = "not measured (cv2 or PIL missing)"
@@ -141,7 +101,6 @@ def step_bench(dev, steps):
     model, opt = pretrain.build(dev, None, seed=0, image_pipeline=True)
     raw = pretrain.synthetic_sample(dev, raw_images=True)
     plain = pretrain.synthetic_sample(dev)
-    times = {"pipeline": [], "default": []}
 
     def run(k):
         model.image_transforms = transforms_on if k == "pipeline" else None
@@ -150,17 +109,9 @@ def step_bench(dev, steps):
     transforms_on = model.image_transforms
     np.random.seed(0)
     random.seed(0)
-    for k in times:                                            # warm up both
-        run(k)
-    for i in range(steps):
-        for k in (("pipeline", "default") if i % 2 == 0 else ("default", "pipeline")):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            run(k)
-            torch.cuda.synchronize()
-            times[k].append((time.perf_counter() - t0) * 1e3)
+    med, ms = host_ms({k: lambda k=k: run(k) for k in ("pipeline", "default")}, steps, 1, raw=True)   # alternating
     model.image_transforms = transforms_on
-    return {k: dict(median_ms=statistics.median(v), all_ms=v) for k, v in times.items()}
+    return {k: dict(median_ms=med[k], all_ms=ms[k]) for k in med}
 
 
 def main():

@@ -15,7 +15,7 @@ import argparse
 import json
 import math
 import os
-import subprocess
+import statistics
 import sys
 
 import numpy as np
@@ -23,19 +23,11 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tools.gpu_timing import card, event_ms  # noqa: E402
 
 HB, WB, D, G, GRID_NUM, STEP, EPS, ACT = 200, 200, 16, 1, 256, 0.5, 1e-3, 1
 BOX = 4                      # box side of a bundle's footprint at one waypoint
 ANGLE_BITS = 20              # angle bins of the cell order (2^20, csrc/latent_render.cu kAngleBits)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def reduction_counts(Hb=HB, Wb=WB, grid_num=GRID_NUM, step=STEP, bundles=(32, 64)):
@@ -118,7 +110,6 @@ def main():
     prob, pooled = torch.empty(R, D, device=dev), torch.empty(R, D * G, device=dev)
     aux = torch.empty(3, R, D, device=dev)
     gpm, gfe, gocc = (torch.zeros(R, D, device=dev) for _ in range(3))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     st = _lib.stream_ptr(dev)
     calls = {
         "latent_prob_fwd": lambda: L.vidar_latent_prob_forward(P(occ), P(prob), P(aux), 1, D, HB, WB, GRID_NUM, STEP, ACT,
@@ -131,18 +122,13 @@ def main():
                                                                 STEP, ACT, 0, R, st),
     }
     times = {}
+
+    def record(k, fn, iters):
+        med, ms = event_ms(fn, iters, a.warmup, flush=True, sync=False, raw=True)
+        times[k] = {"mean_ms": statistics.fmean(ms), "median_ms": med}
+
     for k, fn in calls.items():
-        for _ in range(a.warmup):
-            _lib.check(fn())
-        ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.iters)]
-        for e0, e1 in ev:
-            flush.zero_()
-            e0.record()
-            _lib.check(fn())
-            e1.record()
-        torch.cuda.synchronize()
-        ms = sorted(e0.elapsed_time(e1) for e0, e1 in ev)
-        times[k] = {"mean_ms": sum(ms) / len(ms), "median_ms": ms[len(ms) // 2]}
+        record(k, lambda fn=fn: _lib.check(fn()), a.iters)
 
     if a.profile:
         # kernel split of the backward entry points (cell order + bundle kernel), in a run of its own
@@ -163,17 +149,7 @@ def main():
         e = emb.detach().requires_grad_(True)
         mod.zero_grad(set_to_none=True)
         mod(e).backward(gemb)
-    for _ in range(a.warmup):
-        step()
-    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.iters // 4)]
-    for e0, e1 in ev:
-        flush.zero_()
-        e0.record()
-        step()
-        e1.record()
-    torch.cuda.synchronize()
-    ms = sorted(e0.elapsed_time(e1) for e0, e1 in ev)
-    times["module_fwd_bwd"] = {"mean_ms": sum(ms) / len(ms), "median_ms": ms[len(ms) // 2]}
+    record("module_fwd_bwd", step, a.iters // 4)
     for k, v in times.items():
         print(f"[bench_latent] {k:16s} {v['median_ms']:.4f} ms median, {v['mean_ms']:.4f} ms mean")
     result.update(card=name, iters=a.iters, times=times)

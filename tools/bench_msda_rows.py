@@ -17,8 +17,6 @@ one record per horizontally adjacent corner pair (the distinct valid pixels of e
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 
 import numpy as np
@@ -27,21 +25,13 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tools.gpu_timing import card, event_ms  # noqa: E402
 from vidar_b200 import synthetic  # noqa: E402
 
 CAMS, Q, H, C, P = 6, 40000, 8, 32, 8
 LEVELS = synthetic.SCA_LEVELS
 TILE_ROWS = 256                      # csrc/msda.cu kTileRows
 GROUPS = 64                          # 8-lane groups of the sorted-run pass (512 threads)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name()
 
 
 # ---- counts (CPU) ------------------------------------------------------------------------------------------------
@@ -132,17 +122,6 @@ def counts():
 
 
 # ---- timings (GPU) -----------------------------------------------------------------------------------------------
-def _events_ms(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(iters):
-        ts.append(fn())
-    torch.cuda.synchronize()
-    return statistics.median(a.elapsed_time(b) for a, b in ts)
-
-
 def _kernel_ms(fn, names, calls):
     """profiler kernel time per call of the kernels whose names contain one of `names`"""
     from torch.profiler import ProfilerActivity, profile
@@ -170,30 +149,17 @@ def timings(iters, warmup):
     inv = torch.full((1, Q), 1.0 / CAMS, device=dev)
     g = torch.randn(1, Q, H * C, device=dev, generator=torch.Generator(device=dev).manual_seed(11))
     static = [d["value"], d["loc"], d["attn"]]
-    ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
+    # forward and backward alternate, so each backward is timed alone on the slots of the forward before it
+    graph = []
 
     def forward():
         leaves = [t.detach().requires_grad_(True) for t in static]
         return sca.MSDARowsFunction.apply(plan, 1, Q, d["shapes"], d["lsi"], None, None, inv, *leaves)
 
-    def fwd():
-        a, b = ev(), ev()
-        a.record()
-        forward()
-        b.record()
-        return a, b
-
-    def bwd():
-        slots = forward()
-        a, b = ev(), ev()
-        a.record()
-        slots.backward(g)
-        b.record()
-        return a, b
-
     out = {"card": card(), "shape": f"{CAMS} cameras x {Q} rows, H={H} C={C} L={len(LEVELS)} P={P}"}
-    out["rows_fwd_ms"] = _events_ms(fwd, iters, warmup)
-    out["rows_bwd_ms"] = _events_ms(bwd, iters, warmup)
+    ms = event_ms({"fwd": lambda: graph.append(forward()), "bwd": lambda: graph.pop().backward(g)}, iters, warmup,
+                  sync=False)
+    out["rows_fwd_ms"], out["rows_bwd_ms"] = ms["fwd"], ms["bwd"]
     k = _kernel_ms(lambda: forward().backward(g), ["msda_backward_tile_kernel", "rows_key_kernel", "rows_scan_kernel",
                                                    "rows_scatter_kernel"], 5)
     out["tile_kernel_ms"] = k.pop("msda_backward_tile_kernel")
@@ -205,16 +171,12 @@ def timings(iters, warmup):
     offsets = 4.0 * torch.randn(1, Q, H, len(LEVELS), P, 2, device=dev, generator=gen)
     logits = torch.randn(1, Q, H, len(LEVELS) * P, device=dev, generator=gen)
 
-    def sca_bwd():
+    def sca_fwd():
         o, lg, v = (t.detach().requires_grad_(True) for t in (offsets, logits, d["value"]))
-        slots = sca.SCARowsFunction.apply(plan, 1, d["shapes"], d["lsi"], ref_cam, o, lg, None, None, inv, v)
-        a, b = ev(), ev()
-        a.record()
-        slots.backward(g)
-        b.record()
-        return a, b
+        graph.append(sca.SCARowsFunction.apply(plan, 1, d["shapes"], d["lsi"], ref_cam, o, lg, None, None, inv, v))
 
-    out["sca_rows_bwd_ms"] = _events_ms(sca_bwd, iters, warmup)
+    out["sca_rows_bwd_ms"] = event_ms({"fwd": sca_fwd, "bwd": lambda: graph.pop().backward(g)}, iters, warmup,
+                                      sync=False)["bwd"]
     print(f"card: {out['card']}")
     for key in ("rows_fwd_ms", "rows_bwd_ms", "tile_kernel_ms", "row_order_kernels_ms", "sca_rows_bwd_ms"):
         print(f"{key:>22}: {out[key]:.3f}")

@@ -14,7 +14,6 @@ clock are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -23,20 +22,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import vidar_b200.modules  # noqa: E402,F401  (registers the classes)
+from tools.gpu_timing import card, event_ms  # noqa: E402
 from vidar_b200.registry import build_attention  # noqa: E402
 
 E, BEV = 256, (200, 200)
 Q = BEV[0] * BEV[1]
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", "0"], capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = "power limit / clocks unknown"
-    return f"{name}, {q}"
 
 
 def levels(n):
@@ -81,31 +71,23 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")      # 256 MB > the 50 MB L2
     res = {"card": card(), "iters": args.iters}
     print(res["card"], flush=True)
     for kind in ("tsa", "decoder_self", "decoder_cross"):
         m, fwd, fwd_bwd = setup(kind)
         row = {}
-        for what, fn in (("forward", lambda: fwd()), ("forward+backward", fwd_bwd)):
+        for what, fn in (("forward", fwd), ("forward+backward", fwd_bwd)):
             ctx = torch.no_grad if what == "forward" else torch.enable_grad
-            times = {True: [], False: []}
-            for it in range(args.warmup + args.iters):
-                for fused in (True, False):                     # alternate in one run
-                    m.fuse_epilogue = fused
-                    m.zero_grad(set_to_none=True)
-                    flush.zero_()
-                    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    with ctx():
-                        a.record()
-                        fn()
-                        b.record()
-                    b.synchronize()
-                    if it >= args.warmup:
-                        times[fused].append(a.elapsed_time(b))
+
+            def call(fused, fn=fn, ctx=ctx):
+                m.fuse_epilogue = fused
+                m.zero_grad(set_to_none=True)
+                with ctx():
+                    fn()
+
+            ms = event_ms({f: lambda f=f: call(f) for f in (True, False)}, args.iters, args.warmup, flush=True)
             for fused in (True, False):
-                t = sorted(times[fused])
-                row[f"{what} {'fused' if fused else 'unfused'} ms"] = round(t[len(t) // 2], 4)
+                row[f"{what} {'fused' if fused else 'unfused'} ms"] = round(ms[fused], 4)
         for fused in (True, False):
             m.fuse_epilogue = fused
             m.zero_grad(set_to_none=True)

@@ -13,25 +13,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 from oracle import msda_ref  # noqa: E402
+from tools.gpu_timing import card, window_ms  # noqa: E402
 from vidar_b200 import msda, ray_head  # noqa: E402
-
-
-def timed(fn, n=10, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(n):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / n
 
 
 def main():
     dev = torch.device("cuda:0")
-    out = {}
+    out = {"card": card()}
     # ---- MSDA, one camera of the SCA workload
     d = bench.sca_like_inputs(dev, cams=1)
 
@@ -47,7 +35,7 @@ def main():
                                       d["attn"].detach().requires_grad_(True))
         o.backward(d["grad_out"])
 
-    out["msda_1cam_40000q_fwd_bwd_ms"] = {"vidar_b200": timed(ours), "torch_eager_grid_sample": timed(eager, n=3, warm=1)}
+    out["msda_1cam_40000q_fwd_bwd_ms"] = {"vidar_b200": window_ms(ours, 10, 3), "torch_eager_grid_sample": window_ms(eager, 3, 1)}
     # ---- TSA shape: B=2, 1 level 200x200, P=4
     g = torch.Generator(device=dev).manual_seed(0)
     val = torch.randn(2, 40000, 8, 32, device=dev, generator=g)
@@ -67,7 +55,7 @@ def main():
         v = val.detach().requires_grad_(True)
         o = msda_ref.msda_grid_sample(v, shp.cpu(), loc.detach().requires_grad_(True), aw.detach().requires_grad_(True))
         o.backward(go)
-    out["msda_tsa_B2_Q40000_fwd_bwd_ms"] = {"vidar_b200": timed(tsa), "torch_eager_grid_sample": timed(tsa_eager, n=3, warm=1)}
+    out["msda_tsa_B2_Q40000_fwd_bwd_ms"] = {"vidar_b200": window_ms(tsa, 10, 3), "torch_eager_grid_sample": window_ms(tsa_eager, 3, 1)}
 
     # ---- head ray sampler + CE: 3 frames 16x200x200, 30k rays, 512 waypoints
     from tests.test_ray_head_gpu import _big_case
@@ -90,10 +78,10 @@ def main():
 
     import oracle.ray_head_ref as rr
     _orig = rr.torch.tensor
-    out["ray_ce_30k_rays_512wp_fwd_bwd_ms"] = {"vidar_b200": timed(ce_ours)}
+    out["ray_ce_30k_rays_512wp_fwd_bwd_ms"] = {"vidar_b200": window_ms(ce_ours, 10, 3)}
     try:
         torch.set_default_device(dev)
-        out["ray_ce_30k_rays_512wp_fwd_bwd_ms"]["torch_eager_reference_formula"] = timed(ce_eager, n=3, warm=1)
+        out["ray_ce_30k_rays_512wp_fwd_bwd_ms"]["torch_eager_reference_formula"] = window_ms(ce_eager, 3, 1)
     except Exception as e:
         out["ray_ce_30k_rays_512wp_fwd_bwd_ms"]["torch_eager_reference_formula"] = f"failed: {e}"
     finally:
@@ -115,10 +103,10 @@ def main():
         p, q = latent_render_ref.latent_core(o, f, 256, 0.5, 1e-3, "sigmoid")
         (p.sum() + q.sum()).backward()
 
-    out["latent_render_core_200x200x16_256wp_fwd_bwd_ms"] = {"vidar_b200": timed(lr_ours)}
+    out["latent_render_core_200x200x16_256wp_fwd_bwd_ms"] = {"vidar_b200": window_ms(lr_ours, 10, 3)}
     try:
         torch.set_default_device(dev)
-        out["latent_render_core_200x200x16_256wp_fwd_bwd_ms"]["torch_eager_reference_formula"] = timed(lr_eager, n=3, warm=1)
+        out["latent_render_core_200x200x16_256wp_fwd_bwd_ms"]["torch_eager_reference_formula"] = window_ms(lr_eager, 3, 1)
     except Exception as e:
         out["latent_render_core_200x200x16_256wp_fwd_bwd_ms"]["torch_eager_reference_formula"] = f"failed: {e}"
     finally:
@@ -139,7 +127,7 @@ def main():
     rec = {}
     for fused in (True, False):
         mod.fuse_projections = fused
-        rec["fused_projections" if fused else "cublas_linears_around_core"] = timed(module_step, n=20)
+        rec["fused_projections" if fused else "cublas_linears_around_core"] = window_ms(module_step, 20, 3)
     out["latent_rendering_module_200x200x256_fwd_bwd_ms"] = rec
     # ---- MSDeformableAttention3D module (the per-camera attention of SCA), 6 cameras x 10000 visible pillars:
     #      softmax / sampling-location arithmetic inside the kernel vs materialised like the reference
@@ -162,7 +150,7 @@ def main():
     rec = {}
     for fused in (True, False):
         att.fuse_epilogue = fused
-        rec["fused_epilogue" if fused else "materialised_loc_and_weights"] = timed(att_step, n=10)
+        rec["fused_epilogue" if fused else "materialised_loc_and_weights"] = window_ms(att_step, 10, 3)
     out["msdeformattn3d_module_6cams_10000q_fwd_bwd_ms"] = rec
     print(json.dumps(out, indent=1))
 

@@ -7,30 +7,15 @@ calls bracketed by torch.cuda.synchronize (median of 20 after 5 warm-ups)."""
 import json
 import os
 import sys
-import time
 
-import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import build_ref  # noqa: E402
 from tests.inputs import dvr_inputs_lidar  # noqa: E402
+from tools.gpu_timing import card, host_ms  # noqa: E402
 from vidar_b200 import render  # noqa: E402
-
-
-def timed(fn, n=20, warm=5):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(n):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        ts.append((time.perf_counter() - t0) * 1e3)
-    return float(np.median(ts))
 
 
 def main():
@@ -40,7 +25,7 @@ def main():
     grid = [3, 16, 200, 200]
     rd, rx, rx2 = build_ref.load("ref_dvr"), build_ref.load("ref_dvxlr"), build_ref.load("ref_dvxlr_v2")
     gp = torch.randn(1, 30000, device=dev)
-    out = {"config": "sigma[1,3,16,200,200], 30000 rays, 3 frames", "gpu": torch.cuda.get_device_name(0), "ms": {}}
+    out = {"config": "sigma[1,3,16,200,200], 30000 rays, 3 frames", "gpu": card(), "ms": {}}
 
     def ref_dvxlr_fb():
         pred, gt, dd, idx = rx.render(s, o, p, t)
@@ -61,7 +46,7 @@ def main():
         "dvxlr fwd+bwd (autograd layer)": (ref_dvxlr_fb, our_dvxlr_fb),
     }
     for name, (ref, ours) in cases.items():
-        out["ms"][name] = {"reference_cuda": timed(ref), "vidar_b200": timed(ours)}
+        out["ms"][name] = {"reference_cuda": host_ms(ref, 20, 5), "vidar_b200": host_ms(ours, 20, 5)}
         out["ms"][name]["speedup"] = out["ms"][name]["reference_cuda"] / out["ms"][name]["vidar_b200"]
 
     # direct comparison of outputs, full size

@@ -24,25 +24,15 @@ def build():
 
 def main():
     import torch
+    from tools.gpu_timing import card, window_ms
     from vidar_b200 import msda, synthetic
     L_ = C.CDLL(LIB)
     dev = torch.device("cuda:0")
     p = lambda t: C.c_void_p(t.data_ptr())
     st = lambda: C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
-    def timeit(fn, n=5, warm=2):
-        for _ in range(warm):
-            fn()
-        torch.cuda.synchronize()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(n):
-            fn()
-        b.record()
-        torch.cuda.synchronize()
-        return a.elapsed_time(b) / n
-
-    res = {"what": "MSDA forward / backward, ms per 6-camera pass (cfg2): reference-lineage CUDA mapping vs vidar_b200"}
+    res = {"what": "MSDA forward / backward, ms per 6-camera pass (cfg2): reference-lineage CUDA mapping vs vidar_b200",
+           "card": card()}
     for tag, rows in (("dense_40000", None), ("rebatched_10240", 10240)):
         d = synthetic.sca_like_inputs(dev, rows=rows)
         B, K, H, Cd = d["value"].shape
@@ -71,8 +61,8 @@ def main():
         rel = lambda a, b: float((a - b).abs().max() / b.abs().max())
         agree = {"out": rel(out_o, out_r), "grad_value": rel(gv_o, gv_r), "grad_attn": rel(ga_o, ga_r)}
         r = {"agreement_max_rel": agree,
-             "ref_lineage_fwd_ms": timeit(ref_f), "ref_lineage_bwd_ms": timeit(ref_b),
-             "vidar_fwd_ms": timeit(our_f), "vidar_bwd_ms": timeit(our_b)}
+             "ref_lineage_fwd_ms": window_ms(ref_f, 5, 2), "ref_lineage_bwd_ms": window_ms(ref_b, 5, 2),
+             "vidar_fwd_ms": window_ms(our_f, 5, 2), "vidar_bwd_ms": window_ms(our_b, 5, 2)}
         r["speedup_fwd"] = r["ref_lineage_fwd_ms"] / r["vidar_fwd_ms"]
         r["speedup_bwd"] = r["ref_lineage_bwd_ms"] / r["vidar_bwd_ms"]
         res[tag] = r

@@ -11,24 +11,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 from tests.inputs import dvr_inputs_lidar  # noqa: E402
+from tools.gpu_timing import card, window_ms  # noqa: E402
 from vidar_b200 import msda, ray_head, render  # noqa: E402
 from vidar_b200.modules.latent_rendering import latent_render_core  # noqa: E402
 
 dev = torch.device("cuda:0")
 PEAK = bench.peaks()[0]
-
-
-def timed(fn, n=10, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(n):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / n
 
 
 def row(ms, units, bytes_):
@@ -46,7 +34,7 @@ def msda_sca(Q):
         msda.ext_module.ms_deform_attn_backward(d["value"], d["shapes"], d["lsi"], d["loc"], d["attn"], d["grad_out"], gv, gl, ga, im2col_step=64)
     fb, bb = bench.msda_algorithmic_bytes(6 * Q, 6)
     samples = 6 * Q * 8 * 32
-    return {"fwd": row(timed(f), samples, fb), "bwd": row(timed(b), samples, bb)}
+    return {"fwd": row(window_ms(f, 10, 3), samples, fb), "bwd": row(window_ms(b, 10, 3), samples, bb)}
 
 
 def msda_tsa(n):
@@ -65,7 +53,7 @@ def msda_tsa(n):
     vb = 2 * Q * 256 * 4
     fb = vb + 2 * Q * (8 * 4 * 3 * 4 + 1024)
     bbytes = 3 * vb + 2 * Q * (8 * 4 * 3 * 4 * 2 + 1024)
-    return {"fwd": row(timed(f), 2 * Q * 8 * 4, fb), "bwd": row(timed(b), 2 * Q * 8 * 4, bbytes)}
+    return {"fwd": row(window_ms(f, 10, 3), 2 * Q * 8 * 4, fb), "bwd": row(window_ms(b, 10, 3), 2 * Q * 8 * 4, bbytes)}
 
 
 def latent(n):
@@ -76,7 +64,7 @@ def latent(n):
         o, f = occ.detach().requires_grad_(True), feat.detach().requires_grad_(True)
         p, q = latent_render_core(o, f, 256, 0.5, 1e-3, 1)
         (p.sum() + q.sum()).backward()
-    return row(timed(fb), n * n, 2 * n * n * 256 * 4 + 3 * n * n * 256 * 4)     # module bytes: 82 MB fwd + 123 MB bwd at n=200
+    return row(window_ms(fb, 10, 3), n * n, 2 * n * n * 256 * 4 + 3 * n * n * 256 * 4)     # module bytes: 82 MB fwd + 123 MB bwd at n=200
 
 
 def rays(M, T):
@@ -89,10 +77,10 @@ def rays(M, T):
         sg = s[0].detach().requires_grad_(True)
         c, v = ray_head.ray_ce(sg, o[0].contiguous(), p[0].contiguous(), fr, 512, 1.0)
         c.sum().backward()
-    return {"dvr.render(l2)": row(timed(r), M, 3 * vol + 24 * M), "ray_sampler+CE fwd+bwd": row(timed(ce), M, 3 * vol + 20 * M)}
+    return {"dvr.render(l2)": row(window_ms(r, 10, 3), M, 3 * vol + 24 * M), "ray_sampler+CE fwd+bwd": row(window_ms(ce, 10, 3), M, 3 * vol + 20 * M)}
 
 
-out = {"gpu": torch.cuda.get_device_name(0), "hbm_peak_GBps": PEAK,
+out = {"gpu": card(), "hbm_peak_GBps": PEAK,
        "msda_sca_6cam": {f"Q={Q}": msda_sca(Q) for Q in (10000, 40000)},
        "msda_tsa_B2": {f"bev={n}x{n}": msda_tsa(n) for n in (100, 200, 400)},
        "latent_render_core_fwd_bwd": {f"bev={n}x{n}": latent(n) for n in (100, 200, 400)},
