@@ -657,6 +657,31 @@ int vidar_image_aug_apply(const unsigned char* src, unsigned char* mid, float* o
                           int flip, int to_rgb, const float* mean, const double* stdinv, const float* pad_val, int Hp,
                           int Wp, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (xi) The point half of a pre-training sample (datasets/pipelines/loading.py CustomLoadPointsFromMultiSweeps,
+ * CustomVoxelBasedPointSampler over mmdet3d 0.17.1's VoxelBasedPointSampler; nuscenes_vidar_dataset_v1.py union2one's
+ * point statements) for every frame of a queue, in a fixed number of launches on `stream`.
+ *   raw      float32 raw points, rows of 5 (device); seg_i [S, 5] int64 and seg_d [S, 16] double (device): per
+ *            segment raw row offset, n, offset in the call's point space, filter (0 none, 1 remove-close, 2 also the
+ *            ego box), transform (0 / 1); R row-major, t, ego box (x_lo, y_lo, x_hi, y_hi).  Segments are frame-major
+ *            and the call's point space is their concatenation (n_g points).
+ *   frame_i  [F, 10] int64 (device): merged offset, merged count, output row offset, output rows, queue index,
+ *            voxel sampler (0 / 1), grid offset, perm offset, point-space offset, point-space count;
+ *            frame_f [F, 6] float (voxel lo, voxel size), frame_g [F, 3] int64 (grid dims) (device)
+ *   perm     int32 (device): per voxel frame its shuffled order of the merged points (numpy's draws)
+ *   n_cur    merged points over all frames (the host's count), cells = voxel grid cells over all frames
+ *   ego      host float[4] (x_lo, y_lo, x_hi, y_hi) of union2one's mask, or NULL for no mask
+ *   out      [rows, 5] float32 (device): each frame's kept points (x, y, z, intensity, queue index) in the
+ *            reference's order within its rows; masked and unused rows are NaN
+ *   counts   optional int32 [F, 2] (device): per frame the merged points and the kept points the device found
+ *   out_compact / count: optional float32 [rows, 5] and int64 [1] (device): the non-NaN rows in order and their number
+ * Needs every n below 2^31.  No host sync. */
+int vidar_point_pipeline_gather(const float* raw, const int64_t* seg_i, const double* seg_d, int S,
+                                const int64_t* frame_i, const float* frame_f, const int64_t* frame_g, int F,
+                                const int32_t* perm, long long n_g, long long n_cur, long long cells, const float* ego,
+                                float* out, long long rows, int32_t* counts, float* out_compact, int64_t* count,
+                                void* stream);
+
 #ifdef __cplusplus
 }
 #endif

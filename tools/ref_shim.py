@@ -259,3 +259,316 @@ def install_pipelines():
                                                       os.path.join(REF_PIPELINES, fname))
         spec.loader.exec_module(importlib.util.module_from_spec(spec))
     return pipelines.modules
+
+
+REF_DATASETS = "/root/reference/projects/mmdet3d_plugin/datasets"
+
+
+def _load_methods(path, cls_name, names, ns):
+    """Execute only the named methods of class `cls_name` in a reference file, as plain functions in `ns`."""
+    import ast
+    with open(path) as fh:
+        tree = ast.parse(fh.read(), filename=path)
+    for node in tree.body:
+        if isinstance(node, ast.ClassDef) and node.name == cls_name:
+            for item in node.body:
+                if isinstance(item, ast.FunctionDef) and item.name in names:
+                    exec(compile(ast.Module([item], []), path, "exec"), ns)
+    return {n: ns[n] for n in names}
+
+
+def install_point_pipelines(files=None):
+    """Load the reference's point transforms (datasets/pipelines/loading.py) and NuScenesViDARDatasetV1's
+    `_mask_points` / `union2one` (nuscenes_vidar_dataset_v1.py) with stand-ins for what they take from mmcv, mmdet,
+    mmdet3d and nuscenes-devkit:
+      * `mmcv.FileClient` (reads the file, or `files[path]` when a dict of preloaded bytes is given),
+        `mmcv.check_file_exist`, `mmcv.parallel.DataContainer`, `mmdet.datasets.builder.PIPELINES`;
+      * `BasePoints` / `LiDARPoints` (`tensor`, `shape`, `new_point`, `cat`, column and mask indexing) and
+        `get_points_type`, restated from mmdet3d 0.17.1's core/points/base_points.py;
+      * mmdet3d 0.17.1's `LoadPointsFromFile` and `VoxelBasedPointSampler`, with its `VoxelGenerator` /
+        `points_to_voxel` / `_points_to_voxel_reverse_kernel` run by numba, restated from
+        datasets/pipelines/loading.py, transforms_3d.py and core/voxel/voxel_generator.py;
+      * `transform_matrix` and `Quaternion` (nuscenes-devkit / pyquaternion's definitions).
+    mmdet3d is not part of the reference tree, so the voxel sampler step is checked against this restatement of
+    upstream, not against upstream itself.
+    -> dict of the classes and `union2one(previous_queue, future_queue, ego_mask)`."""
+    import numba
+    import numpy as np
+    install()
+
+    class FileClient:
+        def __init__(self, backend="disk", **kw):
+            self.backend = backend
+
+        def get(self, path):
+            if files is not None:
+                return files[path]
+            with open(path, "rb") as fh:
+                return fh.read()
+
+    class DataContainer:
+        def __init__(self, data, stack=False, padding_value=0, cpu_only=False, pad_dims=2):
+            self.data, self.stack, self.cpu_only = data, stack, cpu_only
+
+    class BasePoints:
+        def __init__(self, tensor, points_dim=3, attribute_dims=None):
+            device = tensor.device if isinstance(tensor, torch.Tensor) else torch.device("cpu")
+            tensor = torch.as_tensor(tensor, dtype=torch.float32, device=device)
+            if tensor.numel() == 0:
+                tensor = tensor.reshape((0, points_dim)).to(dtype=torch.float32, device=device)
+            assert tensor.dim() == 2 and tensor.size(-1) == points_dim, tensor.size()
+            self.tensor, self.points_dim, self.attribute_dims = tensor, points_dim, attribute_dims
+
+        @property
+        def shape(self):
+            return self.tensor.shape
+
+        @property
+        def device(self):
+            return self.tensor.device
+
+        def new_point(self, data):
+            new_tensor = self.tensor.new_tensor(data) if not isinstance(data, torch.Tensor) else data.to(self.device)
+            return type(self)(new_tensor, points_dim=self.points_dim, attribute_dims=self.attribute_dims)
+
+        @classmethod
+        def cat(cls, points_list):
+            return cls(torch.cat([p.tensor for p in points_list]), points_dim=points_list[0].tensor.shape[1],
+                       attribute_dims=points_list[0].attribute_dims)
+
+        def __len__(self):
+            return self.tensor.shape[0]
+
+        def __getitem__(self, item):
+            if isinstance(item, tuple) and len(item) == 2:
+                cols = item[1]
+                if isinstance(cols, slice):
+                    cols = list(range(cols.start or 0, self.tensor.shape[1] if cols.stop is None else cols.stop,
+                                      cols.step or 1))
+                elif isinstance(cols, int):
+                    cols = [cols]
+                p = self.tensor[item[0], cols]
+            elif isinstance(item, (slice, np.ndarray, torch.Tensor)):
+                p = self.tensor[item]
+            else:
+                raise NotImplementedError(type(item))
+            return type(self)(p, points_dim=p.shape[1], attribute_dims=self.attribute_dims)
+
+    class LiDARPoints(BasePoints):
+        pass
+
+    def get_points_type(points_type):
+        assert points_type == "LIDAR", points_type
+        return LiDARPoints
+
+    @numba.jit(nopython=True)
+    def _points_to_voxel_reverse_kernel(points, voxel_size, coors_range, num_points_per_voxel, coor_to_voxelidx,
+                                        voxels, coors, max_points=35, max_voxels=20000):
+        N = points.shape[0]
+        ndim = 3
+        ndim_minus_1 = ndim - 1
+        grid_size = (coors_range[3:] - coors_range[:3]) / voxel_size
+        grid_size = np.round(grid_size, 0, grid_size).astype(np.int32)
+        coor = np.zeros(shape=(3, ), dtype=np.int32)
+        voxel_num = 0
+        failed = False
+        for i in range(N):
+            failed = False
+            for j in range(ndim):
+                c = np.floor((points[i, j] - coors_range[j]) / voxel_size[j])
+                if c < 0 or c >= grid_size[j]:
+                    failed = True
+                    break
+                coor[ndim_minus_1 - j] = c
+            if failed:
+                continue
+            voxelidx = coor_to_voxelidx[coor[0], coor[1], coor[2]]
+            if voxelidx == -1:
+                voxelidx = voxel_num
+                if voxel_num >= max_voxels:
+                    continue
+                voxel_num += 1
+                coor_to_voxelidx[coor[0], coor[1], coor[2]] = voxelidx
+                coors[voxelidx] = coor
+            num = num_points_per_voxel[voxelidx]
+            if num < max_points:
+                voxels[voxelidx, num] = points[i]
+                num_points_per_voxel[voxelidx] += 1
+        return voxel_num
+
+    def points_to_voxel(points, voxel_size, coors_range, max_points=35, reverse_index=True, max_voxels=20000):
+        assert reverse_index
+        voxelmap_shape = (coors_range[3:] - coors_range[:3]) / voxel_size
+        voxelmap_shape = tuple(np.round(voxelmap_shape).astype(np.int32).tolist())[::-1]
+        num_points_per_voxel = np.zeros(shape=(max_voxels, ), dtype=np.int32)
+        coor_to_voxelidx = -np.ones(shape=voxelmap_shape, dtype=np.int32)
+        voxels = np.zeros(shape=(max_voxels, max_points, points.shape[-1]), dtype=points.dtype)
+        coors = np.zeros(shape=(max_voxels, 3), dtype=np.int32)
+        voxel_num = _points_to_voxel_reverse_kernel(points, voxel_size, coors_range, num_points_per_voxel,
+                                                    coor_to_voxelidx, voxels, coors, max_points, max_voxels)
+        return voxels[:voxel_num], coors[:voxel_num], num_points_per_voxel[:voxel_num]
+
+    class VoxelGenerator:
+        def __init__(self, voxel_size, point_cloud_range, max_num_points, max_voxels=20000):
+            point_cloud_range = np.array(point_cloud_range, dtype=np.float32)
+            voxel_size = np.array(voxel_size, dtype=np.float32)
+            grid_size = (point_cloud_range[3:] - point_cloud_range[:3]) / voxel_size
+            self._voxel_size, self._point_cloud_range = voxel_size, point_cloud_range
+            self._max_num_points, self._max_voxels = max_num_points, max_voxels
+            self._grid_size = np.round(grid_size).astype(np.int64)
+
+        def generate(self, points):
+            return points_to_voxel(points, self._voxel_size, self._point_cloud_range, self._max_num_points, True,
+                                   self._max_voxels)
+
+    class VoxelBasedPointSampler:
+        def __init__(self, cur_sweep_cfg, prev_sweep_cfg=None, time_dim=3):
+            self.cur_voxel_generator = VoxelGenerator(**cur_sweep_cfg)
+            self.cur_voxel_num = self.cur_voxel_generator._max_voxels
+            self.time_dim = time_dim
+            if prev_sweep_cfg is not None:
+                assert prev_sweep_cfg["max_num_points"] == cur_sweep_cfg["max_num_points"]
+                self.prev_voxel_generator = VoxelGenerator(**prev_sweep_cfg)
+                self.prev_voxel_num = self.prev_voxel_generator._max_voxels
+            else:
+                self.prev_voxel_generator = None
+                self.prev_voxel_num = 0
+
+        def _sample_points(self, points, sampler, point_dim):
+            voxels, coors, num_points_per_voxel = sampler.generate(points)
+            if voxels.shape[0] < sampler._max_voxels:
+                padding_points = np.zeros([sampler._max_voxels - voxels.shape[0], sampler._max_num_points,
+                                           point_dim], dtype=points.dtype)
+                padding_points[:] = voxels[0]
+                sample_points = np.concatenate([voxels, padding_points], axis=0)
+            else:
+                sample_points = voxels
+            return sample_points
+
+        def __call__(self, results):
+            points = results["points"]
+            original_dim = points.shape[1]
+            map_fields2dim = []
+            start_dim = original_dim
+            points_numpy = points.tensor.numpy()
+            extra_channel = [points_numpy]
+            for idx, key in enumerate(results["pts_mask_fields"]):
+                map_fields2dim.append((key, idx + start_dim))
+                extra_channel.append(results[key][..., None])
+            start_dim += len(results["pts_mask_fields"])
+            for idx, key in enumerate(results["pts_seg_fields"]):
+                map_fields2dim.append((key, idx + start_dim))
+                extra_channel.append(results[key][..., None])
+            points_numpy = np.concatenate(extra_channel, axis=-1)
+            cur_points_flag = (points_numpy[:, self.time_dim] == 0)
+            cur_sweep_points = points_numpy[cur_points_flag]
+            prev_sweeps_points = points_numpy[~cur_points_flag]
+            if prev_sweeps_points.shape[0] == 0:
+                prev_sweeps_points = cur_sweep_points
+            np.random.shuffle(cur_sweep_points)
+            np.random.shuffle(prev_sweeps_points)
+            cur_sweep_points = self._sample_points(cur_sweep_points, self.cur_voxel_generator,
+                                                   points_numpy.shape[1])
+            if self.prev_voxel_generator is not None:
+                prev_sweeps_points = self._sample_points(prev_sweeps_points, self.prev_voxel_generator,
+                                                         points_numpy.shape[1])
+                points_numpy = np.concatenate([cur_sweep_points, prev_sweeps_points], 0)
+            else:
+                points_numpy = cur_sweep_points
+            if self.cur_voxel_generator._max_num_points == 1:
+                points_numpy = points_numpy.squeeze(1)
+            results["points"] = points.new_point(points_numpy[..., :original_dim])
+            for key, dim_index in map_fields2dim:
+                results[key] = points_numpy[..., dim_index]
+            return results
+
+    class LoadPointsFromFile:
+        def __init__(self, coord_type, load_dim=6, use_dim=[0, 1, 2], shift_height=False, use_color=False,
+                     file_client_args=dict(backend="disk")):
+            assert not shift_height and not use_color
+            if isinstance(use_dim, int):
+                use_dim = list(range(use_dim))
+            assert max(use_dim) < load_dim
+            self.coord_type, self.load_dim, self.use_dim = coord_type, load_dim, use_dim
+            self.file_client_args = file_client_args.copy()
+            self.file_client = None
+
+        def _load_points(self, pts_filename):
+            if self.file_client is None:
+                self.file_client = FileClient(**self.file_client_args)
+            return np.frombuffer(self.file_client.get(pts_filename), dtype=np.float32)
+
+        def __call__(self, results):
+            points = self._load_points(results["pts_filename"])
+            points = points.reshape(-1, self.load_dim)
+            points = points[:, self.use_dim]
+            points = get_points_type(self.coord_type)(points, points_dim=points.shape[-1], attribute_dims=None)
+            results["points"] = points
+            return results
+
+    class Quaternion:
+        def __init__(self, q):
+            self.q = np.asarray(q, np.float64)
+
+        @property
+        def rotation_matrix(self):
+            w, x, y, z = self.q / np.linalg.norm(self.q)
+            return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                             [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                             [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+    def transform_matrix(translation=np.array([0, 0, 0]), rotation=Quaternion([1, 0, 0, 0]), inverse=False):
+        tm = np.eye(4)
+        if inverse:
+            rot_inv = rotation.rotation_matrix.T
+            tm[:3, :3] = rot_inv
+            tm[:3, 3] = rot_inv.dot(np.transpose(-np.array(translation)))
+        else:
+            tm[:3, :3] = rotation.rotation_matrix
+            tm[:3, 3] = np.transpose(np.array(translation))
+        return tm
+
+    mmcv = sys.modules["mmcv"]
+    mmcv.FileClient = FileClient
+    mmcv.check_file_exist = lambda *a, **k: None
+    parallel = types.ModuleType("mmcv.parallel")
+    parallel.DataContainer = DataContainer
+    sys.modules["mmcv.parallel"] = parallel
+    pipelines = _Registry()
+    for name in ("mmdet.datasets", "mmdet.datasets.builder"):
+        m = _Permissive(name)
+        m.__path__ = []
+        m.PIPELINES = pipelines
+        sys.modules[name] = m
+    points_mod = types.ModuleType("mmdet3d.core.points")
+    points_mod.BasePoints, points_mod.LiDARPoints, points_mod.get_points_type = BasePoints, LiDARPoints, get_points_type
+    sys.modules["mmdet3d.core"] = _Permissive("mmdet3d.core")
+    sys.modules["mmdet3d.core"].__path__ = []
+    sys.modules["mmdet3d.core.points"] = points_mod
+    dp = types.ModuleType("mmdet3d.datasets.pipelines")
+    dp.VoxelBasedPointSampler = VoxelBasedPointSampler
+    sys.modules["mmdet3d.datasets"] = _Permissive("mmdet3d.datasets")
+    sys.modules["mmdet3d.datasets"].__path__ = []
+    sys.modules["mmdet3d.datasets.pipelines"] = dp
+    spec = importlib.util.spec_from_file_location("vidar_ref_pipelines_loading", os.path.join(REF_PIPELINES, "loading.py"))
+    loading = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(loading)
+
+    ns = dict(np=np, torch=torch, copy=__import__("copy"), DC=DataContainer, transform_matrix=transform_matrix,
+              Quaternion=Quaternion)
+    meths = _load_methods(os.path.join(REF_DATASETS, "nuscenes_vidar_dataset_v1.py"), "NuScenesViDARDatasetV1",
+                          ("_mask_points", "union2one"), ns)
+
+    class _Dataset:
+        _mask_points = meths["_mask_points"]
+        union2one = meths["union2one"]
+
+    def union2one(previous_queue, future_queue, ego_mask):
+        ds = _Dataset()
+        ds.ego_mask, ds.future_length = ego_mask, len(future_queue) - 1
+        return ds.union2one(previous_queue, future_queue)
+
+    return dict(LoadPointsFromFile=LoadPointsFromFile,
+                CustomLoadPointsFromMultiSweeps=loading.CustomLoadPointsFromMultiSweeps,
+                CustomVoxelBasedPointSampler=loading.CustomVoxelBasedPointSampler, LiDARPoints=LiDARPoints,
+                DataContainer=DataContainer, union2one=union2one)

@@ -31,6 +31,7 @@ Sharding over a process group (one sample on all ranks -- the reference has repl
 """
 import copy
 import math
+import os
 
 import numpy as np
 import torch
@@ -40,12 +41,14 @@ import torch.nn.functional as F
 from . import bev_geometry, sca, sharding, synthetic
 from . import modules as _modules  # noqa: F401  (registers the attention classes)
 from . import image_aug
+from . import point_pipeline as point_aug
 from .grid_mask import GridMask
 from .head import ViDARRayHead
 from .modules.deform_attn import _linear
 from .registry import build_attention
 
 PC_RANGE = [-51.2, -51.2, -5.0, 51.2, 51.2, 3.0]
+EGO_MASK = (-0.8, -1.5, 0.8, 2.5)                    # the dataset's ego_mask (config :348)
 EMBED, BEV_H, BEV_W, HEIGHTS = 256, 200, 200, 16
 
 
@@ -298,12 +301,21 @@ class SyntheticViDAR(nn.Module):
     come first, as the dataloader makes them before the step; then each frame's images go through
     `apply_multiview` before the backbone (and GridMask, when on).  bs must be 1 (samples_per_gpu=1).  Under a
     process group every rank draws for all cameras -- numpy and `random` seeded alike on every rank -- and processes
-    only its backbone cameras.  The default False leaves the graph as it was."""
+    only its backbone cameras.  The default False leaves the graph as it was.
+
+    `point_pipeline=True` builds gt_points from raw LiDAR frames on the device (`vidar_b200.point_pipeline`):
+    forward_train / forward_test then take `point_infos`, one results dict per GT frame in queue order (the current
+    frame, then the future ones; `synthetic_sample(..., raw_points=True)`), and ignore their gt_points argument.
+    Training runs the train pipeline's point transforms (vidar_1_8_nusc_3future.py:279-305) on every GT frame first,
+    in queue order, the test path LoadPointsFromFile only (:319-324); then `gather_gt_points` with the dataset's
+    ego mask makes the padded [1, R, 5] gt_points with no host sync.  The default False leaves the graph as it was."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
                  latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None,
-                 grid_mask=False, image_pipeline=False):
+                 grid_mask=False, image_pipeline=False, point_pipeline=False):
         super().__init__()
+        self.point_transforms = ((point_aug.config_train_pipeline(PC_RANGE), point_aug.config_test_pipeline())
+                                 if point_pipeline else None)
         self.image_transforms = image_aug.config_pipeline() if image_pipeline else None
         if backbone_autocast not in (None, torch.float16, torch.bfloat16):
             raise ValueError(f"backbone_autocast must be None, torch.float16 or torch.bfloat16 (got {backbone_autocast})")
@@ -556,12 +568,29 @@ class SyntheticViDAR(nn.Module):
         next_bev_feats = torch.stack(next_bev_feats, 0)
         return self.forward_head(next_bev_feats)                                        # [F, inter, pred_frame, bs, Q, 16]
 
+    def gt_points_of(self, point_infos, training):
+        """The point half of the sample with the point pipeline: every GT frame's transforms in queue order (numpy's
+        draws), then one device pass -> gt_points [1, R, 5] (NaN rows belong to no frame)."""
+        if not point_infos:
+            raise ValueError("point_pipeline: forward needs point_infos (synthetic_sample(..., raw_points=True))")
+        steps = self.point_transforms[0 if training else 1]
+        frames = []
+        for info in point_infos:
+            results = dict(info)
+            for step in steps:
+                results = step(results)
+            frames.append(results)
+        return point_aug.gather_gt_points(frames, EGO_MASK, self.future_bev_embedding.weight.device)
+
     # ---- one training forward (vidar.py:239-387) -> dict of losses ----
-    def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None):
+    def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None, point_infos=None):
         """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
         (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
         frame index 0 = current .. future_frames).  With the image pipeline: img uint8 [1, T, cams, H, W, 3] and
-        host cam2img / lidar2cam [1, cams, 4, 4]; lidar2img is not read."""
+        host cam2img / lidar2cam [1, cams, 4, 4]; lidar2img is not read.  With the point pipeline gt_points is built
+        from point_infos."""
+        if self.point_transforms is not None:
+            gt_points = self.gt_points_of(point_infos, True)
         next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames, cam2img, lidar2cam)
         valid_frames = list(range(1 + self.future_frames))
         losses = {}
@@ -584,12 +613,15 @@ class SyntheticViDAR(nn.Module):
         next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames)
         return dict(next_bev_preds=next_bev_preds, valid_frames=list(range(1 + future_frames)))
 
-    def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None):
+    def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None, point_infos=None):
         """vidar.py:389-502 without submission writing and visualisation -> [ret_dict], ret_dict =
         {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}} for the current frame (t = 0) and every
         future frame, scored on the current head frame (`history_frames`) by ray_head.evaluate (one batched device
         pass).  gt_points as forward_train's, frames 0 .. future_frames; the origin is zero in every frame.  Under a
-        process group every rank computes the same result."""
+        process group every rank computes the same result.  With the point pipeline gt_points is built from
+        point_infos by the test pipeline."""
+        if self.point_transforms is not None:
+            gt_points = self.gt_points_of(point_infos, False)
         pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus)
         cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.history_frames])
         with torch.no_grad():
@@ -601,11 +633,15 @@ class SyntheticViDAR(nn.Module):
 # synthetic sample + step
 # ------------------------------------------------------------------------------------------------
 def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000, future_frames=3, seed=0,
-                     bev_hw=(BEV_H, BEV_W), raw_images=False):
+                     bev_hw=(BEV_H, BEV_W), raw_images=False, raw_points=False, points_per_frame=35000):
     """6 x 3 x 928 x 1600 N(0,1) frames, a nuScenes-like rig, LiDAR-like future point clouds (SURVEY.md 8d cfg4).
     `raw_images=True` (for `SyntheticViDAR(image_pipeline=True)`): seeded uniform uint8 BGR frames
     [1, frames, cams, 900, 1600, 3] (img_hw defaults to the camera size) and the rig's host `cam2img` / `lidar2cam`
-    [1, cams, 4, 4] float64 as well."""
+    [1, cams, 4, 4] float64 as well.
+    `raw_points=True` (for `SyntheticViDAR(point_pipeline=True)`): `point_infos`, the results dicts of the
+    1 + future_frames GT frames, each a LiDAR-like key frame and 2 sweeps of `points_per_frame` points with their
+    own poses and timestamps (`synthetic.lidar_cloud`, `synthetic.sweep_pose`), written as .bin files to a
+    temporary directory that is removed when the process exits."""
     g = torch.Generator(device=device).manual_seed(seed)
     extra = {}
     if raw_images:
@@ -627,7 +663,33 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000
                     p[:, 1] / bev_hw[0] * (PC_RANGE[4] - PC_RANGE[1]) + PC_RANGE[1],
                     p[:, 2] / HEIGHTS * (PC_RANGE[5] - PC_RANGE[2]) + PC_RANGE[2]], -1)
     pts.append(torch.from_numpy(np.concatenate([xyz, tindex[0][:, None]], -1).astype(np.float32)).to(device))
+    if raw_points:
+        extra["point_infos"] = synthetic_point_infos(1 + future_frames, points_per_frame, seed)
     return dict(img=img, lidar2img=lidar2img, gt_points=pts, **extra)
+
+
+def synthetic_point_infos(frames, n, seed=0, sweeps=2):
+    """Results dicts (pts_filename, timestamp, sweeps) of `frames` LiDAR frames, files in a temporary directory."""
+    import atexit
+    import shutil
+    import tempfile
+    root = tempfile.mkdtemp(prefix="vidar_points_")
+    atexit.register(shutil.rmtree, root, True)
+    rng = np.random.default_rng(seed)
+    infos = []
+    for f in range(frames):
+        ts = 1533151603547590 + 500000 * f
+        key = os.path.join(root, f"{f}.bin")
+        synthetic.lidar_cloud(rng, n).tofile(key)
+        sw = []
+        for j in range(sweeps):
+            path = os.path.join(root, f"{f}.sweep{j}.bin")
+            synthetic.lidar_cloud(rng, n).tofile(path)
+            R, t = synthetic.sweep_pose(rng, j + 1)
+            sw.append(dict(data_path=path, timestamp=ts - 50000 * (j + 1), sensor2lidar_rotation=R,
+                           sensor2lidar_translation=t))
+        infos.append(dict(pts_filename=key, timestamp=ts / 1e6, sweeps=sw))
+    return infos
 
 
 def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
@@ -640,7 +702,7 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
         model._mark("start")
     optimizer.zero_grad(set_to_none=True)
     losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"], cam2img=sample.get("cam2img"),
-                                 lidar2cam=sample.get("lidar2cam"))
+                                 lidar2cam=sample.get("lidar2cam"), point_infos=sample.get("point_infos"))
     loss = sum(losses.values())
     (loss if scaler is None else scaler.scale(loss)).backward()
     model._mark("backward")

@@ -125,3 +125,32 @@ def camera_rig_split(cams=6, f=1266.0, pp=(816.0, 491.0), cam_height=1.5, seed=0
         E[:3, 3] = -R @ (fwd * 1.0 + np.array([0, 0, cam_height]))
         exts.append(E)
     return np.stack([K] * len(exts), 0), np.stack(exts, 0)
+
+
+def lidar_cloud(rng, n, lattice=64):
+    """A LiDAR-like float32 [n, 5] cloud (x, y, z, intensity, ring) on a 1/lattice m grid: 32 rings of ground and
+    walls, a few percent of the points inside the ego box (-0.8..0.8, -1.5..2.5), inside the 1 m square around the
+    sensor and outside the +-51.2 m range."""
+    kind = rng.choice(4, n, p=[0.9, 0.04, 0.03, 0.03])
+    ring = rng.integers(0, 32, n)
+    ang = rng.uniform(-np.pi, np.pi, n)
+    r = np.where(ring < 24, 2.5 + 1.6 * ring + rng.normal(0, 0.05, n), rng.uniform(5.0, 45.0, n))
+    z = np.where(ring < 24, -1.8 + rng.normal(0, 0.03, n), rng.uniform(-1.5, 2.5, n))
+    x, y = r * np.cos(ang), r * np.sin(ang)
+    ego, close = kind == 1, kind == 2
+    x[ego], y[ego] = rng.uniform(-0.8, 0.8, ego.sum()), rng.uniform(-1.5, 2.5, ego.sum())
+    x[close], y[close] = rng.uniform(-1.0, 1.0, close.sum()), rng.uniform(-1.0, 1.0, close.sum())
+    far = kind == 3
+    x[far], y[far] = 51.2 + rng.uniform(0.0, 20.0, far.sum()) * np.sign(x[far]), y[far] * 1.5
+    pts = np.stack([x, y, z, rng.integers(0, 100, n), ring], 1)
+    return (np.round(pts * lattice) / lattice).astype(np.float32)
+
+
+def sweep_pose(rng, k):
+    """(sensor2lidar_rotation, sensor2lidar_translation) float64 of the k-th earlier sweep: the ego moving about
+    0.5 m and turning about 0.3 degrees per sweep, with a slight roll."""
+    yaw, roll = rng.normal(0, 0.005) * k, rng.normal(0, 0.001)
+    cz, sz, cr, sr = np.cos(yaw), np.sin(yaw), np.cos(roll), np.sin(roll)
+    R = np.array([[cz, -sz, 0.0], [sz, cz, 0.0], [0.0, 0.0, 1.0]]) @ np.array([[1.0, 0, 0], [0, cr, -sr], [0, sr, cr]])
+    t = np.array([-0.5 * k + rng.normal(0, 0.02), rng.normal(0, 0.02), rng.normal(0, 0.01)])
+    return R, t
