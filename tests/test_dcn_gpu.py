@@ -191,17 +191,23 @@ SMALL = dict(encoder_layers=2, decoder_layers=2, future_frames=2, bev_hw=(40, 40
 SAMPLE = dict(frames=2, img_hw=(96, 160), rays_per_frame=800, future_frames=2, bev_hw=(40, 40))
 
 
-def test_pretrain_step_with_dcn(cuda):
+def run_reduced_pretrain_step(dev):
+    """(model, loss) of one pre-training step of the SMALL model with the DCN backbone on a SAMPLE-sized input."""
     from vidar_b200 import pretrain
     from vidar_b200 import synthetic
-    model, opt = pretrain.build(cuda, None, seed=1, **SMALL)
-    sample = pretrain.synthetic_sample(cuda, **SAMPLE)
+    model, opt = pretrain.build(dev, None, seed=1, **SMALL)
+    sample = pretrain.synthetic_sample(dev, **SAMPLE)
     # the rig's intrinsics are for the full image: scale its pixel rows to the small one so pillars project inside
     l2i = sample["lidar2img"].copy()
     l2i[..., 0, :] *= SAMPLE["img_hw"][1] / synthetic.IMG_HW[1]
     l2i[..., 1, :] *= SAMPLE["img_hw"][0] / synthetic.IMG_HW[0]
     sample["lidar2img"] = l2i
     loss, _ = pretrain.train_step(model, opt, sample, None)
+    return model, loss
+
+
+def test_pretrain_step_with_dcn(cuda):
+    model, loss = run_reduced_pretrain_step(cuda)
     assert torch.isfinite(loss)
     offs = [(n, p) for n, p in model.named_parameters() if "conv_offset" in n]
     assert len(offs) == 2 * 26

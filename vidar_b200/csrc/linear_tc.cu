@@ -7,6 +7,10 @@
 // parity bar.  3xTF32: x = x_hi + x_lo, w = w_hi + w_lo with tf32 parts,
 //     x w  ~=  x_hi w_hi + x_hi w_lo + x_lo w_hi          (dropped term ~2^-22 relative)
 // three wgmma.mma_async (tf32, m64n128k8) per K step accumulating in fp32 registers.
+// The tensor core truncates every sum it accumulates (round toward zero), so one accumulator chained through all
+// 3 K / 8 wgmma carries an error that does not cancel and grows like K (measured at K = 4608: 27x fp32 cuBLAS's RMS
+// error).  Each K block is therefore summed in two fresh accumulators of 6 wgmma each, the small x_hi w_lo and
+// x_lo w_hi products first, and added into the running sum by ordinary round-to-nearest FADDs.
 //
 // Kernel (one persistent CTA per SM, 3 warpgroups, mbarrier pipeline of kStages stages):
 //   warp 0        TMA producer: per K block (32 floats = one 128-byte swizzle row) the raw X tile [128 x 32] and
@@ -14,10 +18,13 @@
 //   warpgroups 1-2  consumers, one per 64-row half of the tile: split their half of the raw X tile in place
 //                 (x_hi to its own tile, x_lo over the raw values: the split is element-wise, so the TMA's swizzle
 //                 pattern is preserved), fence.proxy.async, then 4 K steps x 3 products of wgmma m64n128k8
-//                 with shared-memory descriptors (K-major, SWIZZLE_128B); after the last K block, + bias and
+//                 with shared-memory descriptors (K-major, SWIZZLE_128B) into the block accumulators, which are then
+//                 added to the tile's running sum; after the last K block, + bias and
 //                 8-byte stores straight from the accumulator registers.  The producer runs ahead into the
 //                 next tile while the consumers store, so loads overlap the epilogue.
 // Tiles: (row block of 128) x (column block of 128); K = in_features is looped in blocks of 32.
+// Registers: a consumer thread holds 3 x 64 accumulators, more than the 168 per thread __launch_bounds__(384, 1)
+// allows, so the producer warpgroup drops to 40 (setmaxnreg) and the two consumer warpgroups take 232.
 // Requires in_features % 32 == 0, out_features % 128 == 0; rows are arbitrary (TMA clips, stores are guarded).
 #include <cuda.h>
 #include <stdlib.h>
@@ -72,9 +79,9 @@ __device__ __forceinline__ unsigned long long gmma_desc(const void* tile, int k_
   d |= 1ull << 62;
   return d;
 }
-// d[64x128] += a[64x8] b[8x128]^T, tf32 operands from shared memory, fp32 accumulators in registers
-// (thread layout: d[4j + 2h + e] is row 16 warp + lane / 4 + 8h, column 8j + 2 (lane % 4) + e).
-__device__ __forceinline__ void wgmma_tf32(float (&d)[64], unsigned long long a, unsigned long long b) {
+// d[64x128] = (accumulate ? d : 0) + a[64x8] b[8x128]^T, tf32 operands from shared memory, fp32 accumulators in
+// registers (thread layout: d[4j + 2h + e] is row 16 warp + lane / 4 + 8h, column 8j + 2 (lane % 4) + e).
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], unsigned long long a, unsigned long long b, int accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "setp.ne.b32 p, %66, 0;\n\t"
@@ -92,7 +99,7 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], unsigned long long a,
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(1));
+      : "l"(a), "l"(b), "r"(accumulate));
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -137,9 +144,10 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
       unsigned it = 0;
       for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         const int tm = t / g.tiles_n, tn = t % g.tiles_n;
@@ -157,10 +165,14 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
     }
   } else if (warp >= 4) {
     // ===== consumers: warpgroup c owns rows [64 c, 64 c + 64) of the tile =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int c = (warp >> 2) - 1;
     const int tid = threadIdx.x & 127;
     const int half = c * (kTileBytes / 2);                       // byte offset of this half in an operand tile
     unsigned it = 0;
+    float p0[64], p1[64];                                        // the K block's sums of k steps 0-1 and 2-3
+#pragma unroll
+    for (int i = 0; i < 64; ++i) p0[i] = p1[i] = 0.f;
     for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
       const int tm = t / g.tiles_n, tn = t % g.tiles_n;
       float d[64];
@@ -189,20 +201,30 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
         const unsigned char* xhi = st + kTileBytes + half;
         const unsigned char* whi = st + 2 * kTileBytes;
         const unsigned char* wlo = st + 3 * kTileBytes;
-        fence_acc(d);
+        fence_acc(p0);
+        fence_acc(p1);
         wgmma_fence();
+        // tf32: K = 8 per instruction = 32 bytes.  The first product of each accumulator overwrites it.
 #pragma unroll
-        for (int k = 0; k < kTK / 8; ++k) {                      // tf32: K = 8 per instruction = 32 bytes
-          const int ko = k * 32;
-          wgmma_tf32(d, gmma_desc(xhi, ko), gmma_desc(whi, ko));
-          wgmma_tf32(d, gmma_desc(xhi, ko), gmma_desc(wlo, ko));
-          wgmma_tf32(d, gmma_desc(xlo, ko), gmma_desc(whi, ko));
+        for (int k = 0; k < 2; ++k) {
+          wgmma_tf32(p0, gmma_desc(xhi, 32 * k), gmma_desc(wlo, 32 * k), k);
+          wgmma_tf32(p0, gmma_desc(xlo, 32 * k), gmma_desc(whi, 32 * k), 1);
+          wgmma_tf32(p1, gmma_desc(xhi, 32 * k + 64), gmma_desc(wlo, 32 * k + 64), k);
+          wgmma_tf32(p1, gmma_desc(xlo, 32 * k + 64), gmma_desc(whi, 32 * k + 64), 1);
+        }
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          wgmma_tf32(p0, gmma_desc(xhi, 32 * k), gmma_desc(whi, 32 * k), 1);
+          wgmma_tf32(p1, gmma_desc(xhi, 32 * k + 64), gmma_desc(whi, 32 * k + 64), 1);
         }
         wgmma_commit();
         wgmma_wait_all();
-        fence_acc(d);
+        fence_acc(p0);
+        fence_acc(p1);
         __syncwarp();
         if (lane == 0) mb_arrive(&empty[s]);                     // this warp's reads of the stage are done
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] += p0[i] + p1[i];
       }
       // ===== epilogue: registers + bias -> global =====
       const int row0 = tm * kTM + c * 64 + (warp & 3) * 16 + (lane >> 2);

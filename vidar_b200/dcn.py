@@ -36,9 +36,10 @@ from . import linear as _tc
 from .registry import CONV_LAYERS
 
 MAX_COLS_BYTES = 512 << 20
-# Longest contraction given to the 3xTF32 GEMM.  Its error grows with K faster than fp32 cuBLAS's: at the backbone's
-# forward K = 2304 / 4608 the output was 6x / 20x farther from fp64 than torchvision's fp32 op (tests/test_dcn_gpu.py),
-# so those forwards run on fp32 cuBLAS and the tensor cores take grad_cols (K = Cout = 256 / 512).
+# Longest contraction given to the 3xTF32 GEMM, so the backbone's forwards (K = 2304 / 4608) run on fp32 cuBLAS and the
+# tensor cores take grad_cols (K = Cout = 256 / 512).  The limit once fenced off an accumulation error that grew with K
+# (6x / 20x torchvision's fp32 error at those forwards); the GEMM now holds fp32 cuBLAS's accuracy at any K
+# (tests/test_linear_tc_gpu.py), and whether those forwards are faster on the tensor cores has not been measured.
 TC_MAX_K = 1024
 
 
