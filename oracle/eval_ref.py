@@ -169,6 +169,45 @@ def compute_chamfer_distance_inner(pred_pcd, gt_pcd, pc_range):
     return float((fd.astype(np.float64).sum() / len(p) + bd.astype(np.float64).sum() / len(g)) / 2.0)
 
 
+def decode_clouds(depth, rays, points, tindex, origin_vox, origin, scale, within_grid=False, pc_range=None):
+    """ray_head.decode_clouds (the arg-max decode's clouds of every (sample, frame), eval_metrics.cu) in fp32
+    statements of the kernel's order: gt_dist = norm3(ray - origin_vox) * scale, a row joins cloud b * F + t when
+    its tindex t is a frame in [0, F), gt_dist > 0 and (within_grid) its metre point is inside pc_range; a cloud
+    holds its rows in their original order, both points o + ((p - o) / norm3(p - o)) * dist with dist = depth *
+    scale (pred) and gt_dist (gt); rows past the last cloud are NaN.  norm3(v) = sqrt((x*x + y*y) + z*z).
+    -> pred, gt [bs * M, 3], off [bs * F + 2] int64."""
+    depth, rays, points, tindex = (np.asarray(a, f32) for a in (depth, rays, points, tindex))
+    origin_vox, origin = np.asarray(origin_vox, f32), np.asarray(origin, f32)
+    scale = f32(scale)
+    bs, M = depth.shape
+    F = origin.shape[1]
+    pred = np.full((bs * M, 3), np.nan, f32)
+    gt = np.full((bs * M, 3), np.nan, f32)
+    off = np.zeros(bs * F + 2, np.int64)
+    n3 = lambda v: np.sqrt((v[..., 0] * v[..., 0] + v[..., 1] * v[..., 1]) + v[..., 2] * v[..., 2])
+    row = 0
+    for b in range(bs):
+        t = tindex[b]
+        with np.errstate(invalid="ignore"):
+            frame = (t >= 0) & (t < f32(F)) & (t == np.floor(t))
+        f = np.where(frame, t, 0).astype(np.int64)
+        gd = n3(rays[b] - origin_vox[b, f]) * scale
+        keep = frame & (gd > 0)
+        if within_grid:
+            keep &= get_inside_mask(points[b], pc_range)
+        for fr in range(F):
+            sel = np.nonzero(keep & (f == fr))[0]
+            o = origin[b, fr]
+            v = points[b, sel] - o
+            u = v / n3(v)[:, None]
+            pred[row:row + len(sel)] = o + u * (depth[b, sel] * scale)[:, None]
+            gt[row:row + len(sel)] = o + u * gd[sel][:, None]
+            row += len(sel)
+            off[b * F + fr + 1] = row
+    off[bs * F + 1] = bs * M
+    return pred, gt, off
+
+
 def frame_metrics(pred_pcds, gt_pcds, origin, pc_range, start_idx=0):
     """vidar.py:452-497's per-pair loop on the oracle functions."""
     origin = np.asarray(origin, f32)

@@ -39,6 +39,8 @@ def nn_backward(p1, p2, idx, grad_dists, len1=None, len2=None):
     g2 = np.zeros_like(p2, dtype=np.float64)
     for n in range(N):
         l1 = P1 if len1 is None else int(len1[n])
+        if len2 is not None and int(len2[n]) == 0:                # no candidate: no gradient
+            continue
         j = idx[n, :l1]
         diff = 2.0 * grad_dists[n, :l1, None] * (p1[n, :l1] - p2[n, j])
         g1[n, :l1] = diff
