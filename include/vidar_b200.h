@@ -633,29 +633,44 @@ int vidar_grid_mask_apply(const void* x, const void* offset, void* out, int dtyp
                           int l, int st_h, int st_w, int r, int use_h, int use_w, int mode, void* stream);
 
 /* ------------------------------------------------------------------------------------
- * (x) The multi-view image pipeline of the pre-training configs (datasets/pipelines/transform_3d.py
+ * (x) The multi-view image pipelines of the pre-training and fine-tuning configs (datasets/pipelines/transform_3d.py
  * PhotoMetricDistortionMultiViewImage, NormalizeMultiviewImage, PadMultiViewImage; augmentation.py
- * CropResizeFlipImage) from one frame's uint8 images, in two launches on `stream`, bit for bit the reference's
- * cv2 / PIL / numpy statements.
+ * CropResizeFlipImage, RandomCropResizeFlipImage) from one frame's uint8 images, bit for bit the reference's cv2 /
+ * PIL / numpy statements.
+ *
+ * vidar_image_aug_apply: photometric distortion with numpy's wrapping uint8 cast, crop / resize / window / flip,
+ * normalisation and padding, in two launches on `stream`.
  *   src      [N, H, W, 3] uint8 BGR (device), 1 <= N <= 64
- *   mid      [N, crop_h, out_w, 3] uint8 (device): the intermediate between the two passes, the only scratch
+ *   mid      [N, crop_h, mid_w, 3] uint8 (device): the intermediate between the two passes, the only scratch;
+ *            mid_w = min(win_x + win_w, out_w) - max(win_x, 0), the resized columns inside the window
  *   out      [N, 3, Hp, Wp] float32 (device), every element written
  *   photo_i  host int32 [N, 8] (brightness, contrast, saturation, hue gates, mode 1, perm[3]) and
  *   photo_f  host float [N, 4] (brightness delta, contrast factor, saturation factor, hue delta): one image's
  *            photometric draws each (both NULL: no photometric step); copied into the kernel arguments
  *   crop box (crop_x, crop_y, crop_x + crop_w, crop_y + crop_h) of the image, zero outside it; then Pillow's
- *   bicubic resize to (out_w, out_h) and, with flip, the left-right flip
- *   htaps    [out_w, 2 + hk] int32 (device): per output column (xmin, count, count weights in 2^-22, zero-padded
- *            to hk); given exactly when out_w != crop_w.  vtaps [out_h, 2 + vk] likewise for rows.
+ *   bicubic resize to (out_w, out_h); then the window (win_x, win_y, win_x + win_w, win_y + win_h) of the resized
+ *   image, zero outside it (CropResizeFlipImage: (0, 0, out_w, out_h); RandomCropResizeFlipImage crops the whole
+ *   image, and the window is its crop); with flip, the left-right flip of the window
+ *   htaps    [out_w, 2 + hk] int32 (device): per resized column (xmin, count, count weights in 2^-22, zero-padded
+ *            to hk); given exactly when out_w != crop_w.  vtaps [out_h, 2 + vk] likewise for rows.  Only the
+ *            entries of resized columns / rows inside the window are read.
  *   to_rgb swaps channels 0 and 2; then out = f32(double(x - mean[c]) * stdinv[c]) with mean host float[3] and
- *   stdinv host double[3]; pixels at y >= out_h or x >= out_w are pad_val[c] (host float[3]).
- * Needs every side in [1, 8192], out_h <= Hp, out_w <= Wp, gates 0 or 1, perm a permutation of (0, 1, 2).  No
- * host sync. */
+ *   stdinv host double[3]; pixels at y >= win_h or x >= win_w are pad_val[c] (host float[3]).
+ * Needs every side in [1, 8192], win_h <= Hp, win_w <= Wp, a window that overlaps the resized image, gates 0 or 1,
+ * perm a permutation of (0, 1, 2).  No host sync.
+ *
+ * vidar_image_aug_normalize: the chain without a crop step, in one launch on `stream` with no scratch: the
+ * photometric statements on float32 (no uint8 cast, unclamped) when photo_i / photo_f are given, then the same
+ * normalisation and padding to [N, 3, Hp, Wp] (pixels at y >= H or x >= W are pad_val[c]).  Needs 1 <= N <= 64,
+ * H <= Hp <= 8192, W <= Wp <= 8192.  No host sync. */
 int vidar_image_aug_apply(const unsigned char* src, unsigned char* mid, float* out, int N, int H, int W,
                           const int32_t* photo_i, const float* photo_f, int crop_x, int crop_y, int crop_w,
-                          int crop_h, int out_w, int out_h, const int32_t* htaps, int hk, const int32_t* vtaps, int vk,
-                          int flip, int to_rgb, const float* mean, const double* stdinv, const float* pad_val, int Hp,
-                          int Wp, void* stream);
+                          int crop_h, int out_w, int out_h, int win_x, int win_y, int win_w, int win_h,
+                          const int32_t* htaps, int hk, const int32_t* vtaps, int vk, int flip, int to_rgb,
+                          const float* mean, const double* stdinv, const float* pad_val, int Hp, int Wp, void* stream);
+int vidar_image_aug_normalize(const unsigned char* src, float* out, int N, int H, int W, const int32_t* photo_i,
+                              const float* photo_f, int to_rgb, const float* mean, const double* stdinv,
+                              const float* pad_val, int Hp, int Wp, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * (xi) The point half of a pre-training sample (datasets/pipelines/loading.py CustomLoadPointsFromMultiSweeps,

@@ -1,21 +1,30 @@
-"""The multi-view image pipeline of ViDAR's pre-training configs on the H100 (vidar_1_8_nusc_3future.py:279-317):
+"""The multi-view image pipelines of ViDAR's configs on the H100:
 
-    PhotoMetricDistortionMultiViewImage -> CropResizeFlipImage(ida_aug_conf) -> NormalizeMultiviewImage
-      -> PadMultiViewImage
+    pre-training (vidar_1_8_nusc_3future.py:279-317):
+        PhotoMetricDistortionMultiViewImage -> CropResizeFlipImage(ida_aug_conf) -> NormalizeMultiviewImage
+          -> PadMultiViewImage
+    memory-efficient pre-training (mem_efficient_vidar_1_8_nusc_3future.py:307-314):
+        PhotoMetricDistortionMultiViewImage -> RandomCropResizeFlipImage(ida_aug_conf) -> NormalizeMultiviewImage
+          -> PadMultiViewImage
+    fine-tuning (vidar_finetune/*, bevformer_base.py) and every test pipeline:
+        [PhotoMetricDistortionMultiViewImage ->] NormalizeMultiviewImage -> PadMultiViewImage
 
-The four classes take the reference's constructor arguments (datasets/pipelines/transform_3d.py:7-185,
-augmentation.py:10-202).  Used as dataloader transforms, their `__call__(results)` does only the host work: the
+The five classes take the reference's constructor arguments (datasets/pipelines/transform_3d.py:7-185,
+augmentation.py:10-301).  Used as dataloader transforms, their `__call__(results)` does only the host work: the
 same draws from the same generators in the same order (numpy's global generator for the photometric gates and
-factors and the flip, the stdlib `random` for the resize, cached in `results['aug_param']` so that the later
-frames of a queue reuse it), the `cam2img` / `lidar2img` / `img_norm_cfg` / shape keys as the reference sets them,
-and a record of what to do to the pixels in `results['img_aug']`.  `results['img']` is left as loaded (uint8).
+factors, the crop offset and the flip, the stdlib `random` for the resize, cached in `results['aug_param']` so
+that the later frames of a queue reuse it), the `cam2img` / `lidar2img` / `img_norm_cfg` / shape keys as the
+reference sets them, and a record of what to do to the pixels in `results['img_aug']`.  `results['img']` is left
+as loaded (uint8).
 
-`apply_multiview(img, results)` then runs the recorded chain on the device, on the current stream, in two launches
-(csrc/image_aug.cu, include/vidar_b200.h §x): uint8 [N, H, W, 3] BGR in, float32 [N, 3, Hp, Wp] out, bit for bit
-what the reference's cv2 / PIL / numpy statements give -- including numpy's wrapping `np.uint8` cast of pixels
-that brightness and contrast push past 255 or below 0.  The per-image draws travel in the kernel arguments; the
-resample taps are computed on the host in float64 by Pillow's rules, cached per (input size, output size, device)
-and uploaded once from pinned memory without blocking.  No host sync.  CUDA tensors only.
+`apply_multiview(img, results)` then runs the recorded chain on the device, on the current stream (csrc/image_aug.cu,
+include/vidar_b200.h §x): uint8 [N, H, W, 3] BGR in, float32 [N, 3, Hp, Wp] out, bit for bit what the reference's
+cv2 / PIL / numpy statements give.  With a crop step that is two launches, including numpy's wrapping `np.uint8`
+cast of pixels that brightness and contrast push past 255 or below 0; without one it is one launch, and the
+photometric output reaches the normalisation as unclamped float32, as in the reference.  The per-image draws
+travel in the kernel arguments; the resample taps are computed on the host in float64 by Pillow's rules, cached per
+(input size, output size, device) and uploaded once from pinned memory without blocking.  No host sync.  CUDA
+tensors only.
 """
 import random
 from dataclasses import dataclass, field
@@ -57,12 +66,15 @@ class ImageAugPlan:
     normalized: bool = False
     pad_hw: tuple = None
     pad_val: tuple = (0.0, 0.0, 0.0)
+    window: tuple = None               # (x0, y0, x1, y1) of the resized image, zero outside; None: all of it
 
     @property
     def hw(self):
         """(h, w) of the images after the steps recorded so far."""
         if self.pad_hw is not None:
             return self.pad_hw
+        if self.window is not None:
+            return self.window[3] - self.window[1], self.window[2] - self.window[0]
         return (self.dims[1], self.dims[0]) if self.dims is not None else tuple(self.src_hw)
 
 
@@ -177,6 +189,75 @@ class CropResizeFlipImage:
         return results
 
 
+class RandomCropResizeFlipImage:
+    """augmentation.py:204-301: one resize / crop / flip per frame -- the whole image resized first, then cropped to
+    the conf's crop size, zero outside the resized image.  Training draws the height (stdlib `random.choice`), the
+    crop's x offset (`np.random.uniform(0, max(0, newW - fW))`, a draw even when the range is empty), the bottom-
+    aligned crop's y offset (no draw) and the flip (`np.random.choice([0, 1])` when `rand_flip`); `training=False`
+    resizes to the one height and crops with the conf's box.  The result is cached in results['aug_param'] under
+    the key CropResizeFlipImage uses.  Updates `cam2img[:3, :3]` with [[r, 0, -crop_x], [0, r, -crop_y]] (the
+    translation not scaled, the flip left out, as in the reference) and sets `lidar2img = cam2img @ lidar2cam`."""
+
+    def __init__(self, data_aug_conf=None, training=True):
+        self.data_aug_conf = data_aug_conf
+        self.training = training
+
+    def _sample_augmentation(self, results):
+        if "CropResizeFlipImage_param" in results["aug_param"]:
+            return results["aug_param"]["CropResizeFlipImage_param"]
+        conf = self.data_aug_conf
+        H, W = conf["H"], conf["W"]
+        crop = conf["crop"]
+        fW, fH = int(crop[2] - crop[0]), int(crop[3] - crop[1])
+        resized_h = random.choice(conf["reisze"])
+        if self.training:
+            resized_w = resized_h / H * W
+            resize = resized_h / H
+            resize_dims = (int(resized_w), int(resized_h))
+            newW, newH = resize_dims
+            crop_h = int(max(0, newH - fH))
+            crop_w = int(np.random.uniform(0, max(0, newW - fW)))
+            crop = (crop_w, crop_h, crop_w + fW, crop_h + fH)
+            flip = False
+            if conf["rand_flip"] and np.random.choice([0, 1]):
+                flip = True
+        else:
+            if len(conf["reisze"]) != 1:
+                raise ValueError("RandomCropResizeFlipImage: training=False needs exactly one entry in 'reisze'")
+            resized_w = resized_h / (crop[3] - crop[1]) * (crop[2] - crop[0])
+            resize = resized_h / (crop[3] - crop[1])
+            resize_dims = (int(resized_w), int(resized_h))
+            flip = False
+        results["aug_param"]["CropResizeFlipImage_param"] = (resize, resize_dims, crop, flip)
+        return resize, resize_dims, crop, flip
+
+    def __call__(self, results):
+        plan = _plan(results, "crop")
+        if "aug_param" not in results:
+            results["aug_param"] = {}
+        resize, resize_dims, crop, flip = self._sample_augmentation(results)
+        x0, y0, x1, y1 = (int(round(v)) for v in crop)
+        w, h = (int(v) for v in resize_dims)
+        if not (0 < x1 - x0 <= MAX_SIDE and 0 < y1 - y0 <= MAX_SIDE and 0 < w <= MAX_SIDE and 0 < h <= MAX_SIDE
+                and -MAX_SIDE < x0 < w and -MAX_SIDE < y0 < h and x1 > 0 and y1 > 0):
+            raise ValueError(f"RandomCropResizeFlipImage: resize to {resize_dims} and crop {crop} need sides in "
+                             f"1..{MAX_SIDE} and a crop that overlaps the resized image")
+        ida_rot = np.eye(2)
+        ida_rot *= resize
+        ida_tran = np.zeros(2)
+        ida_tran -= np.array(crop[:2])
+        ida_mat = np.eye(3)
+        ida_mat[:2, :2] = ida_rot
+        ida_mat[:2, 2] = ida_tran
+        for i in range(plan.n):
+            results["cam2img"][i][:3, :3] = np.matmul(ida_mat, results["cam2img"][i][:3, :3])
+        results["lidar2img"] = [np.matmul(results["cam2img"][i], results["lidar2cam"][i])
+                                for i in range(len(results["lidar2cam"]))]
+        H, W = plan.src_hw
+        plan.crop, plan.dims, plan.window, plan.flip = (0, 0, W, H), (w, h), (x0, y0, x1, y1), bool(flip)
+        return results
+
+
 class NormalizeMultiviewImage:
     """transform_3d.py:61-95 (mmcv.imnormalize): optional BGR -> RGB, then (x - mean) / std per channel."""
 
@@ -287,9 +368,10 @@ def _check(img, plan, cams):
     be tested without a GPU."""
     if not isinstance(plan, ImageAugPlan):
         raise ValueError("apply_multiview: results has no recorded image steps (run the transforms first)")
-    if plan.photo is not None and plan.crop is None:
-        raise ValueError("apply_multiview: photometric distortion without CropResizeFlipImage is not supported (the "
-                         "uint8 cast of the distorted pixels happens there)")
+    if plan.photo is not None and plan.crop is None and not plan.normalized:
+        raise ValueError("apply_multiview: photometric distortion without CropResizeFlipImage or "
+                         "NormalizeMultiviewImage is not supported (the float32 pixels it makes are the output of "
+                         "neither)")
     if not isinstance(img, torch.Tensor):
         raise TypeError(f"apply_multiview: img must be a tensor (got {type(img).__name__})")
     if img.dtype != torch.uint8 or img.dim() != 4 or img.shape[-1] != 3:
@@ -306,6 +388,20 @@ def _check(img, plan, cams):
         raise RuntimeError("apply_multiview: img must be a CUDA tensor")
 
 
+def _photo_args(plan, cams):
+    """The draws of the images `cams` as the C entry points take them -> (int32 [n, 8], float32 [n, 4]), or Nones."""
+    if plan.photo is None:
+        return None, None
+    photo_i = np.zeros((len(cams), 8), np.int32)
+    photo_f = np.zeros((len(cams), 4), np.float32)
+    for k, c in enumerate(cams):
+        d = plan.photo[c]
+        photo_i[k] = (d.delta is not None, d.alpha is not None, d.sat is not None, d.hue is not None, d.mode == 1,
+                      *(d.perm or (0, 1, 2)))
+        photo_f[k] = [v if v is not None else 0.0 for v in (d.delta, d.alpha, d.sat, d.hue)]
+    return photo_i, photo_f
+
+
 def apply_multiview(img, results, cams=None):
     """Run the steps recorded in results['img_aug'] on img, uint8 [N, H, W, 3] BGR on a CUDA device -> float32
     [N, 3, Hp, Wp], on the current stream.  `cams`: which of the frame's images img holds (default all, in order),
@@ -314,38 +410,36 @@ def apply_multiview(img, results, cams=None):
     cams = list(range(plan.n)) if cams is None and isinstance(plan, ImageAugPlan) else list(cams or [])
     _check(img, plan, cams)
     n, H, W = img.shape[:3]
-    x0, y0, x1, y1 = plan.crop if plan.crop is not None else (0, 0, W, H)
-    ow, oh = plan.dims if plan.dims is not None else (W, H)
-    cw, ch = x1 - x0, y1 - y0
-    hp, wp = plan.pad_hw if plan.pad_hw is not None else (oh, ow)
-    photo_i = photo_f = None
-    if plan.photo is not None:
-        photo_i = np.zeros((n, 8), np.int32)
-        photo_f = np.zeros((n, 4), np.float32)
-        for k, c in enumerate(cams):
-            d = plan.photo[c]
-            photo_i[k] = (d.delta is not None, d.alpha is not None, d.sat is not None, d.hue is not None,
-                          d.mode == 1, *(d.perm or (0, 1, 2)))
-            photo_f[k] = [v if v is not None else 0.0 for v in (d.delta, d.alpha, d.sat, d.hue)]
+    photo_i, photo_f = _photo_args(plan, cams)
     mean = np.ascontiguousarray(plan.mean, np.float32)
     stdinv = 1 / plan.std.astype(np.float64)
     pad_val = np.asarray(plan.pad_val, np.float32)
+    hp, wp = plan.hw
     img = img.contiguous()
     dev = img.device
+
+    def host(a):
+        return None if a is None else a.ctypes.data
+
     with torch.cuda.device(dev):
+        out = torch.empty((n, 3, hp, wp), dtype=torch.float32, device=dev)
+        if plan.crop is None:
+            _lib.check(_lib.lib().vidar_image_aug_normalize(
+                _lib.ptr(img), _lib.ptr(out), n, H, W, host(photo_i), host(photo_f), int(plan.to_rgb), host(mean),
+                host(stdinv), host(pad_val), hp, wp, _lib.stream_ptr(dev)))
+            return out
+        x0, y0, x1, y1 = plan.crop
+        ow, oh = plan.dims
+        cw, ch = x1 - x0, y1 - y0
+        wx0, wy0, wx1, wy1 = plan.window if plan.window is not None else (0, 0, ow, oh)
         htaps = _taps(cw, ow, dev) if ow != cw else None
         vtaps = _taps(ch, oh, dev) if oh != ch else None
-        mid = torch.empty((n, ch, ow, 3), dtype=torch.uint8, device=dev)
-        out = torch.empty((n, 3, hp, wp), dtype=torch.float32, device=dev)
-
-        def host(a):
-            return None if a is None else a.ctypes.data
-
+        mid = torch.empty((n, ch, max(min(wx1, ow) - max(wx0, 0), 0), 3), dtype=torch.uint8, device=dev)
         _lib.check(_lib.lib().vidar_image_aug_apply(
             _lib.ptr(img), _lib.ptr(mid), _lib.ptr(out), n, H, W, host(photo_i), host(photo_f), x0, y0, cw, ch, ow,
-            oh, _lib.ptr(htaps), htaps.shape[1] - 2 if htaps is not None else 0, _lib.ptr(vtaps),
-            vtaps.shape[1] - 2 if vtaps is not None else 0, int(plan.flip), int(plan.to_rgb), host(mean),
-            host(stdinv), host(pad_val), hp, wp, _lib.stream_ptr(dev)))
+            oh, wx0, wy0, wx1 - wx0, wy1 - wy0, _lib.ptr(htaps), htaps.shape[1] - 2 if htaps is not None else 0,
+            _lib.ptr(vtaps), vtaps.shape[1] - 2 if vtaps is not None else 0, int(plan.flip), int(plan.to_rgb),
+            host(mean), host(stdinv), host(pad_val), hp, wp, _lib.stream_ptr(dev)))
     return out
 
 
