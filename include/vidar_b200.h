@@ -713,6 +713,20 @@ int vidar_point_pipeline_gather(const float* raw, const int64_t* seg_i, const do
 int vidar_jpeg_decode(const void* blob, int n, int nsub, long long blocks, long long samples, long long pixels,
                       unsigned char* out, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (xiii) The gradient bucket of the data-parallel step (vidar_b200/grad_bucket.py): n gradients in and out of one
+ * flat fp32 bucket, for ONE all-reduce of every trainable parameter's gradient.  The table is in HOST memory:
+ *   ptr_host    [n] device address of gradient i (fp32, contiguous, 4-byte aligned); pack: 0 = no gradient (packs
+ *               as zeros); unpack: must be non-zero where numel_host[i] > 0
+ *   numel_host  [n] its elements (0 allowed);  offset_host [n] its first element in the bucket (any value with
+ *               offset + numel <= bucket_numel)
+ *   scale_host  [n] pack only: bucket[offset_i + j] = grad_i[j] * scale_i, one fp32 multiply
+ * unpack writes grad_i[j] = bucket[offset_i + j].  One launch per 1024 tensors on `stream`, no scratch, no host sync. */
+int vidar_grad_bucket_pack(const int64_t* ptr_host, const int64_t* numel_host, const int64_t* offset_host,
+                           const float* scale_host, int n, float* bucket, long long bucket_numel, void* stream);
+int vidar_grad_bucket_unpack(const float* bucket, long long bucket_numel, const int64_t* ptr_host,
+                             const int64_t* numel_host, const int64_t* offset_host, int n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

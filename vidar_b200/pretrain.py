@@ -28,6 +28,9 @@ Sharding over a process group (one sample on all ranks -- the reference has repl
     the camera features, SCA projections) need their gradients summed -- ONE bucketed all-reduce per step
     (`sharding.allreduce_partial_grads`), the counterpart of the reference's DDP all-reduce
     (apis/mmdet_train.py:72-81).
+Data-parallel replicas of that (`build(..., grid=sharding.make_grid(S))`): world / S replicas, each sharding its own
+sample over S ranks; `train_step(..., grid=grid)` averages every trainable gradient over the replicas in ONE
+bucketed all-reduce over the world (`sharding.allreduce_grid_grads`).
 """
 import copy
 import math
@@ -120,7 +123,7 @@ class FPN(nn.Module):
 
 class _ShareCameraFeatures(torch.autograd.Function):
     """Features of a camera whose SCA units are split over two ranks: broadcast from the rank that ran the
-    backbone; the co-owner's gradient is reduced back (all-reduce inside the 2-rank group)."""
+    backbone (`src`: its global rank); the co-owner's gradient is reduced back (all-reduce inside the 2-rank group)."""
 
     @staticmethod
     def forward(ctx, feat, src, group):
@@ -363,7 +366,9 @@ class SyntheticViDAR(nn.Module):
         self.cam_owner = {c: r[0] for c, r in owners.items()}
         self.my_backbone_cams = [c for c, o in self.cam_owner.items() if o == rank]
         self.my_sca_cams = sca.plan_cameras(self.plan)
-        self.cam_groups = sca.camera_groups(world, self.num_cams, rank) if world > 1 else {}
+        self.cam_groups = sca.camera_groups(world, self.num_cams, rank, group) if world > 1 else {}
+        # the broadcast of a shared camera's features names its owner by global rank (`group` may be a sub-group)
+        self.cam_src = {c: dist.get_global_rank(group, o) for c, o in self.cam_owner.items()} if world > 1 else {}
         for layer in self.encoder:
             layer.cross_attn.set_process_group(group if world > 1 else None)
             if layer.latent_render is not None:
@@ -436,7 +441,7 @@ class SyntheticViDAR(nn.Module):
             if c in self.cam_groups:                                                      # shared camera
                 if f is None:
                     f = img.new_zeros((K, bs, EMBED)).requires_grad_(torch.is_grad_enabled())
-                f = _ShareCameraFeatures.apply(f, self.cam_owner[c], self.cam_groups[c])
+                f = _ShareCameraFeatures.apply(f, self.cam_src[c], self.cam_groups[c])
             pieces.append(f if (f is not None and (world == 1 or c in self.my_sca_cams)) else feats[c])
         feats = torch.stack(pieces, 0)
         spatial_shapes = torch.tensor(shapes, dtype=torch.int64, device=img.device)
@@ -692,21 +697,29 @@ def synthetic_point_infos(frames, n, seed=0, sweeps=2):
     return infos
 
 
-def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
+def train_step(model, optimizer, sample, group=None, record=False, scaler=None, grid=None):
     """forward_train + backward + gradient sync of the sharded parameters + clip(35) + AdamW step
     (config :379-388).  With a `torch.amp.GradScaler` (for a float16 `backbone_autocast`) the loss is scaled before
     the backward and the gradients unscaled before the clip; the scaler skips a step whose gradients are not finite.
-    -> (loss value tensor, [(stage, ms)] when `record`)."""
+    `grid` (`sharding.make_grid`, the model built with `build(..., grid=grid)`): `sample` is this replica's sample
+    and the sync is the grid's one bucketed all-reduce (`sharding.allreduce_grid_grads`): every rank ends with the
+    replica mean of the gradients.  -> (loss value tensor -- this replica's --, [(stage, ms)] when `record`)."""
+    if grid is not None and group is not None:
+        raise ValueError("train_step: pass group= or grid=, not both")
     model.timings = [] if record else None
     if record:
         model._mark("start")
     optimizer.zero_grad(set_to_none=True)
-    losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"], cam2img=sample.get("cam2img"),
-                                 lidar2cam=sample.get("lidar2cam"), point_infos=sample.get("point_infos"))
+    losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"], can_bus=sample.get("can_bus"),
+                                 cam2img=sample.get("cam2img"), lidar2cam=sample.get("lidar2cam"),
+                                 point_infos=sample.get("point_infos"))
     loss = sum(losses.values())
     (loss if scaler is None else scaler.scale(loss)).backward()
     model._mark("backward")
-    if group is not None:
+    if grid is not None:
+        sharding.allreduce_grid_grads(model, grid)
+        model._mark("grad_sync")
+    elif group is not None:
         sharding.allreduce_partial_grads(model, group)
         model._mark("grad_sync")
     if scaler is not None:
@@ -727,7 +740,24 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None):
     return loss.detach(), stages
 
 
-def build(device, group=None, lr=2e-4, seed=0, row_sharded=False, **model_kwargs):
+def build(device, group=None, lr=2e-4, seed=0, row_sharded=False, grid=None, **model_kwargs):
+    """-> (SyntheticViDAR in training mode with dropout off, AdamW).  `group`: one sample sharded over it.  `grid`
+    (`sharding.make_grid(S)`): data-parallel replicas of the sharded model -- the model shards over the grid's shard
+    group of S ranks, and `train_step(..., grid=grid)` averages the gradients over the world / S replicas.  Every rank
+    passes the same `seed` (the replicas start from the same parameters).
+
+    Each replica trains on its own sample, and the host draws of a step (GridMask, the image and the point pipeline:
+    numpy's global generator, and `random` for the image pipeline) must agree inside a shard group and differ across
+    replicas.  Seed per replica, for example with base the run's seed:
+        np.random.seed(base + grid.replica); random.seed(base + grid.replica)
+        sample = synthetic_sample(device, seed=base + grid.replica, ...)
+    The row-sharded encoder is not supported under a grid."""
+    if grid is not None:
+        if group is not None:
+            raise ValueError("build: pass group= or grid=, not both")
+        if row_sharded:
+            raise ValueError("build: the row-sharded encoder is not supported under a grid")
+        group = grid.group
     torch.manual_seed(seed)
     model = SyntheticViDAR(**model_kwargs).to(device)
     model.set_process_group(group, row_sharded=row_sharded)

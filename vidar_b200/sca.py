@@ -245,15 +245,21 @@ def camera_ranks(world, cams):
     return owners
 
 
-def camera_groups(world, cams, rank):
+def camera_groups(world, cams, rank, group=None):
     """Process groups of the cameras whose units are split over several ranks: the partial `grad_value`
     of such a camera is summed inside its group (its image features live on every rank of the group).
-    EVERY rank must call this (new_group is collective).  -> {camera: group} for this rank's shared cameras."""
+    EVERY rank must call this (new_group is collective).  `world` / `rank`: size of and rank in the shard group
+    `group` (None: the whole world).  The camera groups of every shard group are made on every rank, in one order,
+    from global ranks (`sharding.shard_layouts`).  -> {camera: group} for this rank's shared cameras."""
     import torch.distributed as dist
+
+    from .sharding import shard_layouts
+    layouts, mine = shard_layouts(group, world)
+    shared = [(c, members) for c, members in camera_ranks(world, cams).items() if len(members) > 1]
     groups = {}
-    for c, members in camera_ranks(world, cams).items():
-        if len(members) > 1:
-            g = dist.new_group(members)
-            if rank in members:
+    for ranks in layouts:
+        for c, members in shared:
+            g = dist.new_group([ranks[m] for m in members])
+            if ranks == mine and rank in members:
                 groups[c] = g
     return groups

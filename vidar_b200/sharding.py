@@ -31,18 +31,103 @@ def cameras_of(rank, world, cams, Q):
     return sorted({c for c, _, _ in shard_rows(rank, world, cams, Q)})
 
 
-def camera_groups(world, cams, Q, rank):
+def shard_layouts(group, world):
+    """Global ranks of the `world` ranks of every rank's shard group -> (every distinct layout, sorted; this rank's).
+    group None or WORLD: the one layout 0 .. world - 1.  Otherwise one all-gather over the world, so EVERY rank must
+    call this, each with its own shard group: sub-groups made from these layouts are then made by every rank in the
+    same order (new_group is collective over the whole world and takes global ranks)."""
+    if group is None or group is dist.group.WORLD:
+        mine = tuple(range(world))
+        return [mine], mine
+    mine = tuple(dist.get_global_rank(group, r) for r in range(world))
+    every = [None] * dist.get_world_size()
+    dist.all_gather_object(every, mine)
+    return sorted(set(every)), mine
+
+
+def camera_groups(world, cams, Q, rank, group=None):
     """Process groups for cameras whose rows are split over several ranks (their partial
     grad_value must be summed).  EVERY rank must call this (new_group is collective).
-    -> {cam: group} for the cameras this rank shares."""
+    `world` / `rank`: size of and rank in the shard group `group` (None: the whole world); every shard group's camera
+    groups are made on every rank, from global ranks.  -> {cam: group} for the cameras this rank shares."""
+    layouts, mine = shard_layouts(group, world)
     groups = {}
-    for c in range(cams):
-        members = [r for r in range(world) if c in cameras_of(r, world, cams, Q)]
-        if len(members) > 1:
-            g = dist.new_group(members)
-            if rank in members:
-                groups[c] = g
+    for ranks in layouts:
+        for c in range(cams):
+            members = [r for r in range(world) if c in cameras_of(r, world, cams, Q)]
+            if len(members) > 1:
+                g = dist.new_group([ranks[m] for m in members])
+                if ranks == mine and rank in members:
+                    groups[c] = g
     return groups
+
+
+# ------------------------------------------------------------------------------------------------
+# Data-parallel replicas of the sharded step: a (replica x shard) process grid.
+#
+# The world splits into R = world / S replicas of S contiguous ranks; each replica trains on its own sample and shards
+# it over its shard group exactly as a single-replica run shards over the world.  After backward a parameter's
+# gradient on a rank is either PARTIAL (tagged `vidar_partial_grad`: the shard group's sum is the replica's gradient)
+# or REPLICATED (every shard rank of the replica holds the whole, identical gradient).  One all-reduce (SUM) over the
+# world of the bucket
+#     partial:     grad * 1/R                        on every rank
+#     replicated:  grad * 1/R on shard rank 0,  * 0  on the other shard ranks
+# leaves on every rank the mean over replicas of the shard sums, and the mean over replicas of the replicated
+# gradients -- taken once per replica, so it never becomes (x + x + x) / 3 with its extra rounding.
+# ------------------------------------------------------------------------------------------------
+class Grid:
+    """This rank's place in the (replica x shard) grid (`make_grid`).
+      group        its shard group (S contiguous global ranks; the world itself when R == 1)
+      replica      replica index, 0 .. replicas - 1 (rank // S)
+      shard_rank   rank in the shard group (rank % S)
+      replicas, shard_size   R and S
+      world_group  the group of the gradient all-reduce (every rank)"""
+
+    def __init__(self, group, replica, shard_rank, replicas, shard_size, world_group):
+        self.group, self.replica, self.shard_rank = group, replica, shard_rank
+        self.replicas, self.shard_size, self.world_group = replicas, shard_size, world_group
+
+    def __repr__(self):
+        return (f"Grid({self.replicas} x {self.shard_size}: replica {self.replica}, shard rank {self.shard_rank})")
+
+
+def make_grid(shard_size):
+    """Split the world into world / shard_size replicas of `shard_size` contiguous ranks.  EVERY rank must call this
+    (each shard group is made by every rank, in the same order).  -> this rank's `Grid`."""
+    world, rank = dist.get_world_size(), dist.get_rank()
+    if not isinstance(shard_size, int) or shard_size < 1 or world % shard_size:
+        raise ValueError(f"shard_size must be a positive divisor of the world size {world}, got {shard_size!r}")
+    replicas = world // shard_size
+    if replicas == 1:
+        group = dist.group.WORLD
+    else:
+        group = None
+        for r in range(replicas):
+            g = dist.new_group(list(range(r * shard_size, (r + 1) * shard_size)))
+            if r == rank // shard_size:
+                group = g
+    return Grid(group, rank // shard_size, rank % shard_size, replicas, shard_size, dist.group.WORLD)
+
+
+def grid_grad_scales(params, grid):
+    """The bucket scale of every parameter (see the comment above `Grid`)."""
+    inv = 1.0 / grid.replicas
+    return [inv if getattr(p, "vidar_partial_grad", False) or grid.shard_rank == 0 else 0.0 for p in params]
+
+
+def allreduce_grid_grads(module, grid):
+    """Every trainable parameter's gradient -> the replica mean (partial ones: of the shard sums), identical on
+    every rank: pack into one fp32 bucket (`grad_bucket.pack`, gradients that are None pack as zeros), ONE all-reduce
+    over the world, unpack into `.grad` (allocated where None).  -> bucket elements."""
+    from . import grad_bucket
+    ps = [p for p in module.parameters() if p.requires_grad]
+    if not ps:
+        return 0
+    bucket = grad_bucket.pack(ps, grid_grad_scales(ps, grid))
+    if grid.replicas * grid.shard_size > 1:
+        dist.all_reduce(bucket, group=grid.world_group)
+    grad_bucket.unpack(bucket, ps)
+    return bucket.numel()
 
 
 def gather_rows(local_rows, world, total_rows, group=None):
