@@ -727,6 +727,28 @@ int vidar_grad_bucket_pack(const int64_t* ptr_host, const int64_t* numel_host, c
 int vidar_grad_bucket_unpack(const float* bucket, long long bucket_numel, const int64_t* ptr_host,
                              const int64_t* numel_host, const int64_t* offset_host, int n, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (xiv) The optimizer step of the pre-training configs (vidar_b200/optim.py): clip every gradient to a total 2-norm
+ * (torch.nn.utils.clip_grad_norm_) and step AdamW (torch.optim.AdamW's single-tensor update) over n parameters.  The
+ * table is in HOST memory:
+ *   param_host   [n] device address of parameter i (fp32, contiguous, 4-byte aligned; non-zero where numel > 0)
+ *   grad_host    [n] device address of its gradient, same layout; 0 = no gradient: parameter i is skipped (no decay,
+ *                no state change) and left out of the norm
+ *   numel_host   [n] elements of parameter i (0 allowed)
+ *   scalar_host  [n, 7] fp32 per parameter: 1 - lr*wd, -lr/bc1, 1/sqrt(bc2) (from its own step count), and
+ *                1 - beta1, beta2, 1 - beta2, eps
+ *   exp_avg, exp_avg_sq  flat fp32 state [state_numel] in table order: parameter i owns the numel_host[i] elements
+ *                after those of parameters 0 .. i-1 (sum of numel_host <= state_numel)
+ *   clip         non-zero: every gradient is multiplied by clamp(max_norm / (norm + 1e-6), max=1) first, norm being
+ *                the 2-norm of every gradient (summed in fp64, in a fixed order), which is stored to grad_norm
+ *                (device fp32 scalar); 0: no clipping, max_norm and grad_norm unused
+ * Launches: one norm kernel (clip only) and one update kernel per run of at most 896 parameters that share beta1,
+ * beta2 and eps -- two for the pre-training model.  Bitwise deterministic; no host sync; the norm partials come from
+ * the library's stream-ordered pool. */
+int vidar_adamw_step(const int64_t* param_host, const int64_t* grad_host, const int64_t* numel_host,
+                     const float* scalar_host, int n, float* exp_avg, float* exp_avg_sq, long long state_numel,
+                     int clip, float max_norm, float* grad_norm, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -129,3 +129,17 @@ def count_syncs(fn, *args):
     torch.cuda.synchronize()
     syncs = [w for w in rec if "called a synchronizing CUDA operation" in str(w.message)]
     return len(syncs), sorted({f"{os.path.relpath(w.filename, ROOT)}:{w.lineno}" for w in syncs})
+
+
+def cuda_kernels(fn, *args):
+    """(GPU kernels fn(*args) launches, every library's, and the sum of their durations in ms) from torch.profiler's
+    CUDA activity, memcpy and memset records excluded.  The sum is device time spent in kernels, without the gaps
+    between them."""
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn(*args)
+        torch.cuda.synchronize()
+    kernels = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+               and not e.name.lower().startswith(("memcpy", "memset"))]
+    return len(kernels), sum(e.time_range.elapsed_us() for e in kernels) / 1e3

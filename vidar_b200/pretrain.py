@@ -41,7 +41,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import bev_geometry, sca, sharding, synthetic
+from . import bev_geometry, optim, sca, sharding, synthetic
 from . import modules as _modules  # noqa: F401  (registers the attention classes)
 from . import image_aug
 from . import point_pipeline as point_aug
@@ -699,7 +699,7 @@ def synthetic_point_infos(frames, n, seed=0, sweeps=2):
 
 def train_step(model, optimizer, sample, group=None, record=False, scaler=None, grid=None):
     """forward_train + backward + gradient sync of the sharded parameters + clip(35) + AdamW step
-    (config :379-388).  With a `torch.amp.GradScaler` (for a float16 `backbone_autocast`) the loss is scaled before
+    (config :379-388); with an `optim.AdamW` (`config_optimizer`) the clip is the one inside its step.  With a `torch.amp.GradScaler` (for a float16 `backbone_autocast`) the loss is scaled before
     the backward and the gradients unscaled before the clip; the scaler skips a step whose gradients are not finite.
     `grid` (`sharding.make_grid`, the model built with `build(..., grid=grid)`): `sample` is this replica's sample
     and the sync is the grid's one bucketed all-reduce (`sharding.allreduce_grid_grads`): every rank ends with the
@@ -724,7 +724,8 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None, 
         model._mark("grad_sync")
     if scaler is not None:
         scaler.unscale_(optimizer)
-    torch.nn.utils.clip_grad_norm_([p for p in model.parameters() if p.requires_grad], 35.0)
+    if not isinstance(optimizer, optim.AdamW):            # optim.AdamW clips inside its step
+        torch.nn.utils.clip_grad_norm_([p for p in model.parameters() if p.requires_grad], 35.0)
     if scaler is None:
         optimizer.step()
     else:
@@ -767,3 +768,12 @@ def build(device, group=None, lr=2e-4, seed=0, row_sharded=False, grid=None, **m
             m.p = 0.0
     opt = torch.optim.AdamW([p for p in model.parameters() if p.requires_grad], lr=lr, weight_decay=0.01)
     return model, opt
+
+
+def config_optimizer(model, lr=2e-4):
+    """The configs' optimizer (vidar_1_8_nusc_3future.py:379-388, built by mmcv's DefaultOptimizerConstructor and
+    OptimizerHook): AdamW, weight decay 0.01, one group per parameter with the backbone at lr_mult 0.1 (the config's
+    `img_backbone` is this model's `backbone`), the gradients clipped to a total 2-norm of 35 -- as one
+    `optim.AdamW` step.  `build()` keeps torch's single-group AdamW; pass this to `train_step` instead."""
+    return optim.AdamW(optim.paramwise_groups(model, lr, 0.01, {"backbone": dict(lr_mult=0.1)}), lr=lr,
+                       weight_decay=0.01, max_grad_norm=35)

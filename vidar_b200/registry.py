@@ -130,16 +130,20 @@ def register_into_mmcv():
     """If mmcv is installed, expose this package's modules under the reference's names in
     mmcv's own ATTENTION registry (force=True replaces the plugin's classes), and its
     deformable convolution as `DCNv2` in mmcv's CONV_LAYERS (what mmdet's ResNet builds for
-    `dcn=dict(type='DCNv2', ...)`)."""
+    `dcn=dict(type='DCNv2', ...)`), and its optimizer as `VidarAdamW` in mmcv's OPTIMIZERS (what `build_optimizer`
+    builds for `optimizer=dict(type='VidarAdamW', ...)`)."""
     try:
         from mmcv.cnn.bricks.registry import ATTENTION as MMCV_ATTENTION
         from mmcv.cnn.bricks.registry import CONV_LAYERS as MMCV_CONV_LAYERS
+        from mmcv.runner.optimizer import OPTIMIZERS as MMCV_OPTIMIZERS
     except Exception:
         return False
     from . import dcn  # noqa: F401  (registers DCNv2)
+    from .optim import AdamW
     for name, cls in ATTENTION.module_dict.items():
         MMCV_ATTENTION.register_module(name=name, force=True, module=cls)
     for name, cls in CONV_LAYERS.module_dict.items():
         if cls.__module__.startswith(__package__ + "."):           # this package's ops only, not torch's Conv2d
             MMCV_CONV_LAYERS.register_module(name=name, force=True, module=cls)
+    MMCV_OPTIMIZERS.register_module(name="VidarAdamW", force=True, module=AdamW)
     return True
