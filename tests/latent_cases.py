@@ -30,3 +30,17 @@ def case(seed=0, bs=2, bev=BEV, embed_dims=64):
     g = torch.Generator().manual_seed(seed)
     return dict(embed=torch.randn(bs, bev[0], bev[1], embed_dims, generator=g),
                 grad=torch.randn(bs, bev[0], bev[1], embed_dims, generator=g))
+
+
+def proj_inputs(rows, E, D, A=16, seed=0, device="cpu"):
+    """fp32 operands of the four projection kernels with non-zero means and gradients of mixed scale
+    (each gradient column scaled by 10^[-3, 1)), so that a relative-to-max tolerance would hide errors
+    on small columns and only elementwise bounds can judge them."""
+    g = torch.Generator().manual_seed(seed)
+    rnd = lambda *s: torch.randn(*s, generator=g)
+    scale = lambda n: 10.0 ** (torch.rand(n, generator=g) * 4 - 3)
+    t = dict(x=2 + rnd(rows, E), w_occ=rnd(D, E) / 16, b_occ=rnd(D), w_feat=rnd(A, E) / 16, b_feat=rnd(A),
+             w_b=rnd(E, A) / 4 + 0.1, b_b=rnd(E), pooled=1 + rnd(rows, A), prob=torch.rand(rows, D, generator=g),
+             g_occ=(0.5 + rnd(rows, D)) * scale(D), g_feat=(0.5 + rnd(rows, A)) * scale(A),
+             g_out=(0.5 + rnd(rows, E)) * scale(E))
+    return {k: v.to(device) for k, v in t.items()}

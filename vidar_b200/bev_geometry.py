@@ -35,18 +35,32 @@ def get_reference_points(H, W, Z=8, num_points_in_pillar=4, dim="3d", bs=1, devi
 
 def point_sampling(reference_points, pc_range, img_metas):
     """reference_points [bs, D, Q, 3] in [0,1]; img_metas: list (len bs) of dicts with 'lidar2img'
-    (num_cam 4x4) and 'img_shape' -> (reference_points_cam [cams,bs,Q,D,2], bev_mask [cams,bs,Q,D] bool)."""
+    (num_cam 4x4) and 'img_shape' -> (reference_points_cam [cams,bs,Q,D,2], bev_mask [cams,bs,Q,D] bool).
+    The kernel reads one lidar2img per sample and six range values, so their shapes are checked first."""
+    if reference_points.dim() != 4 or reference_points.shape[-1] != 3:
+        raise RuntimeError(f"reference_points must be [bs, D, num_query, 3], got {tuple(reference_points.shape)}")
+    bs = reference_points.shape[0]
+    if len(img_metas) != bs:
+        raise RuntimeError(f"point_sampling: {len(img_metas)} img_metas for {bs} samples of reference_points")
+    mats = [np.asarray(m["lidar2img"], dtype=np.float64) for m in img_metas]
+    for b, l2i_b in enumerate(mats):
+        if l2i_b.ndim != 3 or l2i_b.shape[1:] != (4, 4) or l2i_b.shape[0] < 1:
+            raise RuntimeError(f"point_sampling: lidar2img of sample {b} must be [num_cams, 4, 4], got {l2i_b.shape}")
+        if l2i_b.shape[0] != mats[0].shape[0]:
+            raise RuntimeError(f"point_sampling: sample {b} has {l2i_b.shape[0]} cameras, sample 0 has {mats[0].shape[0]}")
+    rng_vals = np.asarray(pc_range, dtype=np.float64).reshape(-1)
+    if rng_vals.size != 6 or not np.isfinite(rng_vals).all():
+        raise RuntimeError(f"point_sampling: pc_range must be 6 finite numbers, got {list(rng_vals)}")
     _lib.require_cuda(reference_points=reference_points.contiguous())
     ref = reference_points.float().contiguous()
-    lidar2img = np.asarray([m["lidar2img"] for m in img_metas])
-    l2i = ref.new_tensor(lidar2img).float().contiguous()                        # [bs, cams, 4, 4]
-    bs, D, Q, _ = ref.shape
+    l2i = ref.new_tensor(np.stack(mats)).float().contiguous()                   # [bs, cams, 4, 4]
+    _, D, Q, _ = ref.shape
     cams = l2i.shape[1]
     img_h, img_w = img_metas[0]["img_shape"][0][0], img_metas[0]["img_shape"][0][1]
     ref_cam = torch.empty((cams, bs, Q, D, 2), dtype=torch.float32, device=ref.device)
     mask = torch.empty((cams, bs, Q, D), dtype=torch.uint8, device=ref.device)
     import ctypes as C
-    rng = (C.c_float * 6)(*[float(v) for v in pc_range])
+    rng = (C.c_float * 6)(*[float(v) for v in rng_vals])
     with torch.cuda.device(ref.device):
         _lib.check(_lib.lib().vidar_point_sampling(
             _lib.ptr(ref), _lib.ptr(l2i), C.cast(rng, C.c_void_p), _lib.ptr(ref_cam), _lib.ptr(mask),

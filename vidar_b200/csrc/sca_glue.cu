@@ -34,7 +34,8 @@ point_sampling_kernel(PsDims P, const float* __restrict__ ref3d, const float* __
   const float y = __fadd_rn(__fmul_rn(r[1], P.rs[1]), P.r0[1]);
   const float z = __fadd_rn(__fmul_rn(r[2], P.rs[2]), P.r0[2]);
   const float* m = l2i + ((size_t)b * P.cams + cam) * 16;
-  // row . (x, y, z, 1): fp32 FMA chain like cuBLAS' dot product
+  // row . (x, y, z, 1): one fp32 FMA chain.  The reference's batched matmul sums in another order, so
+  // only ~20% of coordinates are bit-identical to it; masks differ only within rounding of a border.
   const float px = fmaf(m[0], x, fmaf(m[1], y, fmaf(m[2], z, m[3])));
   const float py = fmaf(m[4], x, fmaf(m[5], y, fmaf(m[6], z, m[7])));
   const float pz = fmaf(m[8], x, fmaf(m[9], y, fmaf(m[10], z, m[11])));
