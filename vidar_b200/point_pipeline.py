@@ -215,14 +215,15 @@ class CustomVoxelBasedPointSampler:
         return results
 
 
-def config_train_pipeline(point_cloud_range=(-51.2, -51.2, -5.0, 51.2, 51.2, 3.0)):
-    """The point transforms of the pre-training config's train_pipeline (vidar_1_8_nusc_3future.py:279-305)."""
+def config_train_pipeline(point_cloud_range=(-51.2, -51.2, -5.0, 51.2, 51.2, 3.0), voxel_size=(1.0, 1.0, 1.0)):
+    """The point transforms of the pre-training config's train_pipeline (vidar_1_8_nusc_3future.py:279-305).
+    `voxel_size`: the voxel sampler's, 0.5 m in the 1-future configs (vidar_full_nusc_1future.py:291-295)."""
     return [LoadPointsFromFile(coord_type="LIDAR", load_dim=5, use_dim=5),
             CustomLoadPointsFromMultiSweeps(sweeps_num=2, use_dim=[0, 1, 2, 3, 4], pad_empty_sweeps=True,
                                             remove_close=True, ego_mask=(-0.8, -1.5, 0.8, 2.5),
                                             hard_sweeps_timestamp=0, random_select=False),
             CustomVoxelBasedPointSampler(cur_sweep_cfg=dict(max_num_points=1, point_cloud_range=list(point_cloud_range),
-                                                            voxel_size=[1.0, 1.0, 1.0], max_voxels=50000),
+                                                            voxel_size=list(voxel_size), max_voxels=50000),
                                          time_dim=4)]
 
 

@@ -14,7 +14,9 @@ This is a HARNESS, not a port of the detector: it composes the reference's step
     (modules/vidar_decoder.py:25-280, dense_heads/vidar_head_base.py:125-173);
   * the per-layer freespace head and the ray losses of ViDARHeadV1 (dense_heads/vidar_head_v1.py:45-92,
     150-219) through `vidar_b200.head.ViDARRayHead.loss`.
-History frames run under no_grad like `obtain_history_bev` (bevformer.py:158-189).
+History frames run under no_grad like `obtain_history_bev` (bevformer.py:158-236); `CONFIGS` holds the training
+regimes of the four nuScenes pre-training configs (the last history frame's encoder with gradient, a random drop
+of the history, one sampled supervised future frame, the head's frames), for `build(device, config=name)`.
 
 Sharding over a process group (one sample on all ranks -- the reference has replica DDP only):
   * cameras: each camera's image goes through backbone + FPN on ONE rank; a camera whose
@@ -171,7 +173,7 @@ class LearnedPositionalEncoding(nn.Module):
 class EncoderLayer(nn.Module):
     """BEVFormerLayerV2 (encoder_v2.py:52-209): self_attn, norm, cross_attn, norm, [latent_render], ffn, norm."""
 
-    def __init__(self, latent_render, bev_hw):
+    def __init__(self, latent_render, bev_hw, grid_step=0.5):
         super().__init__()
         self.bev_hw = bev_hw
         self.self_attn = build_attention(dict(type="TemporalSelfAttention", embed_dims=EMBED, num_levels=1))
@@ -181,8 +183,8 @@ class EncoderLayer(nn.Module):
         self.norms = nn.ModuleList([nn.LayerNorm(EMBED) for _ in range(3)])
         self.ffn = FFN()
         self.latent_render = build_attention(dict(
-            type="LatentRendering", embed_dims=EMBED, num_pred_fcs=0, pred_height=HEIGHTS, grid_num=256, grid_step=0.5,
-            reduction=16, act="sigmoid")) if latent_render else None
+            type="LatentRendering", embed_dims=EMBED, num_pred_fcs=0, pred_height=HEIGHTS, grid_num=256,
+            grid_step=grid_step, reduction=16, act="sigmoid")) if latent_render else None
 
     def forward(self, query, feats, bev_pos, ref_2d, prev_bev, shapes, lsi, ref_cam, bev_mask, bev_shapes, bev_lsi):
         query = self.self_attn(query, prev_bev, prev_bev, None, query_pos=bev_pos, reference_points=ref_2d,
@@ -311,14 +313,58 @@ class SyntheticViDAR(nn.Module):
     frame, then the future ones; `synthetic_sample(..., raw_points=True)`), and ignore their gt_points argument.
     Training runs the train pipeline's point transforms (vidar_1_8_nusc_3future.py:279-305) on every GT frame first,
     in queue order, the test path LoadPointsFromFile only (:319-324); then `gather_gt_points` with the dataset's
-    ego mask makes the padded [1, R, 5] gt_points with no host sync.  The default False leaves the graph as it was."""
+    ego mask makes the padded [1, R, 5] gt_points with no host sync.  The default False leaves the graph as it was.
+
+    Training regime (the options that tell the nuScenes pre-training configs apart; `CONFIGS` holds each config's
+    values, and the defaults are the graph above):
+      * `backward_history_frames` (0 or 1, the configs' backwarded_prev_frame_num): the last history frame's encoder
+        runs with gradient in training, its backbone and FPN under no_grad (bevformer.py:191-215);
+      * `drop_prev_rate` / `drop_prev_end_idx` (random_drop_prev_*, vidar.py:268-281; the start index is 1): with
+        probability `drop_prev_rate` a drop index k = randint(1, end) cuts the frozen history chain -- frame i < k's BEV
+        is discarded (bevformer.py:184-185), so those frames are not computed at all;
+      * `supervise_all_future=False`: one future frame, drawn by np.random.choice, is supervised; the other roll-outs
+        run under no_grad (vidar.py:333-357);
+      * `head_history_frames` / `head_future_frames` / `per_frame_loss_weight`: the head's predicted frames per BEV
+        feature (ViDARHeadV1's pred_history_frame_num / pred_future_frame_num / per_frame_loss_weight); the
+        defaults are `history_frames`, 1 and (0.1, 0.1, 0.1, 1.0, 1.0);
+      * `frame_loss_weight` (the head's loss_weight, e.g. ((1,), (0,))): when given, the loss weighs frames as
+        ViDARHeadV1.loss does -- the current head frame by these weights, every other head frame on the current
+        frame only, each head frame's losses times its `per_frame_loss_weight`.  None keeps the harness's weighting;
+      * `latent_grid_step`: LatentRendering's grid_step;
+      * `future_frames=0`: no decoder is built (the reference deletes it, vidar.py:109-115); the head keeps
+        max(decoder_layers, 1) prediction layers and supervises the current frame;
+      * `point_voxel_size`: the point pipeline's voxel sampler size in metres;
+      * `reference_draws`: forward_train draws from numpy's global generator as the reference's does, before any
+        other draw of the step: A1's rand() (random_drop_image_rate is 0 in every config, so it only consumes the
+        draw), A2's rand() and randint, then the supervised future frame.  None (the default) draws only when a
+        drop rate or `supervise_all_future=False` needs it.  Under a process group every rank of a shard group must
+        seed numpy alike (as for GridMask) so that they draw the same drop index and future frame."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
                  latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None,
-                 grid_mask=False, image_pipeline=False, point_pipeline=False):
+                 grid_mask=False, image_pipeline=False, point_pipeline=False, backward_history_frames=0,
+                 drop_prev_rate=0.0, drop_prev_end_idx=None, supervise_all_future=True, head_history_frames=None,
+                 head_future_frames=1, per_frame_loss_weight=None, frame_loss_weight=None, latent_grid_step=0.5,
+                 point_voxel_size=1.0, reference_draws=None):
         super().__init__()
-        self.point_transforms = ((point_aug.config_train_pipeline(PC_RANGE), point_aug.config_test_pipeline())
-                                 if point_pipeline else None)
+        if backward_history_frames not in (0, 1):
+            raise ValueError(f"backward_history_frames must be 0 or 1 (got {backward_history_frames})")
+        if future_frames < 0 or decoder_layers < 0 or (future_frames > 0 and decoder_layers == 0):
+            raise ValueError(f"future_frames={future_frames} needs decoder_layers >= 1 (got {decoder_layers})")
+        if not 0.0 <= drop_prev_rate <= 1.0:
+            raise ValueError(f"drop_prev_rate must lie in [0, 1] (got {drop_prev_rate})")
+        self.backward_history_frames = backward_history_frames
+        self.drop_prev_rate, self.drop_prev_start_idx, self.drop_prev_end_idx = drop_prev_rate, 1, drop_prev_end_idx
+        self.supervise_all_future = supervise_all_future
+        self.reference_draws = (bool(reference_draws) if reference_draws is not None
+                                else drop_prev_rate > 0 or not supervise_all_future)
+        if not self.reference_draws and (drop_prev_rate > 0 or not supervise_all_future):
+            raise ValueError("drop_prev_rate > 0 and supervise_all_future=False draw from numpy: reference_draws=False "
+                             "cannot hold them")
+        self.head_history_frames = history_frames if head_history_frames is None else head_history_frames
+        self.head_future_frames = head_future_frames
+        self.point_transforms = ((point_aug.config_train_pipeline(PC_RANGE, (point_voxel_size,) * 3),
+                                  point_aug.config_test_pipeline()) if point_pipeline else None)
         self.image_transforms = image_aug.config_pipeline() if image_pipeline else None
         if backbone_autocast not in (None, torch.float16, torch.bfloat16):
             raise ValueError(f"backbone_autocast must be None, torch.float16 or torch.bfloat16 (got {backbone_autocast})")
@@ -334,19 +380,35 @@ class SyntheticViDAR(nn.Module):
         self.level_embeds = nn.Parameter(torch.randn(4, EMBED) * 0.02)
         self.can_bus_mlp = nn.Sequential(nn.Linear(18, EMBED // 2), nn.ReLU(inplace=True), nn.Linear(EMBED // 2, EMBED),
                                          nn.ReLU(inplace=True), nn.LayerNorm(EMBED))
-        self.encoder = nn.ModuleList([EncoderLayer(i == latent_layer, bev_hw) for i in range(encoder_layers)])
-        # future head (ViDARHeadV1)
-        self.future_bev_embedding = nn.Embedding(BEV_H * BEV_W, EMBED)
-        self.future_positional_encoding = LearnedPositionalEncoding(BEV_H, BEV_W)
-        self.prev_frame_embedding = nn.Parameter(torch.randn(1, EMBED))
-        self.future_can_bus_mlp = nn.Sequential(nn.Linear(18, EMBED // 2), nn.ReLU(inplace=True),
-                                                nn.Linear(EMBED // 2, EMBED), nn.ReLU(inplace=True), nn.LayerNorm(EMBED))
-        self.decoder = nn.ModuleList([DecoderLayer() for _ in range(decoder_layers)])
-        self.pred_frame_num = 1 + history_frames + 1                 # 3 history + current + 1 future per BEV feature (cfg :31-33)
-        self.bev_pred_head = nn.ModuleList([nn.Linear(EMBED, self.pred_frame_num * HEIGHTS) for _ in range(decoder_layers)])
+        self.encoder = nn.ModuleList([EncoderLayer(i == latent_layer, bev_hw, latent_grid_step)
+                                      for i in range(encoder_layers)])
+        # future head (ViDARHeadV1); with no future frame the reference deletes the decoder and its embeddings
+        self.future_bev_embedding = self.future_positional_encoding = None
+        self.prev_frame_embedding = self.future_can_bus_mlp = None
+        if future_frames > 0:
+            self.future_bev_embedding = nn.Embedding(BEV_H * BEV_W, EMBED)
+            self.future_positional_encoding = LearnedPositionalEncoding(BEV_H, BEV_W)
+            self.prev_frame_embedding = nn.Parameter(torch.randn(1, EMBED))
+            self.future_can_bus_mlp = nn.Sequential(nn.Linear(18, EMBED // 2), nn.ReLU(inplace=True),
+                                                    nn.Linear(EMBED // 2, EMBED), nn.ReLU(inplace=True),
+                                                    nn.LayerNorm(EMBED))
+        self.decoder = nn.ModuleList([DecoderLayer() for _ in range(decoder_layers if future_frames > 0 else 0)])
+        # head frames per BEV feature: 3 history + current + 1 future by default (cfg :31-33)
+        self.pred_frame_num = 1 + self.head_history_frames + head_future_frames
+        self.bev_pred_head = nn.ModuleList([nn.Linear(EMBED, self.pred_frame_num * HEIGHTS)
+                                            for _ in range(max(decoder_layers, 1))])
+        self.frame_loss_weight = None if frame_loss_weight is None else np.array(frame_loss_weight, np.float64)
+        if self.frame_loss_weight is not None and self.frame_loss_weight.shape != (future_frames + 2, 1):
+            raise ValueError(f"frame_loss_weight: one [w] per frame 0 .. future_frames and a last ignored one "
+                             f"({future_frames + 2} rows), got {frame_loss_weight}")
         self.ray_head = ViDARRayHead(ray_grid_num=ray_grid_num, ray_grid_step=1.0, use_ce_loss=True, use_dist_loss=False,
                                      use_dense_loss=True, loss_weight=[[1.0]] * (1 + future_frames))
-        self.per_frame_loss_weight = (0.1, 0.1, 0.1, 1.0, 1.0)
+        if per_frame_loss_weight is None:
+            self.per_frame_loss_weight = (0.1, 0.1, 0.1, 1.0, 1.0)
+        else:
+            self.per_frame_loss_weight = tuple(float(w) for w in per_frame_loss_weight)
+            if len(self.per_frame_loss_weight) != self.pred_frame_num:
+                raise ValueError(f"per_frame_loss_weight: {self.pred_frame_num} head frames, got {per_frame_loss_weight}")
         self.process_group = None
         self.row_sharded = False
         self.timings = None
@@ -482,6 +544,8 @@ class SyntheticViDAR(nn.Module):
 
     # ---- future decoder (vidar_head_base.py:125-173) ----
     def decode_future(self, prev_bev_input, future_can_bus):
+        if not len(self.decoder):
+            raise RuntimeError("decode_future: the model was built with future_frames=0 and has no future decoder")
         bs = prev_bev_input.shape[0]
         dev = prev_bev_input.device
         BEV_H, BEV_W = self.bev_h, self.bev_w          # noqa: N806
@@ -499,7 +563,7 @@ class SyntheticViDAR(nn.Module):
 
     def forward_head(self, next_bev_feats):
         """vidar_head_v1.py:64-92: [frames, inter, bs, Q, C] -> [frames, inter, pred_frame, bs, Q, heights]."""
-        hist = self.history_frames
+        hist = self.head_history_frames
         preds = []
         for lvl in range(next_bev_feats.shape[1]):
             p = self.bev_pred_head[lvl](next_bev_feats[:, lvl])
@@ -530,11 +594,19 @@ class SyntheticViDAR(nn.Module):
             frames.append(results)
         return frames
 
-    def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None):
-        """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + future_frames, inter, pred_frame, bs, Q, 16]: the history
-        BEV of the first T - 1 frames (no grad), the current frame's BEV as ref_bev, `future_frames` roll-outs with a
-        queue of length 1, then the head.  With the image pipeline, img is uint8 [1, T, cams, H, W, 3] and the
-        camera matrices come from cam2img / lidar2cam."""
+    def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None, train=False,
+                        drop_prev_index=-1, supervised=None):
+        """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + len(supervised), inter, pred_frame, bs, Q, 16]: the
+        history BEV of the first T - 1 frames, the current frame's BEV as ref_bev, `future_frames` roll-outs with a
+        queue of length 1 -- those not in `supervised` (default: all) under no_grad --, then the head over the current
+        and the supervised frames.  With the image pipeline, img is uint8 [1, T, cams, H, W, 3] and the camera
+        matrices come from cam2img / lidar2cam.
+
+        The history as `obtain_history_bev` (bevformer.py:158-236): with `train`, the last
+        `backward_history_frames` frames are backwarded -- backbone under no_grad, encoder with gradient --, the
+        others frozen under no_grad; frozen frame i < `drop_prev_index` is not computed, as its BEV would be
+        discarded.  Each of the two parts makes its eval-mode GridMask draw (one prob gate per extract_feat call of
+        the reference), also when the drop skips every frozen frame."""
         bs, T = img.shape[:2]
         dev = img.device
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
@@ -548,15 +620,25 @@ class SyntheticViDAR(nn.Module):
             metas = [[dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)])
                       for b in range(bs)]] * T
             hw = img.shape[-2:]
+        backwarded = min(self.backward_history_frames, T - 1) if train else 0
+        frozen = T - 1 - backwarded
         prev_bev = None
-        if self.grid_mask is not None and T > 1:                                     # the history's eval-mode call
+        if self.grid_mask is not None and frozen > 0:                                # the history's eval-mode call
             self.grid_mask.sample(*hw, training=False)
-        with torch.no_grad():                                                        # obtain_history_bev
-            for t in range(T - 1):
+        with torch.no_grad():                                                        # _obtain_frozen_history_bev
+            for t in range(min(max(drop_prev_index, 0), frozen), frozen):
                 feats, shapes, lsi = self.extract_feat(inputs[t])
                 self._mark(f"hist{t}.backbone")
                 prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
                 self._mark(f"hist{t}.encoder")
+        if backwarded and self.grid_mask is not None:                                # _obtain_backwarded_history_bev
+            self.grid_mask.sample(*hw, training=False)
+        for t in range(frozen, T - 1):
+            with torch.no_grad():
+                feats, shapes, lsi = self.extract_feat(inputs[t])
+            self._mark(f"hist{t}.backbone")
+            prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
+            self._mark(f"hist{t}.encoder")
         draw = self.grid_mask.sample(*hw) if self.grid_mask is not None else None
         feats, shapes, lsi = self.extract_feat(inputs[T - 1], draw)
         self._mark("cur.backbone")
@@ -565,13 +647,32 @@ class SyntheticViDAR(nn.Module):
         inter_num = len(self.bev_pred_head)
         next_bev_feats = [ref_bev.unsqueeze(0).repeat(inter_num, 1, 1, 1)]
         prev_bev_input = ref_bev.unsqueeze(1)
-        for _ in range(future_frames):
-            pred_feat, last = self.decode_future(prev_bev_input, can_bus)
-            next_bev_feats.append(pred_feat)
+        for k in range(1, future_frames + 1):
+            if supervised is None or k in supervised:
+                pred_feat, last = self.decode_future(prev_bev_input, can_bus)
+                next_bev_feats.append(pred_feat)
+            else:
+                with torch.no_grad():
+                    _, last = self.decode_future(prev_bev_input, can_bus)
             prev_bev_input = last.unsqueeze(1)                                         # queue length 1 (vidar.py:359-360)
         self._mark("future_decoder")
         next_bev_feats = torch.stack(next_bev_feats, 0)
         return self.forward_head(next_bev_feats)                                        # [F, inter, pred_frame, bs, Q, 16]
+
+    def host_draws(self, num_frames):
+        """forward_train's own draws from numpy's global generator, in its order (vidar.py:262-281, :333-338) ->
+        (drop_prev_index, supervised future frames or None for all).  No draw without `reference_draws`."""
+        if not self.reference_draws:
+            return -1, None
+        np.random.rand()                                  # A1: random_drop_image_rate is 0.0 in every config
+        drop_prev_index = -1
+        if np.random.rand() < self.drop_prev_rate:        # A2
+            end = self.drop_prev_end_idx if self.drop_prev_end_idx is not None else num_frames
+            drop_prev_index = int(np.random.randint(self.drop_prev_start_idx, end))
+        supervised = None
+        if self.future_frames > 0 and not self.supervise_all_future:
+            supervised = [int(np.random.choice(np.arange(1, self.future_frames + 1), 1)[0])]
+        return drop_prev_index, supervised
 
     def gt_points_of(self, point_infos, training):
         """The point half of the sample with the point pipeline: every GT frame's transforms in queue order (numpy's
@@ -585,27 +686,38 @@ class SyntheticViDAR(nn.Module):
             for step in steps:
                 results = step(results)
             frames.append(results)
-        return point_aug.gather_gt_points(frames, EGO_MASK, self.future_bev_embedding.weight.device)
+        return point_aug.gather_gt_points(frames, EGO_MASK, self.bev_embedding.weight.device)
 
     # ---- one training forward (vidar.py:239-387) -> dict of losses ----
-    def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None, point_infos=None):
+    def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None, point_infos=None,
+                      draws=None):
         """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
         (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
         frame index 0 = current .. future_frames).  With the image pipeline: img uint8 [1, T, cams, H, W, 3] and
         host cam2img / lidar2cam [1, cams, 4, 4]; lidar2img is not read.  With the point pipeline gt_points is built
-        from point_infos."""
+        from point_infos.  `draws`: `host_draws`'s (drop_prev_index, supervised future frames) to use instead of
+        drawing them."""
+        drop_prev_index, supervised = self.host_draws(img.shape[1]) if draws is None else draws
         if self.point_transforms is not None:
             gt_points = self.gt_points_of(point_infos, True)
-        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames, cam2img, lidar2cam)
-        valid_frames = list(range(1 + self.future_frames))
+        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames, cam2img, lidar2cam,
+                                              train=self.training, drop_prev_index=drop_prev_index,
+                                              supervised=supervised)
+        valid_frames = [0] + (list(range(1, 1 + self.future_frames)) if supervised is None else list(supervised))
+        fw = self.frame_loss_weight
         losses = {}
         for i in range(self.pred_frame_num):                                            # vidar_head_v1.py:179-218
             pred_dict = dict(next_bev_preds=next_bev_preds[:, :, i], valid_frames=valid_frames)
-            lw = np.array([[self.per_frame_loss_weight[i]]] * len(valid_frames))
+            if fw is None:
+                lw = np.array([[self.per_frame_loss_weight[i]]] * len(valid_frames))
+                scale = None
+            else:           # the current head frame by the frame weights, the others on the current frame only
+                lw = fw if i == self.head_history_frames else np.array([[1.0]] + [[0.0]] * (len(fw) - 1))
+                scale = self.per_frame_loss_weight[i]
             ld = self.ray_head.loss(pred_dict, gt_points, 0, self.bev_h, self.bev_w, PC_RANGE, pred_frame_num=1 + self.future_frames,
                                     loss_weight=lw)
             for k, v in ld.items():
-                losses[f"frame.{i}.{k}"] = v
+                losses[f"frame.{i}.{k}"] = v if scale is None else v * scale
         self._mark("head+loss")
         return losses
 
@@ -621,14 +733,14 @@ class SyntheticViDAR(nn.Module):
     def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None, point_infos=None):
         """vidar.py:389-502 without submission writing and visualisation -> [ret_dict], ret_dict =
         {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}} for the current frame (t = 0) and every
-        future frame, scored on the current head frame (`history_frames`) by ray_head.evaluate (one batched device
+        future frame, scored on the current head frame (`head_history_frames`) by ray_head.evaluate (one batched device
         pass).  gt_points as forward_train's, frames 0 .. future_frames; the origin is zero in every frame.  Under a
         process group every rank computes the same result.  With the point pipeline gt_points is built from
         point_infos by the test pipeline."""
         if self.point_transforms is not None:
             gt_points = self.gt_points_of(point_infos, False)
         pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus)
-        cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.history_frames])
+        cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.head_history_frames])
         with torch.no_grad():
             ret = self.ray_head.evaluate(cur, gt_points, 0, self.bev_h, self.bev_w, PC_RANGE)
         return [ret]
@@ -741,13 +853,36 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None, 
     return loss.detach(), stages
 
 
-def build(device, group=None, lr=2e-4, seed=0, row_sharded=False, grid=None, **model_kwargs):
-    """-> (SyntheticViDAR in training mode with dropout off, AdamW).  `group`: one sample sharded over it.  `grid`
+# The training regimes of the four nuScenes pre-training configs (projects/configs/vidar_pretrain/nusc_*), as
+# SyntheticViDAR arguments: `build(device, config=name)`.  Sizes, the backbone (dcn) and the pipelines are not part of
+# a preset; arguments passed to `build` override the preset's.
+_HEAD_5 = dict(head_history_frames=3, head_future_frames=1, per_frame_loss_weight=(0.2, 0.4, 0.6, 1.0, 1.2))
+_ONE_FUTURE = dict(history_frames=3, future_frames=0, decoder_layers=1, backward_history_frames=1, drop_prev_rate=0.1,
+                   drop_prev_end_idx=3, frame_loss_weight=((1.0,), (0.0,)), point_voxel_size=0.5, reference_draws=True,
+                   **_HEAD_5)
+CONFIGS = {
+    "vidar_1_8_nusc_3future": dict(history_frames=3, future_frames=3, decoder_layers=3,
+                                   frame_loss_weight=((1.0,),) * 4 + ((0.0,),), latent_grid_step=0.5,
+                                   reference_draws=True, **_HEAD_5),
+    "vidar_full_nusc_1future": dict(_ONE_FUTURE, latent_grid_step=0.5),
+    "vidar_1_8_nusc_1future": dict(_ONE_FUTURE, latent_grid_step=1.0),
+    "mem_efficient_vidar_1_8_nusc_3future": dict(history_frames=3, future_frames=3, decoder_layers=3,
+                                                 supervise_all_future=False, head_history_frames=0,
+                                                 head_future_frames=0, per_frame_loss_weight=(1.0,),
+                                                 frame_loss_weight=((1.0,),) * 4 + ((0.0,),), latent_grid_step=1.0,
+                                                 reference_draws=True),
+}
+
+
+def build(device, group=None, lr=2e-4, seed=0, row_sharded=False, grid=None, config=None, **model_kwargs):
+    """-> (SyntheticViDAR in training mode with dropout off, AdamW).  `config`: a name in `CONFIGS`, whose training
+    regime `model_kwargs` then override; None builds the default graph.  `group`: one sample sharded over it.  `grid`
     (`sharding.make_grid(S)`): data-parallel replicas of the sharded model -- the model shards over the grid's shard
     group of S ranks, and `train_step(..., grid=grid)` averages the gradients over the world / S replicas.  Every rank
     passes the same `seed` (the replicas start from the same parameters).
 
-    Each replica trains on its own sample, and the host draws of a step (GridMask, the image and the point pipeline:
+    Each replica trains on its own sample, and the host draws of a step (forward_train's drop index and supervised
+    future frame under a preset, GridMask, the image and the point pipeline:
     numpy's global generator, and `random` for the image pipeline) must agree inside a shard group and differ across
     replicas.  Seed per replica, for example with base the run's seed:
         np.random.seed(base + grid.replica); random.seed(base + grid.replica)
@@ -759,6 +894,10 @@ def build(device, group=None, lr=2e-4, seed=0, row_sharded=False, grid=None, **m
         if row_sharded:
             raise ValueError("build: the row-sharded encoder is not supported under a grid")
         group = grid.group
+    if config is not None:
+        if config not in CONFIGS:
+            raise ValueError(f"build: unknown config {config!r}; one of {sorted(CONFIGS)}")
+        model_kwargs = dict(CONFIGS[config], **model_kwargs)
     torch.manual_seed(seed)
     model = SyntheticViDAR(**model_kwargs).to(device)
     model.set_process_group(group, row_sharded=row_sharded)
