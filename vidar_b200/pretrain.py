@@ -34,7 +34,6 @@ Data-parallel replicas of that (`build(..., grid=sharding.make_grid(S))`): world
 sample over S ranks; `train_step(..., grid=grid)` averages every trainable gradient over the replicas in ONE
 bucketed all-reduce over the world (`sharding.allreduce_grid_grads`).
 """
-import copy
 import math
 import os
 
@@ -51,6 +50,7 @@ from .grid_mask import GridMask
 from .head import ViDARRayHead
 from .modules.deform_attn import _linear
 from .registry import build_attention
+from .sample_loader import SampleLoader, run_image_transforms, run_point_transforms  # noqa: F401
 
 PC_RANGE = [-51.2, -51.2, -5.0, 51.2, 51.2, 3.0]
 EGO_MASK = (-0.8, -1.5, 0.8, 2.5)                    # the dataset's ego_mask (config :348)
@@ -454,16 +454,29 @@ class SyntheticViDAR(nn.Module):
             e.record()
             self.timings.append((name, e))
 
+    def backbone_cams(self):
+        """The cameras whose images this rank's backbone runs (all of them without a process group)."""
+        import torch.distributed as dist
+        if self.process_group is None or dist.get_world_size(self.process_group) == 1:
+            return list(range(self.num_cams))
+        return list(self.my_backbone_cams)
+
     # ---- image features of one frame -> [cams, K, bs, C] (only this rank's SCA cameras are filled) ----
-    def extract_feat(self, img, draw=None):
+    def extract_feat(self, img, draw=None, cams_only=False):
         """img [bs, cams, 3, H, W] -> (feat_flatten [cams, K, bs, C], spatial_shapes, level_start_index).  `draw`: a
         GridMask draw (`self.grid_mask.sample`) applied to the images before the backbone.  With the image pipeline,
-        img is (results of the frame's transforms, its uint8 frames [1, cams, H, W, 3])."""
+        img is (results of the frame's transforms, its uint8 frames [1, cams, H, W, 3]).  `cams_only`: img is a
+        `SampleLoader` frame, float32 [len(backbone_cams()), 3, H, W] of this rank's backbone cameras only (bs 1),
+        which goes to the backbone as it is."""
         import torch.distributed as dist
         world = dist.get_world_size(self.process_group) if self.process_group is not None else 1
         rank = dist.get_rank(self.process_group) if world > 1 else 0
         mine = self.my_backbone_cams if world > 1 else list(range(self.num_cams))
-        if self.image_transforms is not None:
+        if cams_only:
+            if img.dim() != 4 or img.shape[0] != len(mine):
+                raise ValueError(f"extract_feat: a loaded frame holds this rank's {len(mine)} backbone cameras as "
+                                 f"[{len(mine)}, 3, H, W] (got {tuple(img.shape)})")
+        elif self.image_transforms is not None:
             results, raw = img
             pipe = image_aug.apply_multiview(raw[0, mine], results, mine) if mine else None
             if mine == list(range(self.num_cams)):
@@ -472,10 +485,10 @@ class SyntheticViDAR(nn.Module):
                 img = raw.new_empty((1, self.num_cams, 3, *results["img_aug"].pad_hw), dtype=torch.float32)
                 if mine:
                     img[0, mine] = pipe
-        bs = img.shape[0]
+        bs = 1 if cams_only else img.shape[0]
         per_cam = {}
         if mine:
-            x = img[:, mine].reshape(bs * len(mine), *img.shape[2:])
+            x = img if cams_only else img[:, mine].reshape(bs * len(mine), *img.shape[2:])
             if draw is not None:
                 x = self.grid_mask.masked(x, draw)
             if self.backbone_autocast is None:
@@ -582,20 +595,12 @@ class SyntheticViDAR(nn.Module):
                              f"{img.dtype} {tuple(img.shape)})")
         if cam2img is None or lidar2cam is None:
             raise ValueError("image_pipeline: forward needs cam2img and lidar2cam")
-        frames, aug_param = [], None
-        for t in range(img.shape[1]):
-            results = dict(img=list(img[0, t]), cam2img=[np.array(m, np.float64) for m in cam2img[0]],
-                           lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]])
-            if aug_param is not None:
-                results["aug_param"] = copy.deepcopy(aug_param)
-            for transform in self.image_transforms:
-                results = transform(results)
-            aug_param = copy.deepcopy(results["aug_param"])
-            frames.append(results)
-        return frames
+        return run_image_transforms(self.image_transforms, [
+            dict(img=list(img[0, t]), cam2img=[np.array(m, np.float64) for m in cam2img[0]],
+                 lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]]) for t in range(img.shape[1])])
 
     def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None, train=False,
-                        drop_prev_index=-1, supervised=None):
+                        drop_prev_index=-1, supervised=None, img_metas=None):
         """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + len(supervised), inter, pred_frame, bs, Q, 16]: the
         history BEV of the first T - 1 frames, the current frame's BEV as ref_bev, `future_frames` roll-outs with a
         queue of length 1 -- those not in `supervised` (default: all) under no_grad --, then the head over the current
@@ -606,11 +611,19 @@ class SyntheticViDAR(nn.Module):
         `backward_history_frames` frames are backwarded -- backbone under no_grad, encoder with gradient --, the
         others frozen under no_grad; frozen frame i < `drop_prev_index` is not computed, as its BEV would be
         discarded.  Each of the two parts makes its eval-mode GridMask draw (one prob gate per extract_feat call of
-        the reference), also when the drop skips every frozen frame."""
-        bs, T = img.shape[:2]
-        dev = img.device
+        the reference), also when the drop skips every frozen frame.
+
+        `img_metas` (a `SampleLoader` sample): img is then a list over the T frames of the pipelined images of this
+        rank's backbone cameras, float32 [len(backbone_cams()), 3, H, W], and img_metas the frames' metas."""
+        loaded = img_metas is not None
+        bs, T = (1, len(img)) if loaded else img.shape[:2]
+        dev = img[0].device if loaded else img.device
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
-        if self.image_transforms is not None:
+        if loaded:
+            if len(img_metas) != T:
+                raise ValueError(f"_next_bev_preds: {T} loaded frames, {len(img_metas)} img_metas")
+            inputs, metas, hw = list(img), img_metas, tuple(img[-1].shape[-2:])
+        elif self.image_transforms is not None:
             frames = self.frame_transforms(img, cam2img, lidar2cam)
             inputs = [(r, img[:, t]) for t, r in enumerate(frames)]
             metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"])] for r in frames]
@@ -627,7 +640,7 @@ class SyntheticViDAR(nn.Module):
             self.grid_mask.sample(*hw, training=False)
         with torch.no_grad():                                                        # _obtain_frozen_history_bev
             for t in range(min(max(drop_prev_index, 0), frozen), frozen):
-                feats, shapes, lsi = self.extract_feat(inputs[t])
+                feats, shapes, lsi = self.extract_feat(inputs[t], cams_only=loaded)
                 self._mark(f"hist{t}.backbone")
                 prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
                 self._mark(f"hist{t}.encoder")
@@ -635,12 +648,12 @@ class SyntheticViDAR(nn.Module):
             self.grid_mask.sample(*hw, training=False)
         for t in range(frozen, T - 1):
             with torch.no_grad():
-                feats, shapes, lsi = self.extract_feat(inputs[t])
+                feats, shapes, lsi = self.extract_feat(inputs[t], cams_only=loaded)
             self._mark(f"hist{t}.backbone")
             prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
             self._mark(f"hist{t}.encoder")
         draw = self.grid_mask.sample(*hw) if self.grid_mask is not None else None
-        feats, shapes, lsi = self.extract_feat(inputs[T - 1], draw)
+        feats, shapes, lsi = self.extract_feat(inputs[T - 1], draw, cams_only=loaded)
         self._mark("cur.backbone")
         ref_bev = self.encode(feats, shapes, lsi, metas[T - 1], can_bus, prev_bev)
         self._mark("cur.encoder")
@@ -679,30 +692,34 @@ class SyntheticViDAR(nn.Module):
         draws), then one device pass -> gt_points [1, R, 5] (NaN rows belong to no frame)."""
         if not point_infos:
             raise ValueError("point_pipeline: forward needs point_infos (synthetic_sample(..., raw_points=True))")
-        steps = self.point_transforms[0 if training else 1]
-        frames = []
-        for info in point_infos:
-            results = dict(info)
-            for step in steps:
-                results = step(results)
-            frames.append(results)
-        return point_aug.gather_gt_points(frames, EGO_MASK, self.bev_embedding.weight.device)
+        return self.gather_points(run_point_transforms(self.point_transforms[0 if training else 1], point_infos))
+
+    def gather_points(self, point_frames):
+        """The device half of gt_points_of: the transformed GT frames' results -> gt_points [1, R, 5], on the current
+        stream."""
+        return point_aug.gather_gt_points(point_frames, EGO_MASK, self.bev_embedding.weight.device)
 
     # ---- one training forward (vidar.py:239-387) -> dict of losses ----
     def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None, point_infos=None,
-                      draws=None):
+                      draws=None, img_metas=None):
         """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
         (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
         frame index 0 = current .. future_frames).  With the image pipeline: img uint8 [1, T, cams, H, W, 3] and
         host cam2img / lidar2cam [1, cams, 4, 4]; lidar2img is not read.  With the point pipeline gt_points is built
         from point_infos.  `draws`: `host_draws`'s (drop_prev_index, supervised future frames) to use instead of
-        drawing them."""
-        drop_prev_index, supervised = self.host_draws(img.shape[1]) if draws is None else draws
-        if self.point_transforms is not None:
+        drawing them.
+
+        A `SampleLoader` sample instead: `img_metas` given, img the list of the T frames' pipelined images of this
+        rank's backbone cameras and gt_points its device [1, R, 5]; the transforms ran in the loader, so neither
+        pipeline runs here and lidar2img, cam2img, lidar2cam and point_infos are not read."""
+        loaded = img_metas is not None
+        num_frames = len(img) if loaded else img.shape[1]
+        drop_prev_index, supervised = self.host_draws(num_frames) if draws is None else draws
+        if self.point_transforms is not None and not loaded:
             gt_points = self.gt_points_of(point_infos, True)
         next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames, cam2img, lidar2cam,
                                               train=self.training, drop_prev_index=drop_prev_index,
-                                              supervised=supervised)
+                                              supervised=supervised, img_metas=img_metas)
         valid_frames = [0] + (list(range(1, 1 + self.future_frames)) if supervised is None else list(supervised))
         fw = self.frame_loss_weight
         losses = {}
@@ -723,23 +740,25 @@ class SyntheticViDAR(nn.Module):
 
     # ---- inference (vidar.py:389-502) ----
     @torch.no_grad()
-    def predict_future(self, img, lidar2img, future_frames, can_bus=None):
+    def predict_future(self, img, lidar2img, future_frames, can_bus=None, img_metas=None):
         """forward_test's prediction (vidar.py:392-437): the same inputs as forward_train, `future_frames` roll-outs
         (the reference's test_future_frame_num) -> pred_dict {next_bev_preds [1 + future_frames, inter, pred_frame,
         bs, Q, 16], valid_frames [0 .. future_frames]}."""
-        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames)
+        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames, img_metas=img_metas)
         return dict(next_bev_preds=next_bev_preds, valid_frames=list(range(1 + future_frames)))
 
-    def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None, point_infos=None):
+    def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None, point_infos=None,
+                     img_metas=None):
         """vidar.py:389-502 without submission writing and visualisation -> [ret_dict], ret_dict =
         {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}} for the current frame (t = 0) and every
         future frame, scored on the current head frame (`head_history_frames`) by ray_head.evaluate (one batched device
         pass).  gt_points as forward_train's, frames 0 .. future_frames; the origin is zero in every frame.  Under a
         process group every rank computes the same result.  With the point pipeline gt_points is built from
-        point_infos by the test pipeline."""
-        if self.point_transforms is not None:
+        point_infos by the test pipeline.  `img_metas`: a `SampleLoader` sample, as in forward_train; its frames and
+        gt_points went through the loader's train transforms, which this path then scores as they are."""
+        if self.point_transforms is not None and img_metas is None:
             gt_points = self.gt_points_of(point_infos, False)
-        pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus)
+        pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus, img_metas=img_metas)
         cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.head_history_frames])
         with torch.no_grad():
             ret = self.ray_head.evaluate(cur, gt_points, 0, self.bev_h, self.bev_w, PC_RANGE)
@@ -750,7 +769,7 @@ class SyntheticViDAR(nn.Module):
 # synthetic sample + step
 # ------------------------------------------------------------------------------------------------
 def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000, future_frames=3, seed=0,
-                     bev_hw=(BEV_H, BEV_W), raw_images=False, raw_points=False, points_per_frame=35000):
+                     bev_hw=(BEV_H, BEV_W), raw_images=False, raw_points=False, points_per_frame=35000, files=False):
     """6 x 3 x 928 x 1600 N(0,1) frames, a nuScenes-like rig, LiDAR-like future point clouds (SURVEY.md 8d cfg4).
     `raw_images=True` (for `SyntheticViDAR(image_pipeline=True)`): seeded uniform uint8 BGR frames
     [1, frames, cams, 900, 1600, 3] (img_hw defaults to the camera size) and the rig's host `cam2img` / `lidar2cam`
@@ -758,7 +777,14 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000
     `raw_points=True` (for `SyntheticViDAR(point_pipeline=True)`): `point_infos`, the results dicts of the
     1 + future_frames GT frames, each a LiDAR-like key frame and 2 sweeps of `points_per_frame` points with their
     own poses and timestamps (`synthetic.lidar_cloud`, `synthetic.sweep_pose`), written as .bin files to a
-    temporary directory that is removed when the process exits."""
+    temporary directory that is removed when the process exits.
+    `files=True` (for `SampleLoader`): instead of a sample, the queue's results dicts as a dataset's get_data_info
+    hands them to its pipeline, one per queue frame, oldest first: the `frames` image frames (the history and the
+    current one) with `img_filename`, `cam2img` and `lidar2cam`, the current and the future frames with the point
+    infos of `raw_points`.  Each camera image is a baseline 4:2:0 JPEG written by cv2.imwrite at quality
+    `JPEG_QUALITY` (img_hw defaults to 900 x 1600), to a temporary directory removed at exit.  `device` is not used."""
+    if files:
+        return synthetic_queue(frames, cams, img_hw or (900, 1600), future_frames, points_per_frame, seed)
     g = torch.Generator(device=device).manual_seed(seed)
     extra = {}
     if raw_images:
@@ -785,13 +811,49 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000
     return dict(img=img, lidar2img=lidar2img, gt_points=pts, **extra)
 
 
-def synthetic_point_infos(frames, n, seed=0, sweeps=2):
-    """Results dicts (pts_filename, timestamp, sweeps) of `frames` LiDAR frames, files in a temporary directory."""
+JPEG_QUALITY = 90
+
+
+def _temp_dir(prefix):
+    """A new temporary directory, removed when the process exits."""
     import atexit
     import shutil
     import tempfile
-    root = tempfile.mkdtemp(prefix="vidar_points_")
+    root = tempfile.mkdtemp(prefix=prefix)
     atexit.register(shutil.rmtree, root, True)
+    return root
+
+
+def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=0):
+    """`synthetic_sample(..., files=True)`: image frames 0 .. frames - 1, point frames frames - 1 .. frames - 1 +
+    future_frames, every frame with the same rig."""
+    import cv2
+    root = _temp_dir("vidar_cameras_")
+    rng = np.random.default_rng(seed + 1000003)
+    cam2img, lidar2cam = synthetic.camera_rig_split(cams)
+    params = [cv2.IMWRITE_JPEG_QUALITY, JPEG_QUALITY, cv2.IMWRITE_JPEG_PROGRESSIVE, 0,
+              cv2.IMWRITE_JPEG_SAMPLING_FACTOR, cv2.IMWRITE_JPEG_SAMPLING_FACTOR_420]
+    queue = []
+    for t in range(frames):
+        names = []
+        for c in range(cams):
+            name = os.path.join(root, f"{t}.cam{c}.jpg")
+            if not cv2.imwrite(name, synthetic.camera_image(rng, img_hw), params):
+                raise RuntimeError(f"synthetic_sample: cv2.imwrite could not write {name}")
+            names.append(name)
+        queue.append(dict(img_filename=names, cam2img=[m.copy() for m in cam2img],
+                          lidar2cam=[m.copy() for m in lidar2cam]))
+    for k, info in enumerate(synthetic_point_infos(1 + future_frames, points_per_frame, seed)):
+        if k == 0:
+            queue[-1].update(info)
+        else:
+            queue.append(info)
+    return queue
+
+
+def synthetic_point_infos(frames, n, seed=0, sweeps=2):
+    """Results dicts (pts_filename, timestamp, sweeps) of `frames` LiDAR frames, files in a temporary directory."""
+    root = _temp_dir("vidar_points_")
     rng = np.random.default_rng(seed)
     infos = []
     for f in range(frames):
@@ -815,7 +877,8 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None, 
     the backward and the gradients unscaled before the clip; the scaler skips a step whose gradients are not finite.
     `grid` (`sharding.make_grid`, the model built with `build(..., grid=grid)`): `sample` is this replica's sample
     and the sync is the grid's one bucketed all-reduce (`sharding.allreduce_grid_grads`): every rank ends with the
-    replica mean of the gradients.  -> (loss value tensor -- this replica's --, [(stage, ms)] when `record`)."""
+    replica mean of the gradients.  `sample` may be a `SampleLoader` sample (its frames decoded and pipelined, its
+    gt_points on the device).  -> (loss value tensor -- this replica's --, [(stage, ms)] when `record`)."""
     if grid is not None and group is not None:
         raise ValueError("train_step: pass group= or grid=, not both")
     model.timings = [] if record else None
@@ -824,7 +887,7 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None, 
     optimizer.zero_grad(set_to_none=True)
     losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"], can_bus=sample.get("can_bus"),
                                  cam2img=sample.get("cam2img"), lidar2cam=sample.get("lidar2cam"),
-                                 point_infos=sample.get("point_infos"))
+                                 point_infos=sample.get("point_infos"), img_metas=sample.get("img_metas"))
     loss = sum(losses.values())
     (loss if scaler is None else scaler.scale(loss)).backward()
     model._mark("backward")

@@ -146,6 +146,17 @@ def lidar_cloud(rng, n, lattice=64):
     return (np.round(pts * lattice) / lattice).astype(np.float32)
 
 
+def camera_image(rng, hw):
+    """A camera-like uint8 [h, w, 3] BGR image: a smooth random field (a 1/32-scale random image, bicubic-upsampled)
+    with a little per-pixel noise, so that it compresses like a photograph rather than like white noise."""
+    import cv2
+    h, w = hw
+    small = rng.integers(0, 256, (h // 32 + 2, w // 32 + 2, 3), dtype=np.uint8)
+    img = cv2.resize(small, (w, h), interpolation=cv2.INTER_CUBIC).astype(np.int16)
+    img += rng.integers(-4, 5, img.shape, dtype=np.int16)
+    return np.clip(img, 0, 255).astype(np.uint8)
+
+
 def sweep_pose(rng, k):
     """(sensor2lidar_rotation, sensor2lidar_translation) float64 of the k-th earlier sweep: the ego moving about
     0.5 m and turning about 0.3 degrees per sweep, with a slight roll."""
