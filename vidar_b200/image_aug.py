@@ -443,12 +443,22 @@ def apply_multiview(img, results, cams=None):
     return out
 
 
+CONFIG_IMG_NORM = dict(mean=[103.530, 116.280, 123.675], std=[1.0, 1.0, 1.0], to_rgb=False)   # cfg :50-51
+
+
 def config_pipeline(ida_aug_conf=None):
     """The four transforms of the pre-training config (vidar_1_8_nusc_3future.py:41-51, 303-314)."""
     conf = ida_aug_conf if ida_aug_conf is not None else dict(
         reisze=[720, 765, 810, 855, 900, 945, 990, 1035, 1080], crop=(0, 0, 1600, 900), H=900, W=1600, rand_flip=True)
     return [PhotoMetricDistortionMultiViewImage(),
             CropResizeFlipImage(data_aug_conf=conf, training=True, debug=False),
-            NormalizeMultiviewImage(mean=[103.530, 116.280, 123.675], std=[1.0, 1.0, 1.0], to_rgb=False),
+            NormalizeMultiviewImage(**CONFIG_IMG_NORM),
             PadMultiViewImage(size_divisor=32)]
+
+
+def config_test_pipeline():
+    """The image transforms of the pre-training config's test_pipeline (vidar_1_8_nusc_3future.py:319-328), after
+    LoadMultiViewImageFromFiles: normalisation with the config's img_norm_cfg, then padding to multiples of 32.  No
+    draw, no crop or resize: `lidar2img` passes through as the dataset gives it, and `img_shape` is the padded shape."""
+    return [NormalizeMultiviewImage(**CONFIG_IMG_NORM), PadMultiViewImage(size_divisor=32)]
 

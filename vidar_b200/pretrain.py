@@ -43,6 +43,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import bev_geometry, optim, sca, sharding, synthetic
+from . import evaluate as eval_metrics
 from . import modules as _modules  # noqa: F401  (registers the attention classes)
 from . import image_aug
 from . import point_pipeline as point_aug
@@ -600,7 +601,7 @@ class SyntheticViDAR(nn.Module):
                  lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]]) for t in range(img.shape[1])])
 
     def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None, train=False,
-                        drop_prev_index=-1, supervised=None, img_metas=None):
+                        drop_prev_index=-1, supervised=None, img_metas=None, feature_cache=None):
         """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + len(supervised), inter, pred_frame, bs, Q, 16]: the
         history BEV of the first T - 1 frames, the current frame's BEV as ref_bev, `future_frames` roll-outs with a
         queue of length 1 -- those not in `supervised` (default: all) under no_grad --, then the head over the current
@@ -614,8 +615,17 @@ class SyntheticViDAR(nn.Module):
         the reference), also when the drop skips every frozen frame.
 
         `img_metas` (a `SampleLoader` sample): img is then a list over the T frames of the pipelined images of this
-        rank's backbone cameras, float32 [len(backbone_cams()), 3, H, W], and img_metas the frames' metas."""
+        rank's backbone cameras, float32 [len(backbone_cams()), 3, H, W], and img_metas the frames' metas.
+
+        `feature_cache` (a dict, with a test-mode `SampleLoader` sample, whose metas carry each frame's `filename`): a
+        frame whose camera files were a frame of the previous call's sample takes that frame's stored extract_feat
+        output (feats, spatial_shapes, level_start_index) instead of running the backbone again; on return the dict
+        holds this sample's frames only.  A frame masked by a GridMask draw is always computed and never stored.  The
+        GridMask draws are made as without the cache."""
         loaded = img_metas is not None
+        if feature_cache is not None and (not loaded or any("filename" not in m[0] for m in img_metas)):
+            raise ValueError("_next_bev_preds: feature_cache needs a test-mode SampleLoader sample (img_metas with "
+                             "each frame's filename)")
         bs, T = (1, len(img)) if loaded else img.shape[:2]
         dev = img[0].device if loaded else img.device
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
@@ -635,12 +645,24 @@ class SyntheticViDAR(nn.Module):
             hw = img.shape[-2:]
         backwarded = min(self.backward_history_frames, T - 1) if train else 0
         frozen = T - 1 - backwarded
+        fresh = None if feature_cache is None else {}
+
+        def features(t, draw=None):
+            if fresh is None or draw is not None:
+                return self.extract_feat(inputs[t], draw, cams_only=loaded)
+            key = tuple(metas[t][0]["filename"])
+            out = feature_cache.get(key)
+            if out is None:
+                out = self.extract_feat(inputs[t], cams_only=loaded)
+            fresh[key] = out
+            return out
+
         prev_bev = None
         if self.grid_mask is not None and frozen > 0:                                # the history's eval-mode call
             self.grid_mask.sample(*hw, training=False)
         with torch.no_grad():                                                        # _obtain_frozen_history_bev
             for t in range(min(max(drop_prev_index, 0), frozen), frozen):
-                feats, shapes, lsi = self.extract_feat(inputs[t], cams_only=loaded)
+                feats, shapes, lsi = features(t)
                 self._mark(f"hist{t}.backbone")
                 prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
                 self._mark(f"hist{t}.encoder")
@@ -648,12 +670,15 @@ class SyntheticViDAR(nn.Module):
             self.grid_mask.sample(*hw, training=False)
         for t in range(frozen, T - 1):
             with torch.no_grad():
-                feats, shapes, lsi = self.extract_feat(inputs[t], cams_only=loaded)
+                feats, shapes, lsi = features(t)
             self._mark(f"hist{t}.backbone")
             prev_bev = self.encode(feats, shapes, lsi, metas[t], can_bus, prev_bev)
             self._mark(f"hist{t}.encoder")
         draw = self.grid_mask.sample(*hw) if self.grid_mask is not None else None
-        feats, shapes, lsi = self.extract_feat(inputs[T - 1], draw, cams_only=loaded)
+        feats, shapes, lsi = features(T - 1, draw)
+        if fresh is not None:                                                        # only this sample's frames
+            feature_cache.clear()
+            feature_cache.update(fresh)
         self._mark("cur.backbone")
         ref_bev = self.encode(feats, shapes, lsi, metas[T - 1], can_bus, prev_bev)
         self._mark("cur.encoder")
@@ -740,11 +765,12 @@ class SyntheticViDAR(nn.Module):
 
     # ---- inference (vidar.py:389-502) ----
     @torch.no_grad()
-    def predict_future(self, img, lidar2img, future_frames, can_bus=None, img_metas=None):
+    def predict_future(self, img, lidar2img, future_frames, can_bus=None, img_metas=None, feature_cache=None):
         """forward_test's prediction (vidar.py:392-437): the same inputs as forward_train, `future_frames` roll-outs
         (the reference's test_future_frame_num) -> pred_dict {next_bev_preds [1 + future_frames, inter, pred_frame,
-        bs, Q, 16], valid_frames [0 .. future_frames]}."""
-        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames, img_metas=img_metas)
+        bs, Q, 16], valid_frames [0 .. future_frames]}.  `feature_cache`: see `_next_bev_preds`."""
+        next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames, img_metas=img_metas,
+                                              feature_cache=feature_cache)
         return dict(next_bev_preds=next_bev_preds, valid_frames=list(range(1 + future_frames)))
 
     def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None, point_infos=None,
@@ -824,9 +850,10 @@ def _temp_dir(prefix):
     return root
 
 
-def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=0):
-    """`synthetic_sample(..., files=True)`: image frames 0 .. frames - 1, point frames frames - 1 .. frames - 1 +
-    future_frames, every frame with the same rig."""
+def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=0, first_gt=None):
+    """`synthetic_sample(..., files=True)`: image frames 0 .. frames - 1, point frames first_gt (default frames - 1)
+    .. frames - 1 + future_frames, every frame with the same rig."""
+    first_gt = frames - 1 if first_gt is None else first_gt
     import cv2
     root = _temp_dir("vidar_cameras_")
     rng = np.random.default_rng(seed + 1000003)
@@ -843,12 +870,35 @@ def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=
             names.append(name)
         queue.append(dict(img_filename=names, cam2img=[m.copy() for m in cam2img],
                           lidar2cam=[m.copy() for m in lidar2cam]))
-    for k, info in enumerate(synthetic_point_infos(1 + future_frames, points_per_frame, seed)):
-        if k == 0:
-            queue[-1].update(info)
+    for k, info in enumerate(synthetic_point_infos(frames - first_gt + future_frames, points_per_frame, seed)):
+        if first_gt + k < frames:
+            queue[first_gt + k].update(info)
         else:
             queue.append(info)
     return queue
+
+
+def synthetic_scene(num_samples, frames, future_frames, cams=6, img_hw=(900, 1600), points_per_frame=35000, seed=0):
+    """One scene's files, written once (`synthetic_queue`), as the sliding-window queues a test dataset builds from
+    consecutive keyframes (no load_frame_interval): sample i's image frames are the scene's frames i .. i + frames - 1
+    (the history and the current frame), its GT frames i + frames - 1 .. i + frames - 1 + future_frames.  Each image
+    frame carries `img_filename`, `cam2img`, `lidar2cam` and the test pipeline's `lidar2img` = cam2img @ lidar2cam
+    (float64), so the queues serve the test-mode and the train-mode `SampleLoader` alike.  Neighbouring samples share
+    frames - 1 image frames' files.  -> [queue] of num_samples queues."""
+    if num_samples < 1 or frames < 1 or future_frames < 0:
+        raise ValueError(f"synthetic_scene: num_samples, frames >= 1 and future_frames >= 0 "
+                         f"(got {num_samples}, {frames}, {future_frames})")
+    total = num_samples + frames - 1
+    scene = synthetic_queue(total, cams, img_hw, future_frames, points_per_frame, seed, first_gt=frames - 1)
+    images = [dict(img_filename=list(f["img_filename"]), cam2img=f["cam2img"], lidar2cam=f["lidar2cam"],
+                   lidar2img=[c @ l for c, l in zip(f["cam2img"], f["lidar2cam"])]) for f in scene[:total]]
+    gts = [{k: f[k] for k in ("pts_filename", "timestamp", "sweeps")} for f in scene if "pts_filename" in f]
+    queues = []
+    for i in range(num_samples):
+        queue = [dict(images[t]) for t in range(i, i + frames)]
+        queue[-1].update(gts[i])
+        queues.append(queue + [dict(g) for g in gts[i + 1:i + 1 + future_frames]])
+    return queues
 
 
 def synthetic_point_infos(frames, n, seed=0, sweeps=2):
@@ -979,3 +1029,85 @@ def config_optimizer(model, lr=2e-4):
     `optim.AdamW` step.  `build()` keeps torch's single-group AdamW; pass this to `train_step` instead."""
     return optim.AdamW(optim.paramwise_groups(model, lr, 0.01, {"backbone": dict(lr_mult=0.1)}), lr=lr,
                        weight_decay=0.01, max_grad_norm=35)
+
+
+# ------------------------------------------------------------------------------------------------
+# evaluation from files (the configs' `evaluation = dict(pipeline=test_pipeline)`, tools/test.py)
+# ------------------------------------------------------------------------------------------------
+def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0, grid=None):
+    """The dataset's evaluation over `samples` (queues of results dicts in dataset order, e.g. `synthetic_scene`'s):
+    the test-mode `SampleLoader`, the prediction of `forward_test` per sample, then `evaluate.summarize` -> the
+    summary {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}}, equal to
+    summarize([model.forward_test(...)[0] for each sample]) in dataset order (the reference's single_gpu_test /
+    multi_gpu_test, then dataset.evaluate).  The model must be built with point_pipeline=True.
+
+      * Each sample's metric table comes from the head's `evaluate_device` and stays on the device; the tables reach
+        the host once, at the end (`summarize_tables`).
+      * Feature reuse: consecutive samples of a scene share all image frames but the newest, and the test chain makes
+        no draw, so a frame's backbone + FPN output is the same in every sample that holds it.  A frame whose camera
+        files were in the previous sample takes that sample's features instead of running the backbone again
+        (`predict_future(..., feature_cache=...)`); across a scene boundary the files differ and the frame is
+        computed.  The cache lives for this call and holds one sample's frames.  GridMask's draws are made as without
+        it, so numpy's generator advances alike.
+      * `grid` (`sharding.make_grid`, the model built with it): replica r evaluates the contiguous block
+        `sharding.shard_range(N, r, R)` of the samples (contiguous, so the reuse keeps working); every rank of its
+        shard group walks the same block, so they hit and miss the cache together.  One all-gather of the tables over
+        the world, then every rank builds the same summary, and raises the same exception for the first failing
+        (sample, frame).
+
+    A queue with fewer than 1 + future_frames GT frames is rejected before any work."""
+    samples = list(samples)
+    for i, queue in enumerate(samples):
+        gt = sum("pts_filename" in f for f in queue)
+        if gt < 1 + future_frames:
+            raise ValueError(f"evaluate: sample {i} has {gt} GT frames; future_frames={future_frames} needs "
+                             f"{1 + future_frames} (the current frame and every future one)")
+    replica, replicas = (grid.replica, grid.replicas) if grid is not None else (0, 1)
+    lo, hi = sharding.shard_range(len(samples), replica, replicas)
+    loader = SampleLoader(model, samples[lo:hi], num_workers=num_workers, prefetch=prefetch, seed=seed, rank=replica,
+                          test_mode=True)
+    dev = model.bev_embedding.weight.device
+    frames = 1 + future_frames
+    tables, cache = [], {}
+    with torch.no_grad():
+        for sample in loader:
+            pred = model.predict_future(sample["img"], None, future_frames, img_metas=sample["img_metas"],
+                                        feature_cache=cache)
+            cur = dict(pred, next_bev_preds=pred["next_bev_preds"][:, :, model.head_history_frames])
+            tables.append(model.ray_head.evaluate_device(cur, sample["gt_points"], 0, model.bev_h, model.bev_w,
+                                                         PC_RANGE))
+            del pred, cur, sample                  # freed before the next sample's device half
+    cache.clear()
+    table = torch.cat(tables) if tables else torch.zeros((0, eval_metrics.FIELDS), dtype=torch.float64, device=dev)
+    return summarize_tables(table, len(samples), frames, grid)
+
+
+def summarize_tables(table, num_samples, frames, grid=None):
+    """The host end of `evaluate`: `table` [(hi - lo) * frames, 8] float64 (evaluate.FIELDS; row (i - lo) * frames +
+    t for sample i, frame t) holds this replica's block [lo, hi) = sharding.shard_range(num_samples, replica, R) of
+    the samples.  With a `grid` of more than one rank, the blocks are padded to the longest and all-gathered over
+    `grid.world_group` (each replica's block is taken from its shard rank 0).  One host copy; then the first failing
+    (sample, frame) in (sample, frame) order raises the exception forward_test raises for it, on every rank, and
+    otherwise -> evaluate.summarize of the per-sample ret_dicts (the same sums, in dataset order)."""
+    replica, replicas, shard = (grid.replica, grid.replicas, grid.shard_size) if grid is not None else (0, 1, 1)
+    blocks = [sharding.shard_range(num_samples, r, replicas) for r in range(replicas)]
+    lo, hi = blocks[replica]
+    if tuple(table.shape) != ((hi - lo) * frames, eval_metrics.FIELDS):
+        raise ValueError(f"summarize_tables: samples [{lo}, {hi}) x {frames} frames need a "
+                         f"[{(hi - lo) * frames}, {eval_metrics.FIELDS}] table (got {tuple(table.shape)})")
+    if replicas * shard > 1:
+        import torch.distributed as dist
+        longest = max(b - a for a, b in blocks) * frames
+        padded = table.new_zeros((longest, eval_metrics.FIELDS))
+        padded[:table.shape[0]] = table
+        parts = [torch.empty_like(padded) for _ in range(replicas * shard)]
+        dist.all_gather(parts, padded, group=grid.world_group)
+        table = torch.cat([parts[r * shard][:(b - a) * frames] for r, (a, b) in enumerate(blocks)])
+    host = table.cpu().numpy()
+    for i in range(num_samples):
+        for t in range(frames):
+            eval_metrics.raise_for_flags(host[i * frames + t, 7], f"sample {i}, frame {t}")
+    if num_samples == 0:
+        return {}
+    # one ret_dict summed over the samples in dataset order: the per-sample dicts' sums, as summarize forms them
+    return eval_metrics.summarize([eval_metrics.frame_metrics_host(host, num_samples, frames)])

@@ -11,6 +11,9 @@ worker (`QueueDataset`) runs, in the order `SyntheticViDAR.forward_train` runs t
     draws), then the image transforms' draws (`run_image_transforms`, with `aug_param` carried across frames; the
     host half of `frame_transforms`).
 
+With `test_mode=True` a worker runs the config's test pipeline instead: LoadPointsFromFile on the GT frames, and
+LoadMultiViewImageFromFiles, normalisation and padding on the image frames, with no draw at all.
+
 It returns the parsed JPEG records, the image plans and the point plans, not pixels.  The model's own draws (A1 / A2
 and the supervised future frame, `host_draws`) and GridMask's stay in the training process, as the reference's
 detector makes them there.  Workers are seeded as mmdet's `worker_init_fn` seeds them: numpy, `random` and torch with
@@ -67,12 +70,14 @@ def run_point_transforms(transforms, infos):
 class QueueDataset(torch.utils.data.Dataset):
     """The host half of a sample: `samples[i]` is a queue of results dicts; frames with `img_filename` are the image
     frames, frames with `pts_filename` the GT frames.  -> dict(frames=[image results], points=[point results],
-    index=i).  Makes no CUDA call."""
+    index=i).  Makes no CUDA call.  `test_mode`: an image frame brings its `lidar2img` (the test chain does not form
+    it) instead of `cam2img` and `lidar2cam`."""
 
-    def __init__(self, samples, image_transforms, point_transforms):
+    def __init__(self, samples, image_transforms, point_transforms, test_mode=False):
         self.samples = list(samples)
         self.image_transforms = list(image_transforms)
         self.point_transforms = list(point_transforms)
+        self.test_mode = bool(test_mode)
         self.load_images = jpeg.LoadMultiViewImageFromFiles(to_float32=True)
 
     def __len__(self):
@@ -81,10 +86,14 @@ class QueueDataset(torch.utils.data.Dataset):
     def __getitem__(self, index):
         queue = self.samples[index]
         points = run_point_transforms(self.point_transforms, [f for f in queue if "pts_filename" in f])
-        frames = [self.load_images(dict(img_filename=list(f["img_filename"]),
-                                        cam2img=[np.array(m, np.float64) for m in f["cam2img"]],
-                                        lidar2cam=[np.array(m, np.float64) for m in f["lidar2cam"]]))
-                  for f in queue if "img_filename" in f]
+        keys = ("lidar2img",) if self.test_mode else ("cam2img", "lidar2cam")
+        frames = []
+        for f in queue:
+            if "img_filename" in f:
+                if self.test_mode and "lidar2img" not in f:
+                    raise ValueError(f"sample {index}: an image frame of the test pipeline needs its lidar2img")
+                frames.append(self.load_images(dict(img_filename=list(f["img_filename"]),
+                                                    **{k: [np.array(m, np.float64) for m in f[k]] for k in keys})))
         if not frames or not points:
             raise ValueError(f"sample {index}: a queue needs image frames (img_filename) and GT frames (pts_filename)")
         return dict(frames=run_image_transforms(self.image_transforms, frames), points=points, index=index)
@@ -109,22 +118,31 @@ class SampleLoader:
     gt_points=[1, R, 5] on the device, lidar2img=None, index).
 
     `model`: a `SyntheticViDAR` built with image_pipeline=True and point_pipeline=True, whose train transforms the
-    workers run (`model.image_transforms`, `model.point_transforms[0]`).  There is no evaluation variant: the
-    model's image transforms are the train chain, and evaluation's chain would differ from it (no photometric
-    distortion, a fixed crop / resize, lidar2img from the dataset); `forward_test` takes a sample of this loader as
-    it is.
+    workers run (`model.image_transforms`, `model.point_transforms[0]`).
+    `test_mode=True` runs the config's test pipeline instead, as its val / test datasets do: per image frame
+    `LoadMultiViewImageFromFiles`, normalisation and padding (`image_aug.config_test_pipeline`: no draw, no crop or
+    resize), with each frame's `lidar2img` taken from its results dict as it is; per GT frame LoadPointsFromFile only
+    (`model.point_transforms[1]`).  The model then needs point_pipeline=True only, and each frame's img_metas also
+    carry `filename`, its camera files, as the reference's metas do (`pretrain.evaluate` keys its feature reuse on
+    them).  The device half is the same.
     `num_workers`: DataLoader worker processes (0: the host half on this process).  `prefetch`: samples whose device
     half runs ahead on a side stream (0: on the current stream, at hand-out).  `seed` and `rank` seed the workers;
     `rank` is the data-parallel replica (`grid.replica`): every rank of a shard group passes the same value and
     iterates the same samples, so their draws agree, and each decodes only its own backbone cameras."""
 
-    def __init__(self, model, samples, num_workers=0, prefetch=1, seed=0, rank=0):
-        if model.image_transforms is None or model.point_transforms is None:
+    def __init__(self, model, samples, num_workers=0, prefetch=1, seed=0, rank=0, test_mode=False):
+        if test_mode and model.point_transforms is None:
+            raise ValueError("SampleLoader(test_mode=True): the model must be built with point_pipeline=True")
+        if not test_mode and (model.image_transforms is None or model.point_transforms is None):
             raise ValueError("SampleLoader: the model must be built with image_pipeline=True and point_pipeline=True")
         if num_workers < 0 or prefetch < 0:
             raise ValueError(f"SampleLoader: num_workers and prefetch must be >= 0 (got {num_workers}, {prefetch})")
         self.model, self.prefetch, self.num_workers = model, int(prefetch), int(num_workers)
-        self.dataset = QueueDataset(samples, model.image_transforms, model.point_transforms[0])
+        self.test_mode = bool(test_mode)
+        if test_mode:
+            self.dataset = QueueDataset(samples, image_aug.config_test_pipeline(), model.point_transforms[1], True)
+        else:
+            self.dataset = QueueDataset(samples, model.image_transforms, model.point_transforms[0])
         init = functools.partial(seed_worker, num_workers=num_workers, rank=rank, seed=seed) if num_workers else None
         self.host_loader = torch.utils.data.DataLoader(self.dataset, batch_size=None, shuffle=False,
                                                        num_workers=num_workers, collate_fn=_one, worker_init_fn=init)
@@ -144,7 +162,8 @@ class SampleLoader:
             img = [image_aug.apply_multiview(raw, r, cams) for r, raw in zip(frames, decoded)]
         else:
             img = [torch.empty((0, 3, *r["img_aug"].pad_hw), dtype=torch.float32, device=dev) for r in frames]
-        metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"])] for r in frames]
+        metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"],
+                       **(dict(filename=list(r["filename"])) if self.test_mode else {}))] for r in frames]
         return dict(img=img, img_metas=metas, gt_points=model.gather_points(host["points"]), lidar2img=None,
                     index=host["index"])
 
