@@ -749,6 +749,22 @@ int vidar_adamw_step(const int64_t* param_host, const int64_t* grad_host, const 
                      const float* scalar_host, int n, float* exp_avg, float* exp_avg_sq, long long state_numel,
                      int clip, float max_norm, float* grad_norm, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * (xv) TemporalSelfAttention's value with ego motion (modules/transformer.py:137-150, modules/encoder.py:225-229,
+ * vidar_b200/ego_motion.py): the previous BEV rotated by the frame's yaw change, stacked with the query.
+ *   prev, query  [bs, Q, C] fp32;  rows [bs, Q] int32: output cell q copies source cell rows[b, q] of sample b's
+ *                previous BEV where rows[b, q] lies in [0, Q), zeros otherwise (any value is safe);  C a multiple
+ *                of 4
+ *   forward   value [bs * 2, Q, C]: value[2b] = the rotated previous BEV, value[2b + 1] = query[b]
+ *   backward  grad_prev[b, s] = the sum of grad_value[2b, q] over the q with rows[b, q] = s, in ascending q (a stable
+ *             radix sort of the map; no float atomics, bitwise deterministic); grad_query[b] = grad_value[2b + 1]
+ * One launch forward; backward one memset, two small kernels, a radix sort and one gather, its scratch from the
+ * library's stream-ordered pool.  No host sync. */
+int vidar_bev_rotate_stack_forward(const float* prev, const float* query, const int32_t* rows, float* value, int bs,
+                                   int Q, int C, void* stream);
+int vidar_bev_rotate_stack_backward(const float* grad_value, const int32_t* rows, float* grad_prev, float* grad_query,
+                                    int bs, int Q, int C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

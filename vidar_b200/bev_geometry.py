@@ -3,8 +3,8 @@
   get_reference_points  BEVFormerEncoder.get_reference_points  (modules/encoder.py:53-92)
   point_sampling        BEVFormerEncoder.point_sampling        (modules/encoder.py:94-156) -- CUDA
                         kernel csrc/sca_glue.cu instead of a 61 MB repeat + batched matmul + masks
-  coords_to_voxel_grids / get_bev_grids / get_bev_grids_3d
-                        bevformer/utils/e2e_predictor_utils.py:36-45, 48-83
+  coords_to_voxel_grids / get_bev_grids / get_bev_grids_3d / bev_grids_to_coordinates / bev_coords_to_grids
+                        bevformer/utils/e2e_predictor_utils.py:8-45, 48-83
 Index/grid generation is plain torch on the target device (no arithmetic worth a kernel).
 """
 import copy
@@ -74,6 +74,26 @@ def coords_to_voxel_grids(ref_coords, bev_h, bev_w, pillar_num, pc_range):
     g[..., 1] = ((g[..., 1] - pc_range[1]) / (pc_range[4] - pc_range[1])) * bev_h
     g[..., 2] = ((g[..., 2] - pc_range[2]) / (pc_range[5] - pc_range[2])) * pillar_num
     return g
+
+
+def bev_grids_to_coordinates(ref_grids, pc_range):
+    """BEV grids in [0, 1] (x, y) -> metres."""
+    c = ref_grids.clone()
+    c[..., 0:1] = c[..., 0:1] * (pc_range[3] - pc_range[0]) + pc_range[0]
+    c[..., 1:2] = c[..., 1:2] * (pc_range[4] - pc_range[1]) + pc_range[1]
+    return c
+
+
+def bev_coords_to_grids(ref_coords, bev_h, bev_w, pc_range):
+    """Metres (x, y) -> (grids in [-1, 1], mask of the points inside the outermost cell centres)."""
+    g = ref_coords.clone()
+    g[..., 0] = (g[..., 0] - pc_range[0]) / (pc_range[3] - pc_range[0])
+    g[..., 1] = (g[..., 1] - pc_range[1]) / (pc_range[4] - pc_range[1])
+    g = g * 2 - 1.
+    x_min, x_max = 0.5 / bev_w * 2 - 1, (bev_w - 0.5) / bev_w * 2 - 1
+    y_min, y_max = 0.5 / bev_h * 2 - 1, (bev_h - 0.5) / bev_h * 2 - 1
+    valid = ((g[..., 0:1] > x_min) & (g[..., 0:1] < x_max) & (g[..., 1:2] > y_min) & (g[..., 1:2] < y_max))
+    return g, valid
 
 
 def get_bev_grids(H, W, bs=1, device="cuda", dtype=torch.float, offset=0.5):

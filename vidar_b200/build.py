@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvidar_b200.so")
 STAMP = os.path.join(HERE, ".libvidar_b200.stamp")
 
-SOURCES = ["core.cu", "msda.cu", "linear_tc.cu", "dvr.cu", "latent_render.cu", "latent_proj.cu", "ray_head.cu", "sca_glue.cu", "knn.cu", "eval_metrics.cu", "dense_chamfer.cu", "dcn.cu", "dcnv3.cu", "grid_mask.cu", "image_aug.cu", "point_pipeline.cu", "jpeg.cu", "grad_bucket.cu", "optim.cu"]
+SOURCES = ["core.cu", "msda.cu", "linear_tc.cu", "dvr.cu", "latent_render.cu", "latent_proj.cu", "ray_head.cu", "sca_glue.cu", "knn.cu", "eval_metrics.cu", "dense_chamfer.cu", "dcn.cu", "dcnv3.cu", "grid_mask.cu", "image_aug.cu", "point_pipeline.cu", "jpeg.cu", "grad_bucket.cu", "optim.cu", "bev_rotate.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -42,7 +42,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import bev_geometry, optim, sca, sharding, synthetic
+from . import bev_geometry, ego_motion as ego, optim, sca, sharding, synthetic
 from . import evaluate as eval_metrics
 from . import modules as _modules  # noqa: F401  (registers the attention classes)
 from . import image_aug
@@ -263,19 +263,22 @@ class DecoderLayer(nn.Module):
         return sharding.all_gather_rows(q[0], Q, group, grad="sum")[None]
 
 
-def run_decoder(layers, query, prev, bev_pos, ref, bev_shapes, bev_lsi, group=None):
+def run_decoder(layers, query, prev, bev_pos, ref, bev_shapes, bev_lsi, group=None, ref_points=None):
     """The future-BEV decoder stack -> (outputs of every layer stacked [inter, bs, Q, C] for the head, last output for
-    the next future frame).  `group`: row-sharded layers (`DecoderLayer.forward_rows`); the stacked outputs are then
-    (like the returned last output) views for replicated consumers (`sharding.replicated_view`)."""
+    the next future frame).  `ref` is the self-attention's reference points (tgt_points), `ref_points` the
+    cross-attention's in the previous frame (default: `ref`).  `group`: row-sharded layers
+    (`DecoderLayer.forward_rows`); the stacked outputs are then (like the returned last output) views for replicated
+    consumers (`sharding.replicated_view`)."""
     inter = []
+    ref_points = ref if ref_points is None else ref_points
     if group is None:
         for layer in layers:
-            query = layer(query, prev, bev_pos, ref, ref, bev_shapes, bev_lsi)
+            query = layer(query, prev, bev_pos, ref, ref_points, bev_shapes, bev_lsi)
             inter.append(query)
         return torch.stack(inter), inter[-1]
     query, prev, bev_pos = (sharding.sum_grad(t, group) for t in (query, prev, bev_pos))
     for layer in layers:
-        query = layer.forward_rows(query, prev, bev_pos, ref, ref, bev_shapes, bev_lsi, group)
+        query = layer.forward_rows(query, prev, bev_pos, ref, ref_points, bev_shapes, bev_lsi, group)
         inter.append(sharding.replicated_view(query, group))
     # the caller's use of the last output (next frame's `prev`, which passes through sum_grad again) is replicated too
     return torch.stack(inter), inter[-1]
@@ -339,15 +342,32 @@ class SyntheticViDAR(nn.Module):
         other draw of the step: A1's rand() (random_drop_image_rate is 0 in every config, so it only consumes the
         draw), A2's rand() and randint, then the supervised future frame.  None (the default) draws only when a
         drop rate or `supervise_all_future=False` needs it.  Under a process group every rank of a shard group must
-        seed numpy alike (as for GridMask) so that they draw the same drop index and future frame."""
+        seed numpy alike (as for GridMask) so that they draw the same drop index and future frame.
+
+    `ego_motion=True` aligns the graph to a moving ego vehicle as the nuScenes configs do (rotate_prev_bev, use_shift,
+    use_can_bus; `vidar_b200.ego_motion`).  Each image frame's metas then carry union2one's pose fields
+    (`ego_motion.queue_metas`: a `SampleLoader` sample has them, the tensor path takes them as `pose_metas`), and:
+      * the encoder embeds the frame's own can_bus, drops the previous BEV where prev_bev_exists is False, shifts the
+        first half of TSA's hybrid reference points by the ego translation and rotates the previous BEV by the yaw
+        change, straight into TSA's value (`ego_motion.rotate_stack`);
+      * TSA's value follows BEVFormerEncoder / CustomBEVFormerEncoder (encoder.py:210-243): [aligned previous BEV,
+        the initial query] from the first layer on, restacked with the LatentRendering layer's output after it
+        (without a previous BEV the value is the layer input twice, as TSA builds it);
+      * each future roll-out's cross-attention samples the previous frame at the target grid moved into its
+        coordinates (`_align_bev_coordnates`), and `future_can_bus_mlp` is the head's Linear(4, 128), ReLU,
+        Linear(128, 256), ReLU, LayerNorm over future_can_bus[k][:, (0, 1, 2, 17)].
+    The default False keeps the graph, the state_dict and the draws as they were: the can_bus is the one passed in
+    (zeros by default) for every frame, nothing is shifted or rotated, and TSA's value is [previous BEV or layer
+    input, layer input] at every layer.  The row-sharded encoder does not support it."""
 
     def __init__(self, num_cams=6, encoder_layers=6, decoder_layers=3, future_frames=3, history_frames=3,
                  latent_layer=2, bev_hw=(BEV_H, BEV_W), ray_grid_num=512, dcn=False, backbone_autocast=None,
                  grid_mask=False, image_pipeline=False, point_pipeline=False, backward_history_frames=0,
                  drop_prev_rate=0.0, drop_prev_end_idx=None, supervise_all_future=True, head_history_frames=None,
                  head_future_frames=1, per_frame_loss_weight=None, frame_loss_weight=None, latent_grid_step=0.5,
-                 point_voxel_size=1.0, reference_draws=None):
+                 point_voxel_size=1.0, reference_draws=None, ego_motion=False):
         super().__init__()
+        self.ego_motion = bool(ego_motion)
         if backward_history_frames not in (0, 1):
             raise ValueError(f"backward_history_frames must be 0 or 1 (got {backward_history_frames})")
         if future_frames < 0 or decoder_layers < 0 or (future_frames > 0 and decoder_layers == 0):
@@ -390,7 +410,8 @@ class SyntheticViDAR(nn.Module):
             self.future_bev_embedding = nn.Embedding(BEV_H * BEV_W, EMBED)
             self.future_positional_encoding = LearnedPositionalEncoding(BEV_H, BEV_W)
             self.prev_frame_embedding = nn.Parameter(torch.randn(1, EMBED))
-            self.future_can_bus_mlp = nn.Sequential(nn.Linear(18, EMBED // 2), nn.ReLU(inplace=True),
+            self.future_can_bus_mlp = nn.Sequential(nn.Linear(len(ego.CAN_BUS_DIMS) if self.ego_motion else 18, EMBED // 2),
+                                                    nn.ReLU(inplace=True),
                                                     nn.Linear(EMBED // 2, EMBED), nn.ReLU(inplace=True),
                                                     nn.LayerNorm(EMBED))
         self.decoder = nn.ModuleList([DecoderLayer() for _ in range(decoder_layers if future_frames > 0 else 0)])
@@ -420,6 +441,8 @@ class SyntheticViDAR(nn.Module):
         `row_sharded=True` additionally runs every row-wise stage of the encoder (TSA, norms, FFN) on the rank's
         block of BEV rows (`EncoderLayer.forward_rows`; bs = 1, rows divisible by the group size)."""
         import torch.distributed as dist
+        if row_sharded and self.ego_motion:
+            raise ValueError("set_process_group: the row-sharded encoder does not support ego_motion=True")
         self.process_group = group
         self.row_sharded = bool(row_sharded) and group is not None and dist.get_world_size(group) > 1
         world = dist.get_world_size(group) if group is not None else 1
@@ -526,9 +549,12 @@ class SyntheticViDAR(nn.Module):
 
     # ---- BEV encoder (transformer.py:102-193 + encoder.py:159-253) ----
     def encode(self, feats, spatial_shapes, lsi, img_metas, can_bus, prev_bev):
+        """One frame's BEV.  With `ego_motion`, `can_bus` is not read: the frame's own comes from img_metas."""
         bs = feats.shape[2]
         dev = feats.device
         BEV_H, BEV_W = self.bev_h, self.bev_w          # noqa: N806
+        if self.ego_motion:
+            return self._encode_ego(feats, spatial_shapes, lsi, img_metas, prev_bev)
         bev_pos = self.positional_encoding(bs)
         query = self.bev_embedding.weight[None].expand(bs, -1, -1) + self.can_bus_mlp(can_bus)[:, None]
         ref_3d = bev_geometry.get_reference_points(BEV_H, BEV_W, PC_RANGE[5] - PC_RANGE[2], 4, dim="3d", bs=bs, device=dev)
@@ -556,8 +582,49 @@ class SyntheticViDAR(nn.Module):
                 query = layer(query, feats, bev_pos, hybrid, pv, spatial_shapes, lsi, ref_cam, bev_mask, bev_shapes, bev_lsi)
         return query
 
+    def _encode_ego(self, feats, spatial_shapes, lsi, img_metas, prev_bev):
+        """`encode` with ego motion (transformer.py:114-157, encoder.py:196-243): the frame's can_bus, the scene cut,
+        the shifted hybrid reference points, and TSA's value [rotated previous BEV, initial query], restacked after
+        the LatentRendering layer.  The host values (can_bus, shift) are uploaded pinned, without blocking."""
+        ego.require_metas(img_metas)
+        bs = feats.shape[2]
+        dev = feats.device
+        BEV_H, BEV_W = self.bev_h, self.bev_w          # noqa: N806
+        Q = BEV_H * BEV_W
+        if not img_metas[0]["prev_bev_exists"]:                                  # bevformer.py:177, vidar.py:280
+            prev_bev = None
+        host = np.concatenate([np.array([m["can_bus"] for m in img_metas], np.float64),
+                               ego.bev_shift(img_metas, BEV_H, BEV_W)], 1)
+        host = ego.upload(host, dev, self.bev_embedding.weight.dtype)            # [bs, 18 + 2]: can_bus, shift x / y
+        can_bus, shift = host[:, :18], host[:, 18:]
+        bev_pos = self.positional_encoding(bs)
+        query = self.bev_embedding.weight[None].expand(bs, -1, -1) + self.can_bus_mlp(can_bus)[:, None]
+        ref_3d = bev_geometry.get_reference_points(BEV_H, BEV_W, PC_RANGE[5] - PC_RANGE[2], 4, dim="3d", bs=bs, device=dev)
+        ref_2d = bev_geometry.get_reference_points(BEV_H, BEV_W, dim="2d", bs=bs, device=dev)
+        ref_cam, bev_mask = bev_geometry.point_sampling(ref_3d, PC_RANGE, img_metas)
+        bev_shapes = torch.tensor([[BEV_H, BEV_W]], device=dev)
+        bev_lsi = torch.tensor([0], device=dev)
+        value = None
+        if prev_bev is not None:
+            shift_ref_2d = ref_2d + shift[:, None, None, :]
+            hybrid = torch.stack([shift_ref_2d, ref_2d], 1).reshape(bs * 2, Q, 1, 2)
+            rows = ego.rotation_rows([m["can_bus"][-1] for m in img_metas], BEV_H, BEV_W, dev)
+            value = ego.rotate_stack(prev_bev, query, rows)                      # [bs * 2, Q, C]
+        else:
+            hybrid = torch.stack([ref_2d, ref_2d], 1).reshape(bs * 2, Q, 1, 2)
+        for layer in self.encoder:
+            pv = value if value is not None else torch.stack([query, query], 1).reshape(bs * 2, Q, EMBED)
+            query = layer(query, feats, bev_pos, hybrid, pv, spatial_shapes, lsi, ref_cam, bev_mask, bev_shapes, bev_lsi)
+            if value is not None and layer.latent_render is not None:            # encoder.py:238-243
+                value = torch.stack([value.view(bs, 2, Q, EMBED)[:, 0], query], 1).reshape(bs * 2, Q, EMBED)
+        return query
+
     # ---- future decoder (vidar_head_base.py:125-173) ----
-    def decode_future(self, prev_bev_input, future_can_bus):
+    def decode_future(self, prev_bev_input, future_can_bus, ref_points=None):
+        """One future roll-out.  With `ego_motion`: `future_can_bus` [bs, 4] is the target frame's future_can_bus at
+        the head's can_bus_dims and `ref_points` [bs, Q, 1, 2] the target grid in the previous frame
+        (`ego_motion.future_grids`), the cross-attention's reference points; the self-attention keeps the target
+        grid."""
         if not len(self.decoder):
             raise RuntimeError("decode_future: the model was built with future_frames=0 and has no future decoder")
         bs = prev_bev_input.shape[0]
@@ -573,7 +640,8 @@ class SyntheticViDAR(nn.Module):
         if rows_mode and (bs != 1 or query.shape[1] % torch.distributed.get_world_size(self.process_group) != 0):
             raise RuntimeError("row-sharded decoder: needs bs == 1 and BEV rows divisible by the group size")
         # -> ([inter, bs, Q, C] for the head, the last layer's output for the next future frame)
-        return run_decoder(self.decoder, query, prev, bev_pos, ref, bev_shapes, bev_lsi, self.process_group if rows_mode else None)
+        return run_decoder(self.decoder, query, prev, bev_pos, ref, bev_shapes, bev_lsi, self.process_group if rows_mode else None,
+                           ref_points=ref_points)
 
     def forward_head(self, next_bev_feats):
         """vidar_head_v1.py:64-92: [frames, inter, bs, Q, C] -> [frames, inter, pred_frame, bs, Q, heights]."""
@@ -601,7 +669,7 @@ class SyntheticViDAR(nn.Module):
                  lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]]) for t in range(img.shape[1])])
 
     def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None, train=False,
-                        drop_prev_index=-1, supervised=None, img_metas=None, feature_cache=None):
+                        drop_prev_index=-1, supervised=None, img_metas=None, feature_cache=None, pose_metas=None):
         """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + len(supervised), inter, pred_frame, bs, Q, 16]: the
         history BEV of the first T - 1 frames, the current frame's BEV as ref_bev, `future_frames` roll-outs with a
         queue of length 1 -- those not in `supervised` (default: all) under no_grad --, then the head over the current
@@ -621,7 +689,10 @@ class SyntheticViDAR(nn.Module):
         frame whose camera files were a frame of the previous call's sample takes that frame's stored extract_feat
         output (feats, spatial_shapes, level_start_index) instead of running the backbone again; on return the dict
         holds this sample's frames only.  A frame masked by a GridMask draw is always computed and never stored.  The
-        GridMask draws are made as without the cache."""
+        GridMask draws are made as without the cache.
+
+        `pose_metas` (with `ego_motion`, for the tensor path): one dict per image frame, `ego_motion.queue_metas`' (bs
+        1), merged into each frame's metas; a `SampleLoader` sample's img_metas carry them already."""
         loaded = img_metas is not None
         if feature_cache is not None and (not loaded or any("filename" not in m[0] for m in img_metas)):
             raise ValueError("_next_bev_preds: feature_cache needs a test-mode SampleLoader sample (img_metas with "
@@ -643,6 +714,15 @@ class SyntheticViDAR(nn.Module):
             metas = [[dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)])
                       for b in range(bs)]] * T
             hw = img.shape[-2:]
+        if pose_metas is not None:
+            if len(pose_metas) != T or bs != 1:
+                raise ValueError(f"_next_bev_preds: pose_metas needs bs 1 and one dict per image frame ({T} frames, "
+                                 f"bs {bs}, got {len(pose_metas)})")
+            metas = [[dict(m[0], **p)] for m, p in zip(metas, pose_metas)]
+        if self.ego_motion:
+            for m in metas:
+                ego.require_metas(m)
+            ego.require_metas(metas[T - 1], future_frames)
         backwarded = min(self.backward_history_frames, T - 1) if train else 0
         frozen = T - 1 - backwarded
         fresh = None if feature_cache is None else {}
@@ -685,13 +765,27 @@ class SyntheticViDAR(nn.Module):
         inter_num = len(self.bev_pred_head)
         next_bev_feats = [ref_bev.unsqueeze(0).repeat(inter_num, 1, 1, 1)]
         prev_bev_input = ref_bev.unsqueeze(1)
+        future_inputs = [(can_bus, None)] * future_frames
+        if self.ego_motion and future_frames:                                        # vidar.py:319-363
+            cur = metas[T - 1]
+            fcb = np.array([[m["future_can_bus"][k][list(ego.CAN_BUS_DIMS)] for m in cur]
+                            for k in range(1, future_frames + 1)], np.float64)       # [F, bs, 4]
+            f2r, r2h = ego.future_matrices(cur, future_frames)                       # [F, bs, 4, 4] each
+            host = ego.upload(np.concatenate([fcb.reshape(-1), f2r.reshape(-1), r2h.reshape(-1)]), dev,
+                              self.bev_embedding.weight.dtype)
+            n4, n16 = fcb.size, f2r.size
+            fcb, f2r, r2h = (host[:n4].view(fcb.shape), host[n4:n4 + n16].view(f2r.shape),
+                             host[n4 + n16:].view(r2h.shape))
+            mats = torch.matmul(f2r, r2h)                                            # fp32 on the device, as vidar.py:215
+            future_inputs = [(fcb[k], ego.future_grids(mats[k], self.bev_h, self.bev_w, PC_RANGE))
+                             for k in range(future_frames)]
         for k in range(1, future_frames + 1):
             if supervised is None or k in supervised:
-                pred_feat, last = self.decode_future(prev_bev_input, can_bus)
+                pred_feat, last = self.decode_future(prev_bev_input, *future_inputs[k - 1])
                 next_bev_feats.append(pred_feat)
             else:
                 with torch.no_grad():
-                    _, last = self.decode_future(prev_bev_input, can_bus)
+                    _, last = self.decode_future(prev_bev_input, *future_inputs[k - 1])
             prev_bev_input = last.unsqueeze(1)                                         # queue length 1 (vidar.py:359-360)
         self._mark("future_decoder")
         next_bev_feats = torch.stack(next_bev_feats, 0)
@@ -726,7 +820,7 @@ class SyntheticViDAR(nn.Module):
 
     # ---- one training forward (vidar.py:239-387) -> dict of losses ----
     def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None, point_infos=None,
-                      draws=None, img_metas=None):
+                      draws=None, img_metas=None, pose_metas=None):
         """img [bs, T, cams, 3, H, W] (T-1 history frames + current), lidar2img: host array [bs, cams, 4, 4]
         (it lives in `img_metas` in the reference), gt_points: list over batch of [M, 4] (x, y, z metric,
         frame index 0 = current .. future_frames).  With the image pipeline: img uint8 [1, T, cams, H, W, 3] and
@@ -736,7 +830,8 @@ class SyntheticViDAR(nn.Module):
 
         A `SampleLoader` sample instead: `img_metas` given, img the list of the T frames' pipelined images of this
         rank's backbone cameras and gt_points its device [1, R, 5]; the transforms ran in the loader, so neither
-        pipeline runs here and lidar2img, cam2img, lidar2cam and point_infos are not read."""
+        pipeline runs here and lidar2img, cam2img, lidar2cam and point_infos are not read.  `pose_metas`: see
+        `_next_bev_preds` (ego_motion)."""
         loaded = img_metas is not None
         num_frames = len(img) if loaded else img.shape[1]
         drop_prev_index, supervised = self.host_draws(num_frames) if draws is None else draws
@@ -744,7 +839,7 @@ class SyntheticViDAR(nn.Module):
             gt_points = self.gt_points_of(point_infos, True)
         next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, self.future_frames, cam2img, lidar2cam,
                                               train=self.training, drop_prev_index=drop_prev_index,
-                                              supervised=supervised, img_metas=img_metas)
+                                              supervised=supervised, img_metas=img_metas, pose_metas=pose_metas)
         valid_frames = [0] + (list(range(1, 1 + self.future_frames)) if supervised is None else list(supervised))
         fw = self.frame_loss_weight
         losses = {}
@@ -765,16 +860,17 @@ class SyntheticViDAR(nn.Module):
 
     # ---- inference (vidar.py:389-502) ----
     @torch.no_grad()
-    def predict_future(self, img, lidar2img, future_frames, can_bus=None, img_metas=None, feature_cache=None):
+    def predict_future(self, img, lidar2img, future_frames, can_bus=None, img_metas=None, feature_cache=None,
+                       pose_metas=None):
         """forward_test's prediction (vidar.py:392-437): the same inputs as forward_train, `future_frames` roll-outs
         (the reference's test_future_frame_num) -> pred_dict {next_bev_preds [1 + future_frames, inter, pred_frame,
-        bs, Q, 16], valid_frames [0 .. future_frames]}.  `feature_cache`: see `_next_bev_preds`."""
+        bs, Q, 16], valid_frames [0 .. future_frames]}.  `feature_cache`, `pose_metas`: see `_next_bev_preds`."""
         next_bev_preds = self._next_bev_preds(img, lidar2img, can_bus, future_frames, img_metas=img_metas,
-                                              feature_cache=feature_cache)
+                                              feature_cache=feature_cache, pose_metas=pose_metas)
         return dict(next_bev_preds=next_bev_preds, valid_frames=list(range(1 + future_frames)))
 
     def forward_test(self, img, lidar2img, gt_points, future_frames=6, can_bus=None, point_infos=None,
-                     img_metas=None):
+                     img_metas=None, pose_metas=None):
         """vidar.py:389-502 without submission writing and visualisation -> [ret_dict], ret_dict =
         {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}} for the current frame (t = 0) and every
         future frame, scored on the current head frame (`head_history_frames`) by ray_head.evaluate (one batched device
@@ -784,7 +880,8 @@ class SyntheticViDAR(nn.Module):
         gt_points went through the loader's train transforms, which this path then scores as they are."""
         if self.point_transforms is not None and img_metas is None:
             gt_points = self.gt_points_of(point_infos, False)
-        pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus, img_metas=img_metas)
+        pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus, img_metas=img_metas,
+                                        pose_metas=pose_metas)
         cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.head_history_frames])
         with torch.no_grad():
             ret = self.ray_head.evaluate(cur, gt_points, 0, self.bev_h, self.bev_w, PC_RANGE)
@@ -795,7 +892,8 @@ class SyntheticViDAR(nn.Module):
 # synthetic sample + step
 # ------------------------------------------------------------------------------------------------
 def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000, future_frames=3, seed=0,
-                     bev_hw=(BEV_H, BEV_W), raw_images=False, raw_points=False, points_per_frame=35000, files=False):
+                     bev_hw=(BEV_H, BEV_W), raw_images=False, raw_points=False, points_per_frame=35000, files=False,
+                     poses=False, scene_change=None):
     """6 x 3 x 928 x 1600 N(0,1) frames, a nuScenes-like rig, LiDAR-like future point clouds (SURVEY.md 8d cfg4).
     `raw_images=True` (for `SyntheticViDAR(image_pipeline=True)`): seeded uniform uint8 BGR frames
     [1, frames, cams, 900, 1600, 3] (img_hw defaults to the camera size) and the rig's host `cam2img` / `lidar2cam`
@@ -808,9 +906,13 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000
     hands them to its pipeline, one per queue frame, oldest first: the `frames` image frames (the history and the
     current one) with `img_filename`, `cam2img` and `lidar2cam`, the current and the future frames with the point
     infos of `raw_points`.  Each camera image is a baseline 4:2:0 JPEG written by cv2.imwrite at quality
-    `JPEG_QUALITY` (img_hw defaults to 900 x 1600), to a temporary directory removed at exit.  `device` is not used."""
+    `JPEG_QUALITY` (img_hw defaults to 900 x 1600), to a temporary directory removed at exit.  `device` is not used.
+    `poses=True` (for `SyntheticViDAR(ego_motion=True)`): the queue frames follow a seeded drive (`synthetic.drive`,
+    `scene_change` = the first frame of a second scene): with `files`, every queue frame carries its pose fields;
+    otherwise the sample holds `pose_metas`, `ego_motion.queue_metas` of the frames + future_frames drive."""
     if files:
-        return synthetic_queue(frames, cams, img_hw or (900, 1600), future_frames, points_per_frame, seed)
+        return synthetic_queue(frames, cams, img_hw or (900, 1600), future_frames, points_per_frame, seed,
+                               poses=poses, scene_change=scene_change)
     g = torch.Generator(device=device).manual_seed(seed)
     extra = {}
     if raw_images:
@@ -834,6 +936,9 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000
     pts.append(torch.from_numpy(np.concatenate([xyz, tindex[0][:, None]], -1).astype(np.float32)).to(device))
     if raw_points:
         extra["point_infos"] = synthetic_point_infos(1 + future_frames, points_per_frame, seed)
+    if poses:
+        drive = synthetic.drive(frames + future_frames, seed, scene_change)
+        extra["pose_metas"] = ego.queue_metas([dict(p, img_filename=()) for p in drive[:frames]] + drive[frames:])
     return dict(img=img, lidar2img=lidar2img, gt_points=pts, **extra)
 
 
@@ -850,9 +955,11 @@ def _temp_dir(prefix):
     return root
 
 
-def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=0, first_gt=None):
+def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=0, first_gt=None, poses=False,
+                    scene_change=None):
     """`synthetic_sample(..., files=True)`: image frames 0 .. frames - 1, point frames first_gt (default frames - 1)
-    .. frames - 1 + future_frames, every frame with the same rig."""
+    .. frames - 1 + future_frames, every frame with the same rig.  `poses`: frame t also carries the pose fields of
+    drive frame t (`synthetic.drive(..., scene_change)`); the default leaves the queue as without them."""
     first_gt = frames - 1 if first_gt is None else first_gt
     import cv2
     root = _temp_dir("vidar_cameras_")
@@ -875,24 +982,32 @@ def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=
             queue[first_gt + k].update(info)
         else:
             queue.append(info)
+    if poses:
+        for f, p in zip(queue, synthetic.drive(len(queue), seed, scene_change)):
+            f.update(p)
     return queue
 
 
-def synthetic_scene(num_samples, frames, future_frames, cams=6, img_hw=(900, 1600), points_per_frame=35000, seed=0):
+def synthetic_scene(num_samples, frames, future_frames, cams=6, img_hw=(900, 1600), points_per_frame=35000, seed=0,
+                    poses=False):
     """One scene's files, written once (`synthetic_queue`), as the sliding-window queues a test dataset builds from
     consecutive keyframes (no load_frame_interval): sample i's image frames are the scene's frames i .. i + frames - 1
     (the history and the current frame), its GT frames i + frames - 1 .. i + frames - 1 + future_frames.  Each image
     frame carries `img_filename`, `cam2img`, `lidar2cam` and the test pipeline's `lidar2img` = cam2img @ lidar2cam
     (float64), so the queues serve the test-mode and the train-mode `SampleLoader` alike.  Neighbouring samples share
-    frames - 1 image frames' files.  -> [queue] of num_samples queues."""
+    frames - 1 image frames' files.  `poses`: every frame carries its pose fields of one drive over the scene
+    (`synthetic.drive`).  -> [queue] of num_samples queues."""
     if num_samples < 1 or frames < 1 or future_frames < 0:
         raise ValueError(f"synthetic_scene: num_samples, frames >= 1 and future_frames >= 0 "
                          f"(got {num_samples}, {frames}, {future_frames})")
     total = num_samples + frames - 1
-    scene = synthetic_queue(total, cams, img_hw, future_frames, points_per_frame, seed, first_gt=frames - 1)
+    scene = synthetic_queue(total, cams, img_hw, future_frames, points_per_frame, seed, first_gt=frames - 1,
+                            poses=poses)
+    pose = ego.POSE_KEYS if poses else ()
     images = [dict(img_filename=list(f["img_filename"]), cam2img=f["cam2img"], lidar2cam=f["lidar2cam"],
-                   lidar2img=[c @ l for c, l in zip(f["cam2img"], f["lidar2cam"])]) for f in scene[:total]]
-    gts = [{k: f[k] for k in ("pts_filename", "timestamp", "sweeps")} for f in scene if "pts_filename" in f]
+                   lidar2img=[c @ l for c, l in zip(f["cam2img"], f["lidar2cam"])], **{k: f[k] for k in pose})
+              for f in scene[:total]]
+    gts = [{k: f[k] for k in ("pts_filename", "timestamp", "sweeps") + pose} for f in scene if "pts_filename" in f]
     queues = []
     for i in range(num_samples):
         queue = [dict(images[t]) for t in range(i, i + frames)]
@@ -937,7 +1052,8 @@ def train_step(model, optimizer, sample, group=None, record=False, scaler=None, 
     optimizer.zero_grad(set_to_none=True)
     losses = model.forward_train(sample["img"], sample["lidar2img"], sample["gt_points"], can_bus=sample.get("can_bus"),
                                  cam2img=sample.get("cam2img"), lidar2cam=sample.get("lidar2cam"),
-                                 point_infos=sample.get("point_infos"), img_metas=sample.get("img_metas"))
+                                 point_infos=sample.get("point_infos"), img_metas=sample.get("img_metas"),
+                                 pose_metas=sample.get("pose_metas"))
     loss = sum(losses.values())
     (loss if scaler is None else scaler.scale(loss)).backward()
     model._mark("backward")

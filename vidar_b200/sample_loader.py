@@ -39,7 +39,7 @@ import random
 import numpy as np
 import torch
 
-from . import image_aug, jpeg
+from . import ego_motion, image_aug, jpeg
 
 
 def run_image_transforms(transforms, frames):
@@ -71,10 +71,12 @@ class QueueDataset(torch.utils.data.Dataset):
     """The host half of a sample: `samples[i]` is a queue of results dicts; frames with `img_filename` are the image
     frames, frames with `pts_filename` the GT frames.  -> dict(frames=[image results], points=[point results],
     index=i).  Makes no CUDA call.  `test_mode`: an image frame brings its `lidar2img` (the test chain does not form
-    it) instead of `cam2img` and `lidar2cam`."""
+    it) instead of `cam2img` and `lidar2cam`.  `poses`: every frame brings its pose fields, and the result also holds
+    poses=[metas per image frame] (`ego_motion.queue_metas`)."""
 
-    def __init__(self, samples, image_transforms, point_transforms, test_mode=False):
+    def __init__(self, samples, image_transforms, point_transforms, test_mode=False, poses=False):
         self.samples = list(samples)
+        self.poses = bool(poses)
         self.image_transforms = list(image_transforms)
         self.point_transforms = list(point_transforms)
         self.test_mode = bool(test_mode)
@@ -96,7 +98,9 @@ class QueueDataset(torch.utils.data.Dataset):
                                                     **{k: [np.array(m, np.float64) for m in f[k]] for k in keys})))
         if not frames or not points:
             raise ValueError(f"sample {index}: a queue needs image frames (img_filename) and GT frames (pts_filename)")
-        return dict(frames=run_image_transforms(self.image_transforms, frames), points=points, index=index)
+        poses = ego_motion.queue_metas(queue) if self.poses else None
+        return dict(frames=run_image_transforms(self.image_transforms, frames), points=points, index=index,
+                    poses=poses)
 
 
 def seed_worker(worker_id, num_workers, rank, seed):
@@ -128,7 +132,9 @@ class SampleLoader:
     `num_workers`: DataLoader worker processes (0: the host half on this process).  `prefetch`: samples whose device
     half runs ahead on a side stream (0: on the current stream, at hand-out).  `seed` and `rank` seed the workers;
     `rank` is the data-parallel replica (`grid.replica`): every rank of a shard group passes the same value and
-    iterates the same samples, so their draws agree, and each decodes only its own backbone cameras."""
+    iterates the same samples, so their draws agree, and each decodes only its own backbone cameras.
+    A model built with ego_motion=True needs every queue frame's pose fields (`ego_motion.POSE_KEYS`); the workers
+    then run `ego_motion.queue_metas` on the queue and each image frame's img_metas carry its result."""
 
     def __init__(self, model, samples, num_workers=0, prefetch=1, seed=0, rank=0, test_mode=False):
         if test_mode and model.point_transforms is None:
@@ -140,9 +146,11 @@ class SampleLoader:
         self.model, self.prefetch, self.num_workers = model, int(prefetch), int(num_workers)
         self.test_mode = bool(test_mode)
         if test_mode:
-            self.dataset = QueueDataset(samples, image_aug.config_test_pipeline(), model.point_transforms[1], True)
+            self.dataset = QueueDataset(samples, image_aug.config_test_pipeline(), model.point_transforms[1], True,
+                                        poses=getattr(model, "ego_motion", False))
         else:
-            self.dataset = QueueDataset(samples, model.image_transforms, model.point_transforms[0])
+            self.dataset = QueueDataset(samples, model.image_transforms, model.point_transforms[0],
+                                        poses=getattr(model, "ego_motion", False))
         init = functools.partial(seed_worker, num_workers=num_workers, rank=rank, seed=seed) if num_workers else None
         self.host_loader = torch.utils.data.DataLoader(self.dataset, batch_size=None, shuffle=False,
                                                        num_workers=num_workers, collate_fn=_one, worker_init_fn=init)
@@ -162,8 +170,10 @@ class SampleLoader:
             img = [image_aug.apply_multiview(raw, r, cams) for r, raw in zip(frames, decoded)]
         else:
             img = [torch.empty((0, 3, *r["img_aug"].pad_hw), dtype=torch.float32, device=dev) for r in frames]
+        poses = host.get("poses") or [{}] * len(frames)
         metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"],
-                       **(dict(filename=list(r["filename"])) if self.test_mode else {}))] for r in frames]
+                       **(dict(filename=list(r["filename"])) if self.test_mode else {}), **p)]
+                 for r, p in zip(frames, poses)]
         return dict(img=img, img_metas=metas, gt_points=model.gather_points(host["points"]), lidar2img=None,
                     index=host["index"])
 

@@ -165,3 +165,40 @@ def sweep_pose(rng, k):
     R = np.array([[cz, -sz, 0.0], [sz, cz, 0.0], [0.0, 0.0, 1.0]]) @ np.array([[1.0, 0, 0], [0, cr, -sr], [0, sr, cr]])
     t = np.array([-0.5 * k + rng.normal(0, 0.02), rng.normal(0, 0.02), rng.normal(0, 0.01)])
     return R, t
+
+
+LIDAR2EGO_TRANSLATION = [0.943713, 0.0, 1.84023]                          # nuScenes' roof LiDAR mounting
+LIDAR2EGO_ROTATION = [0.7077955119163518, -0.006492242056004365, 0.010646214713995808, -0.7063073142877817]
+
+
+def drive(frames, seed=0, scene_change=None, dt=0.5):
+    """A seeded nuScenes-like drive of `frames` keyframes `dt` s apart -> one pose dict per frame (the dataset's info
+    fields): ego2global_translation / rotation (w, x, y, z), lidar2ego_translation / rotation, an 18-value can_bus
+    (position, orientation, acceleration, rotation rate, velocity, two zeros, as nuScenes' CAN bus pose message) and
+    scene_token.  Speed up to about 15 m/s and yaw rate within +-10 deg/s, with small pitch / roll.
+    `scene_change` = i: frames i .. end belong to another scene, starting elsewhere on the map."""
+    rng = np.random.default_rng(seed + 7919)
+    out = []
+    pos, yaw, scene = rng.uniform(300, 1500, 3) * np.array([1, 1, 0]), rng.uniform(-np.pi, np.pi), 0
+    speed = rng.uniform(0, 15)
+    for t in range(frames):
+        if scene_change is not None and t == scene_change:
+            pos, yaw, scene = rng.uniform(300, 1500, 3) * np.array([1, 1, 0]), rng.uniform(-np.pi, np.pi), 1
+            speed = rng.uniform(0, 15)
+        elif t > 0:
+            rate = np.deg2rad(rng.uniform(-10, 10))
+            accel = rng.uniform(-2, 2)
+            speed = float(np.clip(speed + accel * dt, 0, 15))
+            yaw += rate * dt
+            pos = pos + speed * dt * np.array([np.cos(yaw), np.sin(yaw), 0.0])
+        pitch, roll = rng.normal(0, 0.01), rng.normal(0, 0.005)
+        cy, sy, cp, sp, cr, sr = (np.cos(yaw / 2), np.sin(yaw / 2), np.cos(pitch / 2), np.sin(pitch / 2),
+                                  np.cos(roll / 2), np.sin(roll / 2))
+        q = [cr * cp * cy + sr * sp * sy, sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy,
+             cr * cp * sy - sr * sp * cy]
+        can_bus = np.concatenate([pos, q, rng.normal(0, 0.5, 3), rng.normal(0, 0.05, 3), [speed, 0.0, 0.0],
+                                  [0.0, 0.0]])
+        out.append(dict(ego2global_translation=[float(v) for v in pos], ego2global_rotation=[float(v) for v in q],
+                        lidar2ego_translation=list(LIDAR2EGO_TRANSLATION), lidar2ego_rotation=list(LIDAR2EGO_ROTATION),
+                        can_bus=can_bus, scene_token=f"synthetic-{seed}-{scene}"))
+    return out
