@@ -129,3 +129,18 @@ def test_sharded_pretraining_graph_equals_single_process(tmp_path, world):
                 assert gr[n] is not None, (rank, row_sharded, n)
                 torch.testing.assert_close(gr[n], g, rtol=1e-6, atol=1e-8 * scale[n] + 1e-16,
                                            msg=lambda m_: f"world {world} rank {rank} rows {row_sharded} grad {n}: {m_}")
+
+
+def test_model_as_constructed_runs_every_camera_on_one_rank():
+    """A `SyntheticViDAR` used without `set_process_group` has the layout of no group: its backbone runs every
+    camera and every camera's features are filled."""
+    from vidar_b200 import pretrain
+    torch.manual_seed(0)
+    m = pretrain.SyntheticViDAR(num_cams=2, encoder_layers=1, decoder_layers=1, future_frames=1, history_frames=1,
+                                latent_layer=-1, bev_hw=(8, 8), ray_grid_num=16)
+    assert m.backbone_cams() == [0, 1]
+    with torch.no_grad():
+        feats, shapes, lsi = m.extract_feat(torch.randn(1, 2, 3, *IMG))
+    assert shapes.tolist() == [[8, 12], [4, 6], [2, 3], [1, 2]] and lsi.tolist() == [0, 96, 120, 126]
+    assert feats.shape == (2, 128, 1, 256)
+    assert all(feats[c].abs().sum() > 0 for c in range(2))

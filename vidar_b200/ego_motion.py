@@ -23,7 +23,8 @@ Device:
   * `rotate_stack`: TSA's value [bs * 2, Q, C] = [rotated previous BEV, query] in one kernel (csrc/bev_rotate.cu,
     include/vidar_b200.h §xv), with a deterministic backward;
   * `future_grids`: `_align_bev_coordnates` (detectors/vidar.py:196-238): each future frame's BEV grid moved into
-    the previous frame's coordinates.
+    the previous frame's coordinates;
+  * `future_inputs`: every future roll-out's can_bus and moved grid from the current frame's metas.
 Every host-made value reaches the device through a pinned, non-blocking upload: no host sync.
 """
 import copy
@@ -354,3 +355,18 @@ def future_grids(matrices, bev_h, bev_w, pc_range):
     aligned = torch.matmul(coords, matrices)[..., :2]
     aligned, _ = bev_geometry.bev_coords_to_grids(aligned, bev_h, bev_w, pc_range)
     return ((aligned + 1) / 2.0).unsqueeze(2)
+
+
+def future_inputs(metas, future_frames, bev_h, bev_w, pc_range, device, dtype=torch.float32):
+    """The future decoder's inputs for roll-outs k = 1 .. future_frames from the current frame's `metas`
+    (detectors/vidar.py:319-363) -> [(future_can_bus [bs, 4] at CAN_BUS_DIMS, ref_points [bs, Q, 1, 2] = `future_grids`
+    of `future_matrices`' product)], one per roll-out.  The host values go up in one pinned upload in `dtype`; the
+    product is formed on the device in `dtype` (the model's fp32, as vidar.py:215 forms it)."""
+    fcb = np.array([[m["future_can_bus"][k][list(CAN_BUS_DIMS)] for m in metas]
+                    for k in range(1, future_frames + 1)], np.float64)               # [F, bs, 4]
+    f2r, r2h = future_matrices(metas, future_frames)                                  # [F, bs, 4, 4] each
+    host = upload(np.concatenate([fcb.reshape(-1), f2r.reshape(-1), r2h.reshape(-1)]), device, dtype)
+    n4, n16 = fcb.size, f2r.size
+    fcb, f2r, r2h = host[:n4].view(fcb.shape), host[n4:n4 + n16].view(f2r.shape), host[n4 + n16:].view(r2h.shape)
+    mats = torch.matmul(f2r, r2h)
+    return [(fcb[k], future_grids(mats[k], bev_h, bev_w, pc_range)) for k in range(future_frames)]

@@ -431,30 +431,32 @@ class SyntheticViDAR(nn.Module):
             self.per_frame_loss_weight = tuple(float(w) for w in per_frame_loss_weight)
             if len(self.per_frame_loss_weight) != self.pred_frame_num:
                 raise ValueError(f"per_frame_loss_weight: {self.pred_frame_num} head frames, got {per_frame_loss_weight}")
-        self.process_group = None
-        self.row_sharded = False
         self.timings = None
+        self.set_process_group(None)
 
     # ---- sharding ------------------------------------------------------------------------------
     def set_process_group(self, group, row_sharded=False):
         """Shard one sample over `group`: cameras (backbone, SpatialCrossAttention), cells (LatentRendering).
         `row_sharded=True` additionally runs every row-wise stage of the encoder (TSA, norms, FFN) on the rank's
-        block of BEV rows (`EncoderLayer.forward_rows`; bs = 1, rows divisible by the group size)."""
+        block of BEV rows (`EncoderLayer.forward_rows`; bs = 1, rows divisible by the group size).
+
+        Stores the layout the graph reads: `shard_size` / `shard_rank` (1 / 0 without a group), this rank's backbone
+        and SpatialCrossAttention cameras (`my_backbone_cams`, `my_sca_cams`: all of them on one rank), and the
+        groups and owners of the cameras shared by two ranks (`cam_groups`, `cam_src`: empty on one rank).
+        `__init__` sets the layout of no group."""
         import torch.distributed as dist
         if row_sharded and self.ego_motion:
             raise ValueError("set_process_group: the row-sharded encoder does not support ego_motion=True")
-        self.process_group = group
-        self.row_sharded = bool(row_sharded) and group is not None and dist.get_world_size(group) > 1
         world = dist.get_world_size(group) if group is not None else 1
         rank = dist.get_rank(group) if group is not None else 0
-        self.plan = sca.unit_plan(world, rank, self.num_cams)
-        owners = sca.camera_ranks(world, self.num_cams)
-        self.cam_owner = {c: r[0] for c, r in owners.items()}
-        self.my_backbone_cams = [c for c, o in self.cam_owner.items() if o == rank]
-        self.my_sca_cams = sca.plan_cameras(self.plan)
+        self.process_group, self.shard_size, self.shard_rank = group, world, rank
+        self.row_sharded = bool(row_sharded) and world > 1
+        owner = {c: r[0] for c, r in sca.camera_ranks(world, self.num_cams).items()}
+        self.my_backbone_cams = [c for c, o in owner.items() if o == rank]
+        self.my_sca_cams = sca.plan_cameras(sca.unit_plan(world, rank, self.num_cams))
         self.cam_groups = sca.camera_groups(world, self.num_cams, rank, group) if world > 1 else {}
         # the broadcast of a shared camera's features names its owner by global rank (`group` may be a sub-group)
-        self.cam_src = {c: dist.get_global_rank(group, o) for c, o in self.cam_owner.items()} if world > 1 else {}
+        self.cam_src = {c: dist.get_global_rank(group, o) for c, o in owner.items()} if world > 1 else {}
         for layer in self.encoder:
             layer.cross_attn.set_process_group(group if world > 1 else None)
             if layer.latent_render is not None:
@@ -480,35 +482,18 @@ class SyntheticViDAR(nn.Module):
 
     def backbone_cams(self):
         """The cameras whose images this rank's backbone runs (all of them without a process group)."""
-        import torch.distributed as dist
-        if self.process_group is None or dist.get_world_size(self.process_group) == 1:
-            return list(range(self.num_cams))
         return list(self.my_backbone_cams)
 
     # ---- image features of one frame -> [cams, K, bs, C] (only this rank's SCA cameras are filled) ----
     def extract_feat(self, img, draw=None, cams_only=False):
         """img [bs, cams, 3, H, W] -> (feat_flatten [cams, K, bs, C], spatial_shapes, level_start_index).  `draw`: a
-        GridMask draw (`self.grid_mask.sample`) applied to the images before the backbone.  With the image pipeline,
-        img is (results of the frame's transforms, its uint8 frames [1, cams, H, W, 3]).  `cams_only`: img is a
-        `SampleLoader` frame, float32 [len(backbone_cams()), 3, H, W] of this rank's backbone cameras only (bs 1),
-        which goes to the backbone as it is."""
-        import torch.distributed as dist
-        world = dist.get_world_size(self.process_group) if self.process_group is not None else 1
-        rank = dist.get_rank(self.process_group) if world > 1 else 0
-        mine = self.my_backbone_cams if world > 1 else list(range(self.num_cams))
-        if cams_only:
-            if img.dim() != 4 or img.shape[0] != len(mine):
-                raise ValueError(f"extract_feat: a loaded frame holds this rank's {len(mine)} backbone cameras as "
-                                 f"[{len(mine)}, 3, H, W] (got {tuple(img.shape)})")
-        elif self.image_transforms is not None:
-            results, raw = img
-            pipe = image_aug.apply_multiview(raw[0, mine], results, mine) if mine else None
-            if mine == list(range(self.num_cams)):
-                img = pipe[None]
-            else:                                       # only this rank's cameras are filled (and read)
-                img = raw.new_empty((1, self.num_cams, 3, *results["img_aug"].pad_hw), dtype=torch.float32)
-                if mine:
-                    img[0, mine] = pipe
+        GridMask draw (`self.grid_mask.sample`) applied to the images before the backbone.  `cams_only`: img holds
+        this rank's backbone cameras only, float32 [len(backbone_cams()), 3, H, W] (bs 1; a `SampleLoader` frame or
+        the output of the image pipeline), and goes to the backbone as it is."""
+        mine = self.my_backbone_cams
+        if cams_only and (img.dim() != 4 or img.shape[0] != len(mine)):
+            raise ValueError(f"extract_feat: a frame of this rank's {len(mine)} backbone cameras is "
+                             f"[{len(mine)}, 3, H, W] (got {tuple(img.shape)})")
         bs = 1 if cams_only else img.shape[0]
         per_cam = {}
         if mine:
@@ -541,80 +526,65 @@ class SyntheticViDAR(nn.Module):
                 if f is None:
                     f = img.new_zeros((K, bs, EMBED)).requires_grad_(torch.is_grad_enabled())
                 f = _ShareCameraFeatures.apply(f, self.cam_src[c], self.cam_groups[c])
-            pieces.append(f if (f is not None and (world == 1 or c in self.my_sca_cams)) else feats[c])
+            pieces.append(f if f is not None and c in self.my_sca_cams else feats[c])
         feats = torch.stack(pieces, 0)
         spatial_shapes = torch.tensor(shapes, dtype=torch.int64, device=img.device)
         lsi = torch.cat([spatial_shapes.new_zeros(1), (spatial_shapes[:, 0] * spatial_shapes[:, 1]).cumsum(0)[:-1]])
         return feats, spatial_shapes, lsi
 
+    def _bev_grid(self, bs, device, pillars=False):
+        """The BEV grid's constants, built on every call -> (ref_3d [bs, 4, Q, 3], the encoder's pillar points, or
+        None without `pillars`; ref_2d [bs, Q, 1, 2]; bev_shapes [[bev_h, bev_w]]; bev_lsi [0])."""
+        H, W = self.bev_h, self.bev_w          # noqa: N806
+        ref_3d = (bev_geometry.get_reference_points(H, W, PC_RANGE[5] - PC_RANGE[2], 4, dim="3d", bs=bs, device=device)
+                  if pillars else None)
+        ref_2d = bev_geometry.get_reference_points(H, W, dim="2d", bs=bs, device=device)
+        return ref_3d, ref_2d, torch.tensor([[H, W]], device=device), torch.tensor([0], device=device)
+
     # ---- BEV encoder (transformer.py:102-193 + encoder.py:159-253) ----
     def encode(self, feats, spatial_shapes, lsi, img_metas, can_bus, prev_bev):
-        """One frame's BEV.  With `ego_motion`, `can_bus` is not read: the frame's own comes from img_metas."""
+        """One frame's BEV.  With `ego_motion` (transformer.py:114-157, encoder.py:196-243), `can_bus` is not read:
+        the frame's own comes from img_metas, a scene start drops `prev_bev`, and a previous BEV is aligned -- the
+        first half of TSA's hybrid reference points shifted by the ego translation, TSA's value [rotated previous
+        BEV, initial query], restacked after the LatentRendering layer.  The host values (can_bus, shift) are
+        uploaded pinned, without blocking."""
         bs = feats.shape[2]
         dev = feats.device
-        BEV_H, BEV_W = self.bev_h, self.bev_w          # noqa: N806
+        Q = self.bev_h * self.bev_w
+        shift = None
         if self.ego_motion:
-            return self._encode_ego(feats, spatial_shapes, lsi, img_metas, prev_bev)
+            ego.require_metas(img_metas)
+            if not img_metas[0]["prev_bev_exists"]:                              # bevformer.py:177, vidar.py:280
+                prev_bev = None
+            host = np.concatenate([np.array([m["can_bus"] for m in img_metas], np.float64),
+                                   ego.bev_shift(img_metas, self.bev_h, self.bev_w)], 1)
+            host = ego.upload(host, dev, self.bev_embedding.weight.dtype)        # [bs, 18 + 2]: can_bus, shift x / y
+            can_bus, shift = host[:, :18], host[:, 18:]
         bev_pos = self.positional_encoding(bs)
         query = self.bev_embedding.weight[None].expand(bs, -1, -1) + self.can_bus_mlp(can_bus)[:, None]
-        ref_3d = bev_geometry.get_reference_points(BEV_H, BEV_W, PC_RANGE[5] - PC_RANGE[2], 4, dim="3d", bs=bs, device=dev)
-        ref_2d = bev_geometry.get_reference_points(BEV_H, BEV_W, dim="2d", bs=bs, device=dev)
+        ref_3d, ref_2d, bev_shapes, bev_lsi = self._bev_grid(bs, dev, pillars=True)
         ref_cam, bev_mask = bev_geometry.point_sampling(ref_3d, PC_RANGE, img_metas)
-        Q = BEV_H * BEV_W
-        hybrid = torch.stack([ref_2d, ref_2d], 1).reshape(bs * 2, Q, 1, 2)          # can_bus zeros: no ego shift
-        bev_shapes = torch.tensor([[BEV_H, BEV_W]], device=dev)
-        bev_lsi = torch.tensor([0], device=dev)
-        rows_mode = getattr(self, "row_sharded", False)
-        if rows_mode:
-            import torch.distributed as dist
-            world = dist.get_world_size(self.process_group)
-            if bs != 1 or Q % world != 0:
-                raise RuntimeError(f"row-sharded encoder: needs bs == 1 and BEV rows ({Q}) divisible by the group size ({world})")
+        first, value = ref_2d, None
+        if shift is not None and prev_bev is not None:
+            first = ref_2d + shift[:, None, None, :]
+            rows = ego.rotation_rows([m["can_bus"][-1] for m in img_metas], self.bev_h, self.bev_w, dev)
+            value = ego.rotate_stack(prev_bev, query, rows)                      # [bs * 2, Q, C]
+        hybrid = torch.stack([first, ref_2d], 1).reshape(bs * 2, Q, 1, 2)
+        if self.row_sharded:
+            if bs != 1 or Q % self.shard_size != 0:
+                raise RuntimeError(f"row-sharded encoder: needs bs == 1 and BEV rows ({Q}) divisible by the group size "
+                                   f"({self.shard_size})")
             # replicated tensors consumed by sharded stages: their gradients are per-rank partial sums
             query = sharding.sum_grad(query, self.process_group)
             bev_pos = sharding.sum_grad(bev_pos, self.process_group)
         for i, layer in enumerate(self.encoder):
-            pv = torch.stack([prev_bev if prev_bev is not None else query, query], 1).reshape(bs * 2, Q, EMBED)
-            if rows_mode:
+            pv = value if value is not None else torch.stack(
+                [prev_bev if prev_bev is not None else query, query], 1).reshape(bs * 2, Q, EMBED)
+            if self.row_sharded:
                 query = layer.forward_rows(query, feats, bev_pos, hybrid, pv, spatial_shapes, lsi, ref_cam, bev_mask,
                                            bev_shapes, bev_lsi, self.process_group, last=i == len(self.encoder) - 1)
             else:
                 query = layer(query, feats, bev_pos, hybrid, pv, spatial_shapes, lsi, ref_cam, bev_mask, bev_shapes, bev_lsi)
-        return query
-
-    def _encode_ego(self, feats, spatial_shapes, lsi, img_metas, prev_bev):
-        """`encode` with ego motion (transformer.py:114-157, encoder.py:196-243): the frame's can_bus, the scene cut,
-        the shifted hybrid reference points, and TSA's value [rotated previous BEV, initial query], restacked after
-        the LatentRendering layer.  The host values (can_bus, shift) are uploaded pinned, without blocking."""
-        ego.require_metas(img_metas)
-        bs = feats.shape[2]
-        dev = feats.device
-        BEV_H, BEV_W = self.bev_h, self.bev_w          # noqa: N806
-        Q = BEV_H * BEV_W
-        if not img_metas[0]["prev_bev_exists"]:                                  # bevformer.py:177, vidar.py:280
-            prev_bev = None
-        host = np.concatenate([np.array([m["can_bus"] for m in img_metas], np.float64),
-                               ego.bev_shift(img_metas, BEV_H, BEV_W)], 1)
-        host = ego.upload(host, dev, self.bev_embedding.weight.dtype)            # [bs, 18 + 2]: can_bus, shift x / y
-        can_bus, shift = host[:, :18], host[:, 18:]
-        bev_pos = self.positional_encoding(bs)
-        query = self.bev_embedding.weight[None].expand(bs, -1, -1) + self.can_bus_mlp(can_bus)[:, None]
-        ref_3d = bev_geometry.get_reference_points(BEV_H, BEV_W, PC_RANGE[5] - PC_RANGE[2], 4, dim="3d", bs=bs, device=dev)
-        ref_2d = bev_geometry.get_reference_points(BEV_H, BEV_W, dim="2d", bs=bs, device=dev)
-        ref_cam, bev_mask = bev_geometry.point_sampling(ref_3d, PC_RANGE, img_metas)
-        bev_shapes = torch.tensor([[BEV_H, BEV_W]], device=dev)
-        bev_lsi = torch.tensor([0], device=dev)
-        value = None
-        if prev_bev is not None:
-            shift_ref_2d = ref_2d + shift[:, None, None, :]
-            hybrid = torch.stack([shift_ref_2d, ref_2d], 1).reshape(bs * 2, Q, 1, 2)
-            rows = ego.rotation_rows([m["can_bus"][-1] for m in img_metas], BEV_H, BEV_W, dev)
-            value = ego.rotate_stack(prev_bev, query, rows)                      # [bs * 2, Q, C]
-        else:
-            hybrid = torch.stack([ref_2d, ref_2d], 1).reshape(bs * 2, Q, 1, 2)
-        for layer in self.encoder:
-            pv = value if value is not None else torch.stack([query, query], 1).reshape(bs * 2, Q, EMBED)
-            query = layer(query, feats, bev_pos, hybrid, pv, spatial_shapes, lsi, ref_cam, bev_mask, bev_shapes, bev_lsi)
             if value is not None and layer.latent_render is not None:            # encoder.py:238-243
                 value = torch.stack([value.view(bs, 2, Q, EMBED)[:, 0], query], 1).reshape(bs * 2, Q, EMBED)
         return query
@@ -628,20 +598,15 @@ class SyntheticViDAR(nn.Module):
         if not len(self.decoder):
             raise RuntimeError("decode_future: the model was built with future_frames=0 and has no future decoder")
         bs = prev_bev_input.shape[0]
-        dev = prev_bev_input.device
-        BEV_H, BEV_W = self.bev_h, self.bev_w          # noqa: N806
         bev_pos = self.future_positional_encoding(bs)
         query = self.future_bev_embedding.weight[None] + self.future_can_bus_mlp(future_can_bus)[:, None]
         prev = (prev_bev_input + self.prev_frame_embedding[None, :, None, :]).view(bs, -1, EMBED)
-        ref = bev_geometry.get_reference_points(BEV_H, BEV_W, dim="2d", bs=bs, device=dev)      # identity ego motion
-        bev_shapes = torch.tensor([[BEV_H, BEV_W]], device=dev)
-        bev_lsi = torch.tensor([0], device=dev)
-        rows_mode = getattr(self, "row_sharded", False)
-        if rows_mode and (bs != 1 or query.shape[1] % torch.distributed.get_world_size(self.process_group) != 0):
+        _, ref, bev_shapes, bev_lsi = self._bev_grid(bs, prev_bev_input.device)      # ref: identity ego motion
+        if self.row_sharded and (bs != 1 or query.shape[1] % self.shard_size != 0):
             raise RuntimeError("row-sharded decoder: needs bs == 1 and BEV rows divisible by the group size")
         # -> ([inter, bs, Q, C] for the head, the last layer's output for the next future frame)
-        return run_decoder(self.decoder, query, prev, bev_pos, ref, bev_shapes, bev_lsi, self.process_group if rows_mode else None,
-                           ref_points=ref_points)
+        return run_decoder(self.decoder, query, prev, bev_pos, ref, bev_shapes, bev_lsi,
+                           self.process_group if self.row_sharded else None, ref_points=ref_points)
 
     def forward_head(self, next_bev_feats):
         """vidar_head_v1.py:64-92: [frames, inter, bs, Q, C] -> [frames, inter, pred_frame, bs, Q, heights]."""
@@ -668,6 +633,48 @@ class SyntheticViDAR(nn.Module):
             dict(img=list(img[0, t]), cam2img=[np.array(m, np.float64) for m in cam2img[0]],
                  lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]]) for t in range(img.shape[1])])
 
+    def _frames(self, img, lidar2img, cam2img, lidar2cam, img_metas, pose_metas, future_frames, feature_cache):
+        """A sample's image frames in any of its three forms (see `_next_bev_preds`) -> (frame, cams_only, metas, hw):
+        frame(t) is frame t's `extract_feat` input and `cams_only` its form, metas[t] the frame's img_metas with
+        `pose_metas` merged, hw the padded image size.  The image pipeline's host draws are made here, for every frame
+        in the dataset's order; its device half runs when frame(t) is called, just before that frame's backbone, so
+        that only one frame's float images are held at a time."""
+        loaded = img_metas is not None
+        if feature_cache is not None and (not loaded or any("filename" not in m[0] for m in img_metas)):
+            raise ValueError("_next_bev_preds: feature_cache needs a test-mode SampleLoader sample (img_metas with "
+                             "each frame's filename)")
+        if loaded:
+            if len(img_metas) != len(img):
+                raise ValueError(f"_next_bev_preds: {len(img)} loaded frames, {len(img_metas)} img_metas")
+            frame, metas, hw = img.__getitem__, img_metas, tuple(img[-1].shape[-2:])
+        elif self.image_transforms is not None:
+            results = self.frame_transforms(img, cam2img, lidar2cam)
+            metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"])] for r in results]
+            hw = results[-1]["img_aug"].pad_hw
+            mine = self.my_backbone_cams
+
+            def frame(t):                             # this rank's cameras, as a SampleLoader frame holds them
+                if not mine:
+                    return img.new_empty((0, 3, *results[t]["img_aug"].pad_hw), dtype=torch.float32)
+                return image_aug.apply_multiview(img[0, t, mine], results[t], mine)
+        else:
+            def frame(t):
+                return img[:, t]
+            metas = [[dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)])
+                      for b in range(img.shape[0])]] * img.shape[1]
+            hw = img.shape[-2:]
+        T, bs = len(metas), len(metas[0])
+        if pose_metas is not None:
+            if len(pose_metas) != T or bs != 1:
+                raise ValueError(f"_next_bev_preds: pose_metas needs bs 1 and one dict per image frame ({T} frames, "
+                                 f"bs {bs}, got {len(pose_metas)})")
+            metas = [[dict(m[0], **p)] for m, p in zip(metas, pose_metas)]
+        if self.ego_motion:
+            for m in metas:
+                ego.require_metas(m)
+            ego.require_metas(metas[T - 1], future_frames)
+        return frame, loaded or self.image_transforms is not None, metas, hw
+
     def _next_bev_preds(self, img, lidar2img, can_bus, future_frames, cam2img=None, lidar2cam=None, train=False,
                         drop_prev_index=-1, supervised=None, img_metas=None, feature_cache=None, pose_metas=None):
         """img [bs, T, cams, 3, H, W] -> next_bev_preds [1 + len(supervised), inter, pred_frame, bs, Q, 16]: the
@@ -693,47 +700,22 @@ class SyntheticViDAR(nn.Module):
 
         `pose_metas` (with `ego_motion`, for the tensor path): one dict per image frame, `ego_motion.queue_metas`' (bs
         1), merged into each frame's metas; a `SampleLoader` sample's img_metas carry them already."""
-        loaded = img_metas is not None
-        if feature_cache is not None and (not loaded or any("filename" not in m[0] for m in img_metas)):
-            raise ValueError("_next_bev_preds: feature_cache needs a test-mode SampleLoader sample (img_metas with "
-                             "each frame's filename)")
-        bs, T = (1, len(img)) if loaded else img.shape[:2]
-        dev = img[0].device if loaded else img.device
+        frame, cams_only, metas, hw = self._frames(img, lidar2img, cam2img, lidar2cam, img_metas, pose_metas,
+                                                   future_frames, feature_cache)
+        T, bs = len(metas), len(metas[0])
+        dev = img[0].device
         can_bus = torch.zeros(bs, 18, device=dev) if can_bus is None else can_bus
-        if loaded:
-            if len(img_metas) != T:
-                raise ValueError(f"_next_bev_preds: {T} loaded frames, {len(img_metas)} img_metas")
-            inputs, metas, hw = list(img), img_metas, tuple(img[-1].shape[-2:])
-        elif self.image_transforms is not None:
-            frames = self.frame_transforms(img, cam2img, lidar2cam)
-            inputs = [(r, img[:, t]) for t, r in enumerate(frames)]
-            metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"])] for r in frames]
-            hw = frames[-1]["img_aug"].pad_hw
-        else:
-            inputs = [img[:, t] for t in range(T)]
-            metas = [[dict(lidar2img=np.asarray(lidar2img[b]), img_shape=[(img.shape[-2], img.shape[-1], 3)])
-                      for b in range(bs)]] * T
-            hw = img.shape[-2:]
-        if pose_metas is not None:
-            if len(pose_metas) != T or bs != 1:
-                raise ValueError(f"_next_bev_preds: pose_metas needs bs 1 and one dict per image frame ({T} frames, "
-                                 f"bs {bs}, got {len(pose_metas)})")
-            metas = [[dict(m[0], **p)] for m, p in zip(metas, pose_metas)]
-        if self.ego_motion:
-            for m in metas:
-                ego.require_metas(m)
-            ego.require_metas(metas[T - 1], future_frames)
         backwarded = min(self.backward_history_frames, T - 1) if train else 0
         frozen = T - 1 - backwarded
         fresh = None if feature_cache is None else {}
 
         def features(t, draw=None):
             if fresh is None or draw is not None:
-                return self.extract_feat(inputs[t], draw, cams_only=loaded)
+                return self.extract_feat(frame(t), draw, cams_only=cams_only)
             key = tuple(metas[t][0]["filename"])
             out = feature_cache.get(key)
             if out is None:
-                out = self.extract_feat(inputs[t], cams_only=loaded)
+                out = self.extract_feat(frame(t), cams_only=cams_only)
             fresh[key] = out
             return out
 
@@ -767,18 +749,8 @@ class SyntheticViDAR(nn.Module):
         prev_bev_input = ref_bev.unsqueeze(1)
         future_inputs = [(can_bus, None)] * future_frames
         if self.ego_motion and future_frames:                                        # vidar.py:319-363
-            cur = metas[T - 1]
-            fcb = np.array([[m["future_can_bus"][k][list(ego.CAN_BUS_DIMS)] for m in cur]
-                            for k in range(1, future_frames + 1)], np.float64)       # [F, bs, 4]
-            f2r, r2h = ego.future_matrices(cur, future_frames)                       # [F, bs, 4, 4] each
-            host = ego.upload(np.concatenate([fcb.reshape(-1), f2r.reshape(-1), r2h.reshape(-1)]), dev,
-                              self.bev_embedding.weight.dtype)
-            n4, n16 = fcb.size, f2r.size
-            fcb, f2r, r2h = (host[:n4].view(fcb.shape), host[n4:n4 + n16].view(f2r.shape),
-                             host[n4 + n16:].view(r2h.shape))
-            mats = torch.matmul(f2r, r2h)                                            # fp32 on the device, as vidar.py:215
-            future_inputs = [(fcb[k], ego.future_grids(mats[k], self.bev_h, self.bev_w, PC_RANGE))
-                             for k in range(future_frames)]
+            future_inputs = ego.future_inputs(metas[T - 1], future_frames, self.bev_h, self.bev_w, PC_RANGE, dev,
+                                              self.bev_embedding.weight.dtype)
         for k in range(1, future_frames + 1):
             if supervised is None or k in supervised:
                 pred_feat, last = self.decode_future(prev_bev_input, *future_inputs[k - 1])
@@ -882,10 +854,15 @@ class SyntheticViDAR(nn.Module):
             gt_points = self.gt_points_of(point_infos, False)
         pred_dict = self.predict_future(img, lidar2img, future_frames, can_bus, img_metas=img_metas,
                                         pose_metas=pose_metas)
-        cur = dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.head_history_frames])
         with torch.no_grad():
-            ret = self.ray_head.evaluate(cur, gt_points, 0, self.bev_h, self.bev_w, PC_RANGE)
+            ret = self.ray_head.evaluate(self._current_head_frame(pred_dict), gt_points, 0, self.bev_h, self.bev_w,
+                                         PC_RANGE)
         return [ret]
+
+    def _current_head_frame(self, pred_dict):
+        """`predict_future`'s pred_dict with the current head frame (`head_history_frames`) only, the frame that
+        forward_test and `evaluate` score."""
+        return dict(pred_dict, next_bev_preds=pred_dict["next_bev_preds"][:, :, self.head_history_frames])
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1189,10 +1166,9 @@ def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0,
         for sample in loader:
             pred = model.predict_future(sample["img"], None, future_frames, img_metas=sample["img_metas"],
                                         feature_cache=cache)
-            cur = dict(pred, next_bev_preds=pred["next_bev_preds"][:, :, model.head_history_frames])
-            tables.append(model.ray_head.evaluate_device(cur, sample["gt_points"], 0, model.bev_h, model.bev_w,
-                                                         PC_RANGE))
-            del pred, cur, sample                  # freed before the next sample's device half
+            tables.append(model.ray_head.evaluate_device(model._current_head_frame(pred), sample["gt_points"], 0,
+                                                         model.bev_h, model.bev_w, PC_RANGE))
+            del pred, sample                       # freed before the next sample's device half
     cache.clear()
     table = torch.cat(tables) if tables else torch.zeros((0, eval_metrics.FIELDS), dtype=torch.float64, device=dev)
     return summarize_tables(table, len(samples), frames, grid)
