@@ -671,14 +671,25 @@ int vidar_image_aug_apply(const unsigned char* src, unsigned char* mid, float* o
 int vidar_image_aug_normalize(const unsigned char* src, float* out, int N, int H, int W, const int32_t* photo_i,
                               const float* photo_f, int to_rgb, const float* mean, const double* stdinv,
                               const float* pad_val, int Hp, int Wp, void* stream);
+/* vidar_image_aug_scale: the OpenScene configs' chain in one launch on `stream` with no scratch: the photometric
+ * statements on float32 (unclamped) when photo_i / photo_f are given, the same normalisation, then
+ * RandomScaleImageMultiViewImage's mmcv.imresize by 2/3 (cv2.resize INTER_LINEAR on float32, as cv2 with IPP
+ * computes it: along x within each source row, then between the rows, each a + t * (b - a) with one fused
+ * multiply-add) to out_h x out_w, then padding to [N, 3, Hp, Wp] (pixels at y >= out_h or x >= out_w are
+ * pad_val[c]).  Needs 1 <= N <= 64, 2 * H == 3 * out_h, 2 * W == 3 * out_w, out_h <= Hp <= 8192,
+ * out_w <= Wp <= 8192.  No host sync. */
+int vidar_image_aug_scale(const unsigned char* src, float* out, int N, int H, int W, const int32_t* photo_i,
+                          const float* photo_f, int to_rgb, const float* mean, const double* stdinv,
+                          const float* pad_val, int out_h, int out_w, int Hp, int Wp, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * (xi) The point half of a pre-training sample (datasets/pipelines/loading.py CustomLoadPointsFromMultiSweeps,
  * CustomVoxelBasedPointSampler over mmdet3d 0.17.1's VoxelBasedPointSampler; nuscenes_vidar_dataset_v1.py union2one's
  * point statements) for every frame of a queue, in a fixed number of launches on `stream`.
- *   raw      float32 raw points, rows of 5 (device); seg_i [S, 5] int64 and seg_d [S, 16] double (device): per
- *            segment raw row offset, n, offset in the call's point space, filter (0 none, 1 remove-close, 2 also the
- *            ego box), transform (0 / 1); R row-major, t, ego box (x_lo, y_lo, x_hi, y_hi).  Segments are frame-major
+ *   raw      float32 raw points, rows of `cols` = 5 (nuScenes) or 6 (nuPlan) (device); seg_i [S, 5] int64 and seg_d
+ *            [S, 17] double (device): per segment raw row offset, n, offset in the call's point space, filter (0 none,
+ *            1 remove-close, 2 also the ego box), flags (bit 0 the sweep transform, bit 1 column 4 := time, 6 columns
+ *            only); R row-major, t, ego box (x_lo, y_lo, x_hi, y_hi), time.  Segments are frame-major
  *            and the call's point space is their concatenation (n_g points).
  *   frame_i  [F, 10] int64 (device): merged offset, merged count, output row offset, output rows, queue index,
  *            voxel sampler (0 / 1), grid offset, perm offset, point-space offset, point-space count;
@@ -686,16 +697,17 @@ int vidar_image_aug_normalize(const unsigned char* src, float* out, int N, int H
  *   perm     int32 (device): per voxel frame its shuffled order of the merged points (numpy's draws)
  *   n_cur    merged points over all frames (the host's count), cells = voxel grid cells over all frames
  *   ego      host float[4] (x_lo, y_lo, x_hi, y_hi) of union2one's mask, or NULL for no mask
- *   out      [rows, 5] float32 (device): each frame's kept points (x, y, z, intensity, queue index) in the
- *            reference's order within its rows; masked and unused rows are NaN
+ *   out      [rows, cols] float32 (device): each frame's kept points (x, y, z, intensity, queue index; with 6 columns
+ *            x, y, z, intensity, column 4 -- the segment's time with flag bit 1, else the raw value --, queue index)
+ *            in the reference's order within its rows; masked and unused rows are NaN
  *   counts   optional int32 [F, 2] (device): per frame the merged points and the kept points the device found
- *   out_compact / count: optional float32 [rows, 5] and int64 [1] (device): the non-NaN rows in order and their number
+ *   out_compact / count: optional float32 [rows, cols] and int64 [1] (device): the non-NaN rows in order and their number
  * Needs every n below 2^31.  No host sync. */
 int vidar_point_pipeline_gather(const float* raw, const int64_t* seg_i, const double* seg_d, int S,
                                 const int64_t* frame_i, const float* frame_f, const int64_t* frame_g, int F,
                                 const int32_t* perm, long long n_g, long long n_cur, long long cells, const float* ego,
                                 float* out, long long rows, int32_t* counts, float* out_compact, int64_t* count,
-                                void* stream);
+                                int cols, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * (xii) Baseline JPEG decoding of a queue's camera images (the pre-training loader's cv2.imread(name,

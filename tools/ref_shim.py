@@ -553,6 +553,7 @@ def install_point_pipelines(files=None):
     spec = importlib.util.spec_from_file_location("vidar_ref_pipelines_loading", os.path.join(REF_PIPELINES, "loading.py"))
     loading = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(loading)
+    sys.modules["vidar_ref_pipelines_loading"] = loading
 
     ns = dict(np=np, torch=torch, copy=__import__("copy"), DC=DataContainer, transform_matrix=transform_matrix,
               Quaternion=Quaternion)
@@ -571,4 +572,56 @@ def install_point_pipelines(files=None):
     return dict(LoadPointsFromFile=LoadPointsFromFile,
                 CustomLoadPointsFromMultiSweeps=loading.CustomLoadPointsFromMultiSweeps,
                 CustomVoxelBasedPointSampler=loading.CustomVoxelBasedPointSampler, LiDARPoints=LiDARPoints,
-                DataContainer=DataContainer, union2one=union2one)
+                DataContainer=DataContainer, union2one=union2one, transform_matrix=transform_matrix,
+                Quaternion=Quaternion)
+
+
+def install_nuplan_pipelines():
+    """Load the reference's nuPlan point loaders (datasets/pipelines/nuplan_loading.py: `PointCloud`,
+    `LoadNuPlanPointsFromFile`, `LoadNuPlanPointsFromMultiSweeps` over loading.py's LoadPointsFromMultiSweeps) and
+    NuPlanViDARDatasetV1's `_mask_points` / `union2one`, on the stand-ins of `install_point_pipelines`.
+    -> that dict with these names added."""
+    import numpy as np
+    ref = install_point_pipelines()
+    pkg = types.ModuleType("vidar_ref_nuplan")
+    pkg.__path__ = [REF_PIPELINES]
+    sys.modules["vidar_ref_nuplan"] = pkg
+    sys.modules["vidar_ref_nuplan.loading"] = sys.modules.get("vidar_ref_pipelines_loading") or _load_loading()
+    spec = importlib.util.spec_from_file_location("vidar_ref_nuplan.nuplan_loading",
+                                                  os.path.join(REF_PIPELINES, "nuplan_loading.py"))
+    mod = importlib.util.module_from_spec(spec)
+    sys.modules[spec.name] = mod
+    spec.loader.exec_module(mod)
+    ns = dict(np=np, torch=torch, copy=__import__("copy"), DC=ref["DataContainer"],
+              transform_matrix=ref["transform_matrix"], Quaternion=ref["Quaternion"])
+    meths = _load_methods(os.path.join(REF_DATASETS, "nuplan_vidar_dataset_v1.py"), "NuPlanViDARDatasetV1",
+                          ("_mask_points", "union2one"), ns)
+
+    class _Dataset:
+        _mask_points = meths["_mask_points"]
+        union2one = meths["union2one"]
+
+    def union2one(previous_queue, future_queue, ego_mask):
+        ds = _Dataset()
+        ds.ego_mask, ds.future_length = ego_mask, len(future_queue) - 1
+        return ds.union2one(previous_queue, future_queue)
+
+    return dict(ref, PointCloud=mod.PointCloud, LoadNuPlanPointsFromFile=mod.LoadNuPlanPointsFromFile,
+                LoadNuPlanPointsFromMultiSweeps=mod.LoadNuPlanPointsFromMultiSweeps, nuplan_union2one=union2one)
+
+
+def _load_loading():
+    spec = importlib.util.spec_from_file_location("vidar_ref_nuplan.loading", os.path.join(REF_PIPELINES, "loading.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def install_scale_pipeline():
+    """The reference's RandomScaleImageMultiViewImage (transform_3d.py), with mmcv.imresize restated from mmcv 1.x
+    (mmcv/image/geometric.py): cv2.resize(img, size, interpolation=cv2.INTER_LINEAR), the 'bilinear' default."""
+    import cv2
+    classes = install_pipelines()
+    sys.modules["mmcv"].imresize = lambda img, size, return_scale=False, interpolation="bilinear": cv2.resize(
+        img, size, interpolation={"bilinear": cv2.INTER_LINEAR}[interpolation])
+    return classes["RandomScaleImageMultiViewImage"]

@@ -4,7 +4,9 @@
 //   * PhotoMetricDistortionMultiViewImage -> CropResizeFlipImage (crop, then resize) or RandomCropResizeFlipImage
 //     (resize, then crop) -> NormalizeMultiviewImage -> PadMultiViewImage, in two launches (vidar_image_aug_apply);
 //   * PhotoMetricDistortionMultiViewImage (optional) -> NormalizeMultiviewImage -> PadMultiViewImage, in one launch
-//     on the unclamped float32 photometric output (vidar_image_aug_normalize).
+//     on the unclamped float32 photometric output (vidar_image_aug_normalize);
+//   * the OpenScene configs' PhotoMetricDistortionMultiViewImage (optional) -> NormalizeMultiviewImage ->
+//     RandomScaleImageMultiViewImage(scales=[2/3]) -> PadMultiViewImage, in one launch (vidar_image_aug_scale).
 //
 // Pass 1 (one block per cropped row and image): every source pixel of the row gets the photometric float32 math
 // once -- brightness x + delta, contrast x * alpha (before the HSV round trip in mode 1, after it in mode 0),
@@ -278,6 +280,61 @@ __global__ void __launch_bounds__(kThreads) image_aug_normalize_kernel(const uns
   }
 }
 
+// The OpenScene chain (RandomScaleImageMultiViewImage after the normalisation): the photometric statements (when
+// PHOTO) on float32, the normalisation, then mmcv.imresize -- cv2.resize INTER_LINEAR on float32 HWC -- by 2/3, then
+// the padding, for one output row, written as CHW.  At a 3:2 ratio output pixel d reads source pixels floor(1.5 d)
+// and the next one with weight 0.25 (d even) or 0.75 (d odd), never past the last one.  cv2 with IPP, as the
+// package's wheel ships it, interpolates each of the two source rows along x first and then between them, each
+// step a + t * (b - a) with one fused multiply-add; the source pixels are recomputed for each output pixel that
+// reads them.
+template <bool PHOTO>
+__device__ __forceinline__ void scale_source(const Geom& g, const Photo& p, const unsigned char* px, float v[3]) {
+  float x[3];
+  if (PHOTO) {
+    photometric(p, px, x);
+  } else {
+    x[0] = px[0];
+    x[1] = px[1];
+    x[2] = px[2];
+  }
+  normalize(g, x, v);
+}
+
+template <bool PHOTO>
+__global__ void __launch_bounds__(kThreads) image_aug_scale_kernel(const unsigned char* __restrict__ src,
+                                                                   float* __restrict__ out, const Geom g,
+                                                                   const Photos photos) {
+  const int y = blockIdx.x, n = blockIdx.y;
+  const long long plane = (long long)g.Hp * g.Wp;
+  float* o = out + (long long)n * 3 * plane + (long long)y * g.Wp;
+  const bool row_in = y < g.oh;
+  const int sy = (3 * y) >> 1;
+  const float fy = (y & 1) ? 0.75f : 0.25f;
+  const unsigned char* r0 = src + ((long long)n * g.H + (row_in ? sy : 0)) * g.W * 3;
+  const unsigned char* r1 = r0 + (row_in ? (long long)g.W * 3 : 0);
+  const Photo& p = photos.p[n];
+  for (int x = threadIdx.x; x < g.Wp; x += kThreads) {
+    float v[3] = {g.pad[0], g.pad[1], g.pad[2]};
+    if (row_in && x < g.ow) {
+      const int sx = (3 * x) >> 1;
+      const float fx = (x & 1) ? 0.75f : 0.25f;
+      float a0[3], a1[3], b0[3], b1[3];
+      scale_source<PHOTO>(g, p, r0 + 3 * sx, a0);
+      scale_source<PHOTO>(g, p, r0 + 3 * sx + 3, a1);
+      scale_source<PHOTO>(g, p, r1 + 3 * sx, b0);
+      scale_source<PHOTO>(g, p, r1 + 3 * sx + 3, b1);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float h0 = __fmaf_rn(fx, __fsub_rn(a1[c], a0[c]), a0[c]);
+        const float h1 = __fmaf_rn(fx, __fsub_rn(b1[c], b0[c]), b0[c]);
+        v[c] = __fmaf_rn(fy, __fsub_rn(h1, h0), h0);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c * plane + x] = v[c];
+  }
+}
+
 // photo_i / photo_f (host) -> the kernel-argument copy of the draws, after checking them.
 int read_photos(const char* who, int N, const int32_t* photo_i, const float* photo_f, Photos& photos) {
   for (int n = 0; n < N; ++n) {
@@ -385,5 +442,35 @@ extern "C" int vidar_image_aug_normalize(const unsigned char* src, float* out, i
   const dim3 grid((unsigned)Hp, (unsigned)N);
   if (photo_i) image_aug_normalize_kernel<true><<<grid, kThreads, 0, st>>>(src, out, g, photos);
   else image_aug_normalize_kernel<false><<<grid, kThreads, 0, st>>>(src, out, g, photos);
+  return check_launch(who);
+}
+
+extern "C" int vidar_image_aug_scale(const unsigned char* src, float* out, int N, int H, int W,
+                                     const int32_t* photo_i, const float* photo_f, int to_rgb, const float* mean,
+                                     const double* stdinv, const float* pad_val, int out_h, int out_w, int Hp, int Wp,
+                                     void* stream) {
+  const char* who = "image_aug_scale";
+  VIDAR_REQUIRE(src && out && mean && stdinv && pad_val, "%s: null pointer argument", who);
+  VIDAR_REQUIRE(N >= 1 && N <= kMaxImages, "%s: %d images per call (need 1..%d)", who, N, kMaxImages);
+  VIDAR_REQUIRE(H >= 3 && W >= 3 && H <= kMaxSide && W <= kMaxSide && 2 * H == 3 * out_h && 2 * W == 3 * out_w,
+                "%s: image %d x %d to %d x %d: only a scale of 2/3 on sides divisible by 3 is supported", who, H, W,
+                out_h, out_w);
+  VIDAR_REQUIRE(Hp >= out_h && Wp >= out_w && Hp <= kMaxSide && Wp <= kMaxSide,
+                "%s: padded size %d x %d must hold the %d x %d image and be at most %d", who, Hp, Wp, out_h, out_w,
+                kMaxSide);
+  VIDAR_REQUIRE(to_rgb == 0 || to_rgb == 1, "%s: to_rgb must be 0 or 1", who);
+  VIDAR_REQUIRE((photo_i == nullptr) == (photo_f == nullptr), "%s: photo_i and photo_f go together", who);
+  Photos photos{};
+  if (photo_i) {
+    const int rc = read_photos(who, N, photo_i, photo_f, photos);
+    if (rc != VIDAR_OK) return rc;
+  }
+  Geom g{};
+  g.H = H; g.W = W; g.oh = out_h; g.ow = out_w; g.Hp = Hp; g.Wp = Wp; g.to_rgb = to_rgb;
+  set_norm(g, mean, stdinv, pad_val);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((unsigned)Hp, (unsigned)N);
+  if (photo_i) image_aug_scale_kernel<true><<<grid, kThreads, 0, st>>>(src, out, g, photos);
+  else image_aug_scale_kernel<false><<<grid, kThreads, 0, st>>>(src, out, g, photos);
   return check_launch(who);
 }

@@ -6,10 +6,13 @@
     memory-efficient pre-training (mem_efficient_vidar_1_8_nusc_3future.py:307-314):
         PhotoMetricDistortionMultiViewImage -> RandomCropResizeFlipImage(ida_aug_conf) -> NormalizeMultiviewImage
           -> PadMultiViewImage
-    fine-tuning (vidar_finetune/*, bevformer_base.py) and every test pipeline:
+    fine-tuning (vidar_finetune/*, bevformer_base.py) and every nuScenes test pipeline:
         [PhotoMetricDistortionMultiViewImage ->] NormalizeMultiviewImage -> PadMultiViewImage
+    OpenScene pre-training and test (vidar_OpenScene_*_3future.py:297-312):
+        [PhotoMetricDistortionMultiViewImage ->] NormalizeMultiviewImage -> RandomScaleImageMultiViewImage([2/3])
+          -> PadMultiViewImage
 
-The five classes take the reference's constructor arguments (datasets/pipelines/transform_3d.py:7-185,
+The six classes take the reference's constructor arguments (datasets/pipelines/transform_3d.py:7-185,
 augmentation.py:10-301).  Used as dataloader transforms, their `__call__(results)` does only the host work: the
 same draws from the same generators in the same order (numpy's global generator for the photometric gates and
 factors, the crop offset and the flip, the stdlib `random` for the resize, cached in `results['aug_param']` so
@@ -21,7 +24,8 @@ as loaded (uint8).
 include/vidar_b200.h §x): uint8 [N, H, W, 3] BGR in, float32 [N, 3, Hp, Wp] out, bit for bit what the reference's
 cv2 / PIL / numpy statements give.  With a crop step that is two launches, including numpy's wrapping `np.uint8`
 cast of pixels that brightness and contrast push past 255 or below 0; without one it is one launch, and the
-photometric output reaches the normalisation as unclamped float32, as in the reference.  The per-image draws
+photometric output reaches the normalisation as unclamped float32, as in the reference.  With a rescale step
+(the OpenScene chains) it is one launch too: photometric, normalisation, mmcv.imresize and padding per output pixel.  The per-image draws
 travel in the kernel arguments; the resample taps are computed on the host in float64 by Pillow's rules, cached per
 (input size, output size, device) and uploaded once from pinned memory without blocking.  No host sync.  CUDA
 tensors only.
@@ -67,12 +71,15 @@ class ImageAugPlan:
     pad_hw: tuple = None
     pad_val: tuple = (0.0, 0.0, 0.0)
     window: tuple = None               # (x0, y0, x1, y1) of the resized image, zero outside; None: all of it
+    scale_hw: tuple = None             # (h, w) after RandomScaleImageMultiViewImage, or None
 
     @property
     def hw(self):
         """(h, w) of the images after the steps recorded so far."""
         if self.pad_hw is not None:
             return self.pad_hw
+        if self.scale_hw is not None:
+            return self.scale_hw
         if self.window is not None:
             return self.window[3] - self.window[1], self.window[2] - self.window[0]
         return (self.dims[1], self.dims[0]) if self.dims is not None else tuple(self.src_hw)
@@ -91,13 +98,13 @@ def _plan(results, step):
     elif plan.n != len(imgs):
         raise ValueError(f"image pipeline: {len(imgs)} images, the recorded steps saw {plan.n}")
     done = {"photo": plan.photo is not None, "crop": plan.crop is not None, "norm": plan.normalized,
-            "pad": plan.pad_hw is not None}
-    order = ["photo", "crop", "norm", "pad"]
+            "scale": plan.scale_hw is not None, "pad": plan.pad_hw is not None}
+    order = ["photo", "crop", "norm", "scale", "pad"]
     later = order[order.index(step):]
     if any(done[s] for s in later):
         raise ValueError(f"image pipeline: step '{step}' after {[s for s in order if done[s]]}; the device chain "
-                         "runs photometric distortion, crop / resize / flip, normalisation and padding in this order, "
-                         "each at most once")
+                         "runs photometric distortion, crop / resize / flip, normalisation, rescale and padding in "
+                         "this order, each at most once")
     return plan
 
 
@@ -275,6 +282,37 @@ class NormalizeMultiviewImage:
         return results
 
 
+class RandomScaleImageMultiViewImage:
+    """transform_3d.py:295-327: one scale per call from `scales`, drawn as the reference draws it --
+    `np.random.permutation(range(len(scales)))[0]`, one permutation per call even with one scale --, then every
+    image resized to (int(h * scale), int(w * scale)) with mmcv.imresize (cv2 INTER_LINEAR), `lidar2img` :=
+    diag(scale, scale, 1, 1) @ lidar2img, and `img_shape` / `ori_shape` the resized shapes.  The device step supports
+    the configs' 2/3 on sides divisible by 3 (1920 x 1080 -> 1280 x 720); other sizes are rejected here."""
+
+    def __init__(self, scales=[]):
+        self.scales = scales
+        if len(self.scales) != 1:
+            raise ValueError(f"RandomScaleImageMultiViewImage: exactly one scale, as the reference asserts (got "
+                             f"{scales})")
+
+    def __call__(self, results):
+        plan = _plan(results, "scale")
+        rand_scale = self.scales[np.random.permutation(range(len(self.scales)))[0]]
+        h, w = plan.hw
+        y_size, x_size = int(h * rand_scale), int(w * rand_scale)
+        if plan.crop is not None or 2 * h != 3 * y_size or 2 * w != 3 * x_size:
+            raise ValueError(f"RandomScaleImageMultiViewImage: {h} x {w} by {rand_scale} -> {y_size} x {x_size}: the "
+                             "device chain supports a scale of 2/3 on sides divisible by 3, after no crop step")
+        scale_factor = np.eye(4)
+        scale_factor[0, 0] *= rand_scale
+        scale_factor[1, 1] *= rand_scale
+        results["lidar2img"] = [scale_factor @ l2i for l2i in results["lidar2img"]]
+        results["img_shape"] = [(y_size, x_size, 3)] * plan.n
+        results["ori_shape"] = [(y_size, x_size, 3)] * plan.n
+        plan.scale_hw = (y_size, x_size)
+        return results
+
+
 class PadMultiViewImage:
     """transform_3d.py:7-58 (mmcv.impad / impad_to_multiple): bottom / right padding to `size` or to multiples of
     `size_divisor`.  A number `pad_val` fills channel 0 only and leaves 0 in the others, as cv2.copyMakeBorder does
@@ -368,6 +406,9 @@ def _check(img, plan, cams):
     be tested without a GPU."""
     if not isinstance(plan, ImageAugPlan):
         raise ValueError("apply_multiview: results has no recorded image steps (run the transforms first)")
+    if plan.scale_hw is not None and not plan.normalized:
+        raise ValueError("apply_multiview: RandomScaleImageMultiViewImage without NormalizeMultiviewImage is not "
+                         "supported (the configs rescale the normalised float32 images)")
     if plan.photo is not None and plan.crop is None and not plan.normalized:
         raise ValueError("apply_multiview: photometric distortion without CropResizeFlipImage or "
                          "NormalizeMultiviewImage is not supported (the float32 pixels it makes are the output of "
@@ -423,6 +464,11 @@ def apply_multiview(img, results, cams=None):
 
     with torch.cuda.device(dev):
         out = torch.empty((n, 3, hp, wp), dtype=torch.float32, device=dev)
+        if plan.scale_hw is not None:
+            _lib.check(_lib.lib().vidar_image_aug_scale(
+                _lib.ptr(img), _lib.ptr(out), n, H, W, host(photo_i), host(photo_f), int(plan.to_rgb), host(mean),
+                host(stdinv), host(pad_val), *plan.scale_hw, hp, wp, _lib.stream_ptr(dev)))
+            return out
         if plan.crop is None:
             _lib.check(_lib.lib().vidar_image_aug_normalize(
                 _lib.ptr(img), _lib.ptr(out), n, H, W, host(photo_i), host(photo_f), int(plan.to_rgb), host(mean),
@@ -462,3 +508,18 @@ def config_test_pipeline():
     draw, no crop or resize: `lidar2img` passes through as the dataset gives it, and `img_shape` is the padded shape."""
     return [NormalizeMultiviewImage(**CONFIG_IMG_NORM), PadMultiViewImage(size_divisor=32)]
 
+
+def config_openscene_pipeline():
+    """The image transforms of the OpenScene configs' train_pipeline (vidar_OpenScene_*_3future.py:297-303), after
+    LoadMultiViewImageFromFiles: photometric distortion, normalisation, the rescale by 2/3 and padding to multiples of
+    32 -- 1920 x 1080 cameras become 1280 x 720, padded to 1280 x 736.  No crop: `lidar2img` is the dataset's,
+    scaled."""
+    return [PhotoMetricDistortionMultiViewImage(), NormalizeMultiviewImage(**CONFIG_IMG_NORM),
+            RandomScaleImageMultiViewImage(scales=[2 / 3]), PadMultiViewImage(size_divisor=32)]
+
+
+def config_openscene_test_pipeline():
+    """The image transforms of the OpenScene configs' test_pipeline (vidar_OpenScene_*_3future.py:309-311):
+    normalisation, the rescale by 2/3 (its one permutation draw per frame) and padding to multiples of 32."""
+    return [NormalizeMultiviewImage(**CONFIG_IMG_NORM), RandomScaleImageMultiViewImage(scales=[2 / 3]),
+            PadMultiViewImage(size_divisor=32)]

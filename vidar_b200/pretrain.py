@@ -174,12 +174,12 @@ class LearnedPositionalEncoding(nn.Module):
 class EncoderLayer(nn.Module):
     """BEVFormerLayerV2 (encoder_v2.py:52-209): self_attn, norm, cross_attn, norm, [latent_render], ffn, norm."""
 
-    def __init__(self, latent_render, bev_hw, grid_step=0.5):
+    def __init__(self, latent_render, bev_hw, grid_step=0.5, num_cams=6):
         super().__init__()
         self.bev_hw = bev_hw
         self.self_attn = build_attention(dict(type="TemporalSelfAttention", embed_dims=EMBED, num_levels=1))
         self.cross_attn = build_attention(dict(
-            type="SpatialCrossAttention", pc_range=PC_RANGE, embed_dims=EMBED,
+            type="SpatialCrossAttention", pc_range=PC_RANGE, embed_dims=EMBED, num_cams=num_cams,
             deformable_attention=dict(type="MSDeformableAttention3D", embed_dims=EMBED, num_points=8, num_levels=4)))
         self.norms = nn.ModuleList([nn.LayerNorm(EMBED) for _ in range(3)])
         self.ffn = FFN()
@@ -344,6 +344,14 @@ class SyntheticViDAR(nn.Module):
         drop rate or `supervise_all_future=False` needs it.  Under a process group every rank of a shard group must
         seed numpy alike (as for GridMask) so that they draw the same drop index and future frame.
 
+    `openscene=True` selects the OpenScene configs' pipelines (vidar_OpenScene_*_3future.py:274-312) wherever
+    `image_pipeline` / `point_pipeline` are on: the nuPlan .pcd point loaders with sweeps_num=0 and the voxel sampler
+    at 1 m (`point_pipeline.config_openscene_train_pipeline`; `point_voxel_size` is not read), gt_points of 6 columns,
+    and photometric distortion, normalisation, the rescale by 2/3 and padding on the images
+    (`image_aug.config_openscene_pipeline`): no crop, each frame's `lidar2img` is the dataset's scaled by 2/3 (the
+    in-step pipeline forms it as cam2img @ lidar2cam, as `NuPlanViDARDatasetTemplate.get_data_info` does).  The test
+    chains (`test_image_transforms`, `point_transforms[1]`) are the OpenScene test pipeline's.  It holds no state.
+
     `ego_motion=True` aligns the graph to a moving ego vehicle as the nuScenes configs do (rotate_prev_bev, use_shift,
     use_can_bus; `vidar_b200.ego_motion`).  Each image frame's metas then carry union2one's pose fields
     (`ego_motion.queue_metas`: a `SampleLoader` sample has them, the tensor path takes them as `pose_metas`), and:
@@ -365,8 +373,9 @@ class SyntheticViDAR(nn.Module):
                  grid_mask=False, image_pipeline=False, point_pipeline=False, backward_history_frames=0,
                  drop_prev_rate=0.0, drop_prev_end_idx=None, supervise_all_future=True, head_history_frames=None,
                  head_future_frames=1, per_frame_loss_weight=None, frame_loss_weight=None, latent_grid_step=0.5,
-                 point_voxel_size=1.0, reference_draws=None, ego_motion=False):
+                 point_voxel_size=1.0, reference_draws=None, ego_motion=False, openscene=False):
         super().__init__()
+        self.openscene = bool(openscene)
         self.ego_motion = bool(ego_motion)
         if backward_history_frames not in (0, 1):
             raise ValueError(f"backward_history_frames must be 0 or 1 (got {backward_history_frames})")
@@ -384,9 +393,18 @@ class SyntheticViDAR(nn.Module):
                              "cannot hold them")
         self.head_history_frames = history_frames if head_history_frames is None else head_history_frames
         self.head_future_frames = head_future_frames
-        self.point_transforms = ((point_aug.config_train_pipeline(PC_RANGE, (point_voxel_size,) * 3),
-                                  point_aug.config_test_pipeline()) if point_pipeline else None)
-        self.image_transforms = image_aug.config_pipeline() if image_pipeline else None
+        if not point_pipeline:
+            self.point_transforms = None
+        elif openscene:
+            self.point_transforms = (point_aug.config_openscene_train_pipeline(PC_RANGE),
+                                     point_aug.config_openscene_test_pipeline())
+        else:
+            self.point_transforms = (point_aug.config_train_pipeline(PC_RANGE, (point_voxel_size,) * 3),
+                                     point_aug.config_test_pipeline())
+        self.image_transforms = ((image_aug.config_openscene_pipeline() if openscene else image_aug.config_pipeline())
+                                 if image_pipeline else None)
+        self.test_image_transforms = (image_aug.config_openscene_test_pipeline() if openscene
+                                      else image_aug.config_test_pipeline())
         if backbone_autocast not in (None, torch.float16, torch.bfloat16):
             raise ValueError(f"backbone_autocast must be None, torch.float16 or torch.bfloat16 (got {backbone_autocast})")
         self.backbone_autocast = backbone_autocast
@@ -401,7 +419,7 @@ class SyntheticViDAR(nn.Module):
         self.level_embeds = nn.Parameter(torch.randn(4, EMBED) * 0.02)
         self.can_bus_mlp = nn.Sequential(nn.Linear(18, EMBED // 2), nn.ReLU(inplace=True), nn.Linear(EMBED // 2, EMBED),
                                          nn.ReLU(inplace=True), nn.LayerNorm(EMBED))
-        self.encoder = nn.ModuleList([EncoderLayer(i == latent_layer, bev_hw, latent_grid_step)
+        self.encoder = nn.ModuleList([EncoderLayer(i == latent_layer, bev_hw, latent_grid_step, num_cams)
                                       for i in range(encoder_layers)])
         # future head (ViDARHeadV1); with no future frame the reference deletes the decoder and its embeddings
         self.future_bev_embedding = self.future_positional_encoding = None
@@ -629,9 +647,14 @@ class SyntheticViDAR(nn.Module):
                              f"{img.dtype} {tuple(img.shape)})")
         if cam2img is None or lidar2cam is None:
             raise ValueError("image_pipeline: forward needs cam2img and lidar2cam")
-        return run_image_transforms(self.image_transforms, [
-            dict(img=list(img[0, t]), cam2img=[np.array(m, np.float64) for m in cam2img[0]],
-                 lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]]) for t in range(img.shape[1])])
+        frames = []
+        for t in range(img.shape[1]):
+            f = dict(img=list(img[0, t]), cam2img=[np.array(m, np.float64) for m in cam2img[0]],
+                     lidar2cam=[np.array(m, np.float64) for m in lidar2cam[0]])
+            if self.openscene:                                  # get_data_info's lidar2img: no crop step forms it
+                f["lidar2img"] = [c @ l for c, l in zip(f["cam2img"], f["lidar2cam"])]
+            frames.append(f)
+        return run_image_transforms(self.image_transforms, frames)
 
     def _frames(self, img, lidar2img, cam2img, lidar2cam, img_metas, pose_metas, future_frames, feature_cache):
         """A sample's image frames in any of its three forms (see `_next_bev_preds`) -> (frame, cams_only, metas, hw):
@@ -785,10 +808,10 @@ class SyntheticViDAR(nn.Module):
             raise ValueError("point_pipeline: forward needs point_infos (synthetic_sample(..., raw_points=True))")
         return self.gather_points(run_point_transforms(self.point_transforms[0 if training else 1], point_infos))
 
-    def gather_points(self, point_frames):
-        """The device half of gt_points_of: the transformed GT frames' results -> gt_points [1, R, 5], on the current
-        stream."""
-        return point_aug.gather_gt_points(point_frames, EGO_MASK, self.bev_embedding.weight.device)
+    def gather_points(self, point_frames, ego_mask=EGO_MASK):
+        """The device half of gt_points_of: the transformed GT frames' results -> gt_points [1, R, 5] (6 columns with
+        `openscene`), on the current stream.  `ego_mask`: union2one's ego box."""
+        return point_aug.gather_gt_points(point_frames, ego_mask, self.bev_embedding.weight.device)
 
     # ---- one training forward (vidar.py:239-387) -> dict of losses ----
     def forward_train(self, img, lidar2img, gt_points, can_bus=None, cam2img=None, lidar2cam=None, point_infos=None,
@@ -870,7 +893,7 @@ class SyntheticViDAR(nn.Module):
 # ------------------------------------------------------------------------------------------------
 def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000, future_frames=3, seed=0,
                      bev_hw=(BEV_H, BEV_W), raw_images=False, raw_points=False, points_per_frame=35000, files=False,
-                     poses=False, scene_change=None):
+                     poses=False, scene_change=None, openscene=False):
     """6 x 3 x 928 x 1600 N(0,1) frames, a nuScenes-like rig, LiDAR-like future point clouds (SURVEY.md 8d cfg4).
     `raw_images=True` (for `SyntheticViDAR(image_pipeline=True)`): seeded uniform uint8 BGR frames
     [1, frames, cams, 900, 1600, 3] (img_hw defaults to the camera size) and the rig's host `cam2img` / `lidar2cam`
@@ -886,10 +909,16 @@ def synthetic_sample(device, frames=4, cams=6, img_hw=None, rays_per_frame=10000
     `JPEG_QUALITY` (img_hw defaults to 900 x 1600), to a temporary directory removed at exit.  `device` is not used.
     `poses=True` (for `SyntheticViDAR(ego_motion=True)`): the queue frames follow a seeded drive (`synthetic.drive`,
     `scene_change` = the first frame of a second scene): with `files`, every queue frame carries its pose fields;
-    otherwise the sample holds `pose_metas`, `ego_motion.queue_metas` of the frames + future_frames drive."""
+    otherwise the sample holds `pose_metas`, `ego_motion.queue_metas` of the frames + future_frames drive.
+    `openscene=True` (with `files`, for the OpenScene presets): an OpenScene rig instead -- 8 cameras of 1920 x 1080
+    (`synthetic.nuplan_camera_rig_split`; `cams` and `img_hw` are not read), every image frame also carrying the
+    dataset's `lidar2img` = cam2img @ lidar2cam and a `sample_idx`, and each GT frame a binary .pcd with nuPlan's six
+    fields and sweeps=[], as NuPlanViDARDatasetTemplate.get_data_info hands them on."""
+    if openscene and not files:
+        raise ValueError("synthetic_sample: openscene=True needs files=True")
     if files:
         return synthetic_queue(frames, cams, img_hw or (900, 1600), future_frames, points_per_frame, seed,
-                               poses=poses, scene_change=scene_change)
+                               poses=poses, scene_change=scene_change, openscene=openscene)
     g = torch.Generator(device=device).manual_seed(seed)
     extra = {}
     if raw_images:
@@ -933,15 +962,20 @@ def _temp_dir(prefix):
 
 
 def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=0, first_gt=None, poses=False,
-                    scene_change=None):
+                    scene_change=None, openscene=False):
     """`synthetic_sample(..., files=True)`: image frames 0 .. frames - 1, point frames first_gt (default frames - 1)
     .. frames - 1 + future_frames, every frame with the same rig.  `poses`: frame t also carries the pose fields of
-    drive frame t (`synthetic.drive(..., scene_change)`); the default leaves the queue as without them."""
+    drive frame t (`synthetic.drive(..., scene_change)`); the default leaves the queue as without them.
+    `openscene`: the OpenScene rig of `synthetic_sample`."""
     first_gt = frames - 1 if first_gt is None else first_gt
     import cv2
     root = _temp_dir("vidar_cameras_")
     rng = np.random.default_rng(seed + 1000003)
-    cam2img, lidar2cam = synthetic.camera_rig_split(cams)
+    if openscene:
+        cams, img_hw = 8, synthetic.NUPLAN_IMG_HW
+        cam2img, lidar2cam = synthetic.nuplan_camera_rig_split()
+    else:
+        cam2img, lidar2cam = synthetic.camera_rig_split(cams)
     params = [cv2.IMWRITE_JPEG_QUALITY, JPEG_QUALITY, cv2.IMWRITE_JPEG_PROGRESSIVE, 0,
               cv2.IMWRITE_JPEG_SAMPLING_FACTOR, cv2.IMWRITE_JPEG_SAMPLING_FACTOR_420]
     queue = []
@@ -954,7 +988,10 @@ def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=
             names.append(name)
         queue.append(dict(img_filename=names, cam2img=[m.copy() for m in cam2img],
                           lidar2cam=[m.copy() for m in lidar2cam]))
-    for k, info in enumerate(synthetic_point_infos(frames - first_gt + future_frames, points_per_frame, seed)):
+        if openscene:
+            queue[-1].update(lidar2img=[c @ l for c, l in zip(cam2img, lidar2cam)], sample_idx=f"s{seed}f{t}")
+    for k, info in enumerate(synthetic_point_infos(frames - first_gt + future_frames, points_per_frame, seed,
+                                                   pcd=openscene)):
         if first_gt + k < frames:
             queue[first_gt + k].update(info)
         else:
@@ -966,23 +1003,25 @@ def synthetic_queue(frames, cams, img_hw, future_frames, points_per_frame, seed=
 
 
 def synthetic_scene(num_samples, frames, future_frames, cams=6, img_hw=(900, 1600), points_per_frame=35000, seed=0,
-                    poses=False):
+                    poses=False, openscene=False):
     """One scene's files, written once (`synthetic_queue`), as the sliding-window queues a test dataset builds from
     consecutive keyframes (no load_frame_interval): sample i's image frames are the scene's frames i .. i + frames - 1
     (the history and the current frame), its GT frames i + frames - 1 .. i + frames - 1 + future_frames.  Each image
     frame carries `img_filename`, `cam2img`, `lidar2cam` and the test pipeline's `lidar2img` = cam2img @ lidar2cam
     (float64), so the queues serve the test-mode and the train-mode `SampleLoader` alike.  Neighbouring samples share
     frames - 1 image frames' files.  `poses`: every frame carries its pose fields of one drive over the scene
-    (`synthetic.drive`).  -> [queue] of num_samples queues."""
+    (`synthetic.drive`).  `openscene`: the OpenScene rig of `synthetic_sample`, each image frame with its
+    `sample_idx`.  -> [queue] of num_samples queues."""
     if num_samples < 1 or frames < 1 or future_frames < 0:
         raise ValueError(f"synthetic_scene: num_samples, frames >= 1 and future_frames >= 0 "
                          f"(got {num_samples}, {frames}, {future_frames})")
     total = num_samples + frames - 1
     scene = synthetic_queue(total, cams, img_hw, future_frames, points_per_frame, seed, first_gt=frames - 1,
-                            poses=poses)
+                            poses=poses, openscene=openscene)
     pose = ego.POSE_KEYS if poses else ()
+    tags = ("sample_idx",) if openscene else ()
     images = [dict(img_filename=list(f["img_filename"]), cam2img=f["cam2img"], lidar2cam=f["lidar2cam"],
-                   lidar2img=[c @ l for c, l in zip(f["cam2img"], f["lidar2cam"])], **{k: f[k] for k in pose})
+                   lidar2img=[c @ l for c, l in zip(f["cam2img"], f["lidar2cam"])], **{k: f[k] for k in pose + tags})
               for f in scene[:total]]
     gts = [{k: f[k] for k in ("pts_filename", "timestamp", "sweeps") + pose} for f in scene if "pts_filename" in f]
     queues = []
@@ -993,13 +1032,19 @@ def synthetic_scene(num_samples, frames, future_frames, cams=6, img_hw=(900, 160
     return queues
 
 
-def synthetic_point_infos(frames, n, seed=0, sweeps=2):
-    """Results dicts (pts_filename, timestamp, sweeps) of `frames` LiDAR frames, files in a temporary directory."""
+def synthetic_point_infos(frames, n, seed=0, sweeps=2, pcd=False):
+    """Results dicts (pts_filename, timestamp, sweeps) of `frames` LiDAR frames, files in a temporary directory.
+    `pcd`: nuPlan key frames instead, binary .pcd files of six fields (`synthetic.write_pcd`) with sweeps=[]."""
     root = _temp_dir("vidar_points_")
     rng = np.random.default_rng(seed)
     infos = []
     for f in range(frames):
         ts = 1533151603547590 + 500000 * f
+        if pcd:
+            key = os.path.join(root, f"{f}.pcd")
+            synthetic.write_pcd(key, synthetic.nuplan_cloud(rng, n))
+            infos.append(dict(pts_filename=key, timestamp=ts / 1e6, sweeps=[]))
+            continue
         key = os.path.join(root, f"{f}.bin")
         synthetic.lidar_cloud(rng, n).tofile(key)
         sw = []
@@ -1066,6 +1111,20 @@ _HEAD_5 = dict(head_history_frames=3, head_future_frames=1, per_frame_loss_weigh
 _ONE_FUTURE = dict(history_frames=3, future_frames=0, decoder_layers=1, backward_history_frames=1, drop_prev_rate=0.1,
                    drop_prev_end_idx=3, frame_loss_weight=((1.0,), (0.0,)), point_voxel_size=0.5, reference_draws=True,
                    **_HEAD_5)
+# The four OpenScene (nuPlan) training configs (projects/configs/vidar_pretrain/OpenScene/vidar_OpenScene_{train,mini}_
+# {1_8,full}_3future.py) share one graph; only their dataset split and load_frame_interval (8 for 1_8, 1 for full)
+# differ, and neither is part of the step.  num_cams=8; queue_length 4 = history_frames 3 + the current frame.
+# future_queue_length_train = 3 is the number of future GT frames the dataset appends after the current one (its
+# future_length): frames 0 .. 3, exactly the 1 + future_frames the model predicts and supervises (frame_loss_weight's
+# fifth row belongs to no frame).  The nuScenes 3-future configs set future_queue_length_train = 4 with
+# future_pred_frame_num_train = 3: the dataset appends a fourth future frame that no roll-out predicts, so those
+# presets also take future_frames=3 with 1 + 3 GT frames.  The submit config is test-time only (queue_length 5, six
+# roll-outs, ego_mask (0, 0, 0, 0)): `evaluate(..., future_frames=6, ego_mask=(0, 0, 0, 0), submission_path=...)`.
+_OPENSCENE = dict(num_cams=8, history_frames=3, future_frames=3, decoder_layers=3, head_history_frames=0,
+                  head_future_frames=0, per_frame_loss_weight=(1.0,), frame_loss_weight=((1.0,),) * 4 + ((0.0,),),
+                  supervise_all_future=True, latent_grid_step=0.5, reference_draws=True, openscene=True)
+OPENSCENE_CONFIGS = ("vidar_OpenScene_train_1_8_3future", "vidar_OpenScene_mini_1_8_3future",
+                     "vidar_OpenScene_train_full_3future", "vidar_OpenScene_mini_full_3future")
 CONFIGS = {
     "vidar_1_8_nusc_3future": dict(history_frames=3, future_frames=3, decoder_layers=3,
                                    frame_loss_weight=((1.0,),) * 4 + ((0.0,),), latent_grid_step=0.5,
@@ -1077,6 +1136,7 @@ CONFIGS = {
                                                  head_future_frames=0, per_frame_loss_weight=(1.0,),
                                                  frame_loss_weight=((1.0,),) * 4 + ((0.0,),), latent_grid_step=1.0,
                                                  reference_draws=True),
+    **{name: dict(_OPENSCENE) for name in OPENSCENE_CONFIGS},
 }
 
 
@@ -1127,7 +1187,8 @@ def config_optimizer(model, lr=2e-4):
 # ------------------------------------------------------------------------------------------------
 # evaluation from files (the configs' `evaluation = dict(pipeline=test_pipeline)`, tools/test.py)
 # ------------------------------------------------------------------------------------------------
-def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0, grid=None):
+def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0, grid=None, ego_mask=EGO_MASK,
+             submission_path=None):
     """The dataset's evaluation over `samples` (queues of results dicts in dataset order, e.g. `synthetic_scene`'s):
     the test-mode `SampleLoader`, the prediction of `forward_test` per sample, then `evaluate.summarize` -> the
     summary {f"frame.{t}": {count, chamfer_distance, l1_error, absrel_error}}, equal to
@@ -1148,7 +1209,14 @@ def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0,
         the world, then every rank builds the same summary, and raises the same exception for the first failing
         (sample, frame).
 
-    A queue with fewer than 1 + future_frames GT frames is rejected before any work."""
+    A queue with fewer than 1 + future_frames GT frames is rejected before any work.
+
+    The test chain is the model's (`test_image_transforms` and `point_transforms[1]`: the OpenScene test pipeline for
+    a model built with openscene=True).  `ego_mask`: the dataset's union2one ego box (the submit config's is
+    (0, 0, 0, 0)).  `submission_path` (the submit config's `_submission`, vidar.py:491-519): each sample's predicted
+    points of every future frame t > 0 also go to `<submission_path>/<sample_idx>_<t>.txt`, one '%f' depth (the
+    norm of the predicted point) per line, where `sample_idx` is the current image frame's; the depths of a sample's
+    frames reach the host in one copy.  Every rank of a grid writes its replica's samples when its shard rank is 0."""
     samples = list(samples)
     for i, queue in enumerate(samples):
         gt = sum("pts_filename" in f for f in queue)
@@ -1157,8 +1225,19 @@ def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0,
                              f"{1 + future_frames} (the current frame and every future one)")
     replica, replicas = (grid.replica, grid.replicas) if grid is not None else (0, 1)
     lo, hi = sharding.shard_range(len(samples), replica, replicas)
+    names = None
+    if submission_path is not None:
+        names = []
+        for i, queue in enumerate(samples[lo:hi]):
+            current = [f for f in queue if "img_filename" in f][-1]
+            if "sample_idx" not in current:
+                raise ValueError(f"evaluate: submission_path needs each sample's current image frame's sample_idx "
+                                 f"(sample {lo + i} has none)")
+            names.append(str(current["sample_idx"]))
+        os.makedirs(submission_path, exist_ok=True)
+    write = names is not None and (grid is None or grid.shard_rank == 0)
     loader = SampleLoader(model, samples[lo:hi], num_workers=num_workers, prefetch=prefetch, seed=seed, rank=replica,
-                          test_mode=True)
+                          test_mode=True, ego_mask=ego_mask)
     dev = model.bev_embedding.weight.device
     frames = 1 + future_frames
     tables, cache = [], {}
@@ -1168,10 +1247,30 @@ def evaluate(model, samples, future_frames=6, num_workers=0, prefetch=1, seed=0,
                                         feature_cache=cache)
             tables.append(model.ray_head.evaluate_device(model._current_head_frame(pred), sample["gt_points"], 0,
                                                          model.bev_h, model.bev_w, PC_RANGE))
+            if write:
+                save_predictions(model, pred, sample["gt_points"], submission_path, names[sample["index"]])
             del pred, sample                       # freed before the next sample's device half
     cache.clear()
     table = torch.cat(tables) if tables else torch.zeros((0, eval_metrics.FIELDS), dtype=torch.float64, device=dev)
     return summarize_tables(table, len(samples), frames, grid)
+
+
+def save_predictions(model, pred, gt_points, path, sample_idx):
+    """The reference's `_save_prediction` for one sample (vidar.py:491-519): the head's decoded prediction
+    (`get_point_cloud_prediction` of the current head frame), then per future frame t > 0 the file
+    `<path>/<sample_idx>_<t>.txt` with sqrt(sum(pred_pcd ** 2, 1)) -- one '%f' per line.  The depths of all frames are
+    computed on the device and copied to the host once."""
+    decode = model.ray_head.get_point_cloud_prediction(model._current_head_frame(pred), gt_points, 0, model.bev_h,
+                                                       model.bev_w, PC_RANGE)
+    pcds = decode["pred_pcds"][0][1:]
+    if not pcds:
+        return
+    depth = torch.cat([torch.sqrt((p ** 2).sum(1)) for p in pcds]).cpu().numpy()
+    start = 0
+    for t, p in enumerate(pcds, 1):
+        with open(os.path.join(path, f"{sample_idx}_{t}.txt"), "w") as fh:
+            fh.writelines("%f\n" % d for d in depth[start:start + p.shape[0]])
+        start += p.shape[0]
 
 
 def summarize_tables(table, num_samples, frames, grid=None):

@@ -72,14 +72,17 @@ class QueueDataset(torch.utils.data.Dataset):
     frames, frames with `pts_filename` the GT frames.  -> dict(frames=[image results], points=[point results],
     index=i).  Makes no CUDA call.  `test_mode`: an image frame brings its `lidar2img` (the test chain does not form
     it) instead of `cam2img` and `lidar2cam`.  `poses`: every frame brings its pose fields, and the result also holds
-    poses=[metas per image frame] (`ego_motion.queue_metas`)."""
+    poses=[metas per image frame] (`ego_motion.queue_metas`).  `lidar2img`: whether an image frame brings the
+    dataset's `lidar2img` (default: in test mode), as the OpenScene train chain needs it too -- it has no crop step
+    to form it."""
 
-    def __init__(self, samples, image_transforms, point_transforms, test_mode=False, poses=False):
+    def __init__(self, samples, image_transforms, point_transforms, test_mode=False, poses=False, lidar2img=None):
         self.samples = list(samples)
         self.poses = bool(poses)
         self.image_transforms = list(image_transforms)
         self.point_transforms = list(point_transforms)
         self.test_mode = bool(test_mode)
+        self.lidar2img = self.test_mode if lidar2img is None else bool(lidar2img)
         self.load_images = jpeg.LoadMultiViewImageFromFiles(to_float32=True)
 
     def __len__(self):
@@ -88,12 +91,12 @@ class QueueDataset(torch.utils.data.Dataset):
     def __getitem__(self, index):
         queue = self.samples[index]
         points = run_point_transforms(self.point_transforms, [f for f in queue if "pts_filename" in f])
-        keys = ("lidar2img",) if self.test_mode else ("cam2img", "lidar2cam")
+        keys = ("lidar2img",) if self.lidar2img else ("cam2img", "lidar2cam")
         frames = []
         for f in queue:
             if "img_filename" in f:
-                if self.test_mode and "lidar2img" not in f:
-                    raise ValueError(f"sample {index}: an image frame of the test pipeline needs its lidar2img")
+                if self.lidar2img and "lidar2img" not in f:
+                    raise ValueError(f"sample {index}: an image frame of this pipeline needs its lidar2img")
                 frames.append(self.load_images(dict(img_filename=list(f["img_filename"]),
                                                     **{k: [np.array(m, np.float64) for m in f[k]] for k in keys})))
         if not frames or not points:
@@ -133,10 +136,14 @@ class SampleLoader:
     half runs ahead on a side stream (0: on the current stream, at hand-out).  `seed` and `rank` seed the workers;
     `rank` is the data-parallel replica (`grid.replica`): every rank of a shard group passes the same value and
     iterates the same samples, so their draws agree, and each decodes only its own backbone cameras.
+    A model built with openscene=True runs the OpenScene chains (`model.image_transforms`,
+    `model.test_image_transforms`, the nuPlan point loaders), and its image frames bring their `lidar2img` in both
+    modes.  `ego_mask`: union2one's ego box for gt_points (default the configs' `pretrain.EGO_MASK`; the submit
+    config's is (0, 0, 0, 0)).
     A model built with ego_motion=True needs every queue frame's pose fields (`ego_motion.POSE_KEYS`); the workers
     then run `ego_motion.queue_metas` on the queue and each image frame's img_metas carry its result."""
 
-    def __init__(self, model, samples, num_workers=0, prefetch=1, seed=0, rank=0, test_mode=False):
+    def __init__(self, model, samples, num_workers=0, prefetch=1, seed=0, rank=0, test_mode=False, ego_mask=None):
         if test_mode and model.point_transforms is None:
             raise ValueError("SampleLoader(test_mode=True): the model must be built with point_pipeline=True")
         if not test_mode and (model.image_transforms is None or model.point_transforms is None):
@@ -145,12 +152,14 @@ class SampleLoader:
             raise ValueError(f"SampleLoader: num_workers and prefetch must be >= 0 (got {num_workers}, {prefetch})")
         self.model, self.prefetch, self.num_workers = model, int(prefetch), int(num_workers)
         self.test_mode = bool(test_mode)
+        self.ego_mask = ego_mask
+        lidar2img = True if getattr(model, "openscene", False) else None
         if test_mode:
-            self.dataset = QueueDataset(samples, image_aug.config_test_pipeline(), model.point_transforms[1], True,
-                                        poses=getattr(model, "ego_motion", False))
+            self.dataset = QueueDataset(samples, model.test_image_transforms, model.point_transforms[1], True,
+                                        poses=getattr(model, "ego_motion", False), lidar2img=lidar2img)
         else:
             self.dataset = QueueDataset(samples, model.image_transforms, model.point_transforms[0],
-                                        poses=getattr(model, "ego_motion", False))
+                                        poses=getattr(model, "ego_motion", False), lidar2img=lidar2img)
         init = functools.partial(seed_worker, num_workers=num_workers, rank=rank, seed=seed) if num_workers else None
         self.host_loader = torch.utils.data.DataLoader(self.dataset, batch_size=None, shuffle=False,
                                                        num_workers=num_workers, collate_fn=_one, worker_init_fn=init)
@@ -174,7 +183,8 @@ class SampleLoader:
         metas = [[dict(lidar2img=np.stack(r["lidar2img"]), img_shape=r["img_shape"],
                        **(dict(filename=list(r["filename"])) if self.test_mode else {}), **p)]
                  for r, p in zip(frames, poses)]
-        return dict(img=img, img_metas=metas, gt_points=model.gather_points(host["points"]), lidar2img=None,
+        gt_points = model.gather_points(host["points"], *(() if self.ego_mask is None else (self.ego_mask,)))
+        return dict(img=img, img_metas=metas, gt_points=gt_points, lidar2img=None,
                     index=host["index"])
 
     def __iter__(self):

@@ -107,11 +107,12 @@ def camera_rig(cams=6, img_hw=(900, 1600), f=1266.0, pp=(816.0, 491.0), cam_heig
     return torch.from_numpy(np.stack(mats, 0).astype(np.float32))
 
 
-def camera_rig_split(cams=6, f=1266.0, pp=(816.0, 491.0), cam_height=1.5, seed=0):
+def camera_rig_split(cams=6, f=1266.0, pp=(816.0, 491.0), cam_height=1.5, seed=0, yaws_deg=None):
     """(cam2img, lidar2cam), each [cams, 4, 4] float64, of camera_rig's rig: the intrinsics and the extrinsics that
     the reference's image pipeline keeps apart (CropResizeFlipImage rescales cam2img, then forms
-    lidar2img = cam2img @ lidar2cam).  Their product is camera_rig(cams) before its float32 cast."""
-    yaws = np.deg2rad([0.0, 55.0, -55.0, 110.0, -110.0, 180.0])[:cams]
+    lidar2img = cam2img @ lidar2cam).  Their product is camera_rig(cams) before its float32 cast.  `yaws_deg`: the
+    cameras' yaws (default nuScenes-like six)."""
+    yaws = np.deg2rad([0.0, 55.0, -55.0, 110.0, -110.0, 180.0] if yaws_deg is None else yaws_deg)[:cams]
     rng = np.random.default_rng(seed)
     K = np.array([[f, 0, pp[0], 0], [0, f, pp[1], 0], [0, 0, 1, 0], [0, 0, 0, 1]], np.float64)
     exts = []
@@ -202,3 +203,34 @@ def drive(frames, seed=0, scene_change=None, dt=0.5):
                         lidar2ego_translation=list(LIDAR2EGO_TRANSLATION), lidar2ego_rotation=list(LIDAR2EGO_ROTATION),
                         can_bus=can_bus, scene_token=f"synthetic-{seed}-{scene}"))
     return out
+
+
+NUPLAN_YAWS = (0.0, 45.0, -45.0, 90.0, -90.0, 135.0, -135.0, 180.0)
+NUPLAN_IMG_HW = (1080, 1920)
+
+
+def nuplan_camera_rig_split():
+    """(cam2img, lidar2cam) of an 8-camera 1920 x 1080 rig like OpenScene's."""
+    return camera_rig_split(8, f=1545.0, pp=(960.0, 560.0), yaws_deg=NUPLAN_YAWS)
+
+
+def write_pcd(path, cloud, garbage=16):
+    """Writes float32 [n, 6] (x, y, z, intensity, ring, lidar_info) as a binary .pcd with nuPlan's six fields: the
+    coordinates and intensity float32, ring uint16 and lidar_info uint8 (the values are cast), followed by `garbage`
+    zero bytes, as nuPlan's files carry trailing bytes."""
+    row = np.dtype([("x", np.float32), ("y", np.float32), ("z", np.float32), ("intensity", np.float32),
+                    ("ring", np.uint16), ("lidar_info", np.uint8)])
+    rec = np.zeros(len(cloud), row)
+    for j, name in enumerate(row.names):
+        rec[name] = cloud[:, j]
+    head = ("# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z intensity ring lidar_info\n"
+            "SIZE 4 4 4 4 2 1\nTYPE F F F F U U\nCOUNT 1 1 1 1 1 1\n"
+            f"WIDTH {len(cloud)}\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS {len(cloud)}\nDATA binary\n")
+    with open(path, "wb") as fh:
+        fh.write(head.encode("utf8") + rec.tobytes() + bytes(garbage))
+
+
+def nuplan_cloud(rng, n):
+    """lidar_cloud's points with nuPlan's six columns: the ring as column 4 and a lidar_info id in 0..4."""
+    c = lidar_cloud(rng, n)
+    return np.concatenate([c, rng.integers(0, 5, (n, 1)).astype(np.float32)], 1)
